@@ -1,4 +1,4 @@
-"""The operator table the engines run on: `editanything_b200.ops` (ctypes over libea_b200.so, sm_100a kernels).
+"""The operator table the engines run on: `editanything_b200.ops` (ctypes over libea_b200.so, sm_90a kernels).
 
 There is ONE product backend and no fallback.  `OPS` exists so that the host-side logic (graph of launches, buffer
 plumbing, scheduling, checkpoint loading) can be exercised on machines without a GPU: the CPU test-suite assigns

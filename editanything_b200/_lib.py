@@ -117,7 +117,7 @@ def load():
 
 
 def lib():
-    """Library handle, initialised for compute (requires a B200)."""
+    """Library handle, initialised for compute (requires an H100)."""
     global _inited
     l = load()
     if not _inited:

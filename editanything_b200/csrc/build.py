@@ -1,4 +1,4 @@
-"""Build libea_b200.so (sm_100a only) in-tree with nvcc.  Usage: python -m editanything_b200.csrc.build"""
+"""Build libea_b200.so (sm_90a only) in-tree with nvcc.  Usage: python -m editanything_b200.csrc.build"""
 import os
 import subprocess
 import sys
@@ -7,7 +7,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 PKG = os.path.dirname(HERE)
 LIB = os.path.join(PKG, "lib", "libea_b200.so")
 SOURCES = ["ea_api.cu", "ea_gemm.cu", "ea_attn.cu", "ea_pointwise.cu"]
-HEADERS = ["ea_common.cuh", "ea_internal.h", os.path.join("..", "..", "include", "editanything_b200.h")]
+HEADERS = ["ea_common.cuh", "ea_wgmma.cuh", "ea_internal.h", os.path.join("..", "..", "include", "editanything_b200.h")]
 
 
 def _stale():
@@ -21,7 +21,7 @@ def _stale():
 
 
 def build(force=False, verbose=False, extra=()):
-    """Compile every .cu for sm_100a into editanything_b200/lib/libea_b200.so."""
+    """Compile every .cu for sm_90a into editanything_b200/lib/libea_b200.so."""
     if os.environ.get("EA_NVCC_EXTRA"):
         force = True
     if not force and not _stale():
@@ -32,7 +32,7 @@ def build(force=False, verbose=False, extra=()):
     procs = []
     for src in SOURCES:
         obj = os.path.join(PKG, "lib", src.replace(".cu", ".o"))
-        cmd = [nvcc, "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+        cmd = [nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
                "-Xcompiler", "-fPIC", "--use_fast_math" if False else "-DEA_PRECISE_MATH",
                "-c", os.path.join(HERE, src), "-o", obj] + list(extra) + os.environ.get("EA_NVCC_EXTRA", "").split()
         if verbose:

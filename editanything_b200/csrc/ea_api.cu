@@ -53,7 +53,7 @@ int ea_sm_count() {
   const int d = ea_dev();
   if (!n_sm[d]) {
     int n = 0;
-    n_sm[d] = (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, d) == cudaSuccess && n > 0) ? n : 148;
+    n_sm[d] = (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, d) == cudaSuccess && n > 0) ? n : 132;
   }
   return n_sm[d];
 }

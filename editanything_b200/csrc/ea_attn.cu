@@ -1,31 +1,22 @@
-// ea_attn.cu — fused attention on tcgen05 (sm_100a): O = softmax(Q K^T * scale [+ bias]) V.
+// ea_attn.cu — fused attention on wgmma (sm_90a): O = softmax(Q K^T * scale [+ bias]) V.
 //
 // Replaces the einsum -> softmax -> einsum of CrossAttention.forward
 // (ldm/modules/attention.py:170-193; QK^T accumulated in fp32 like the reference's
 // _ATTN_PRECISION="fp32" path) and SAM's windowed / global attention with decomposed relative
 // position bias (SURVEY.md App. C).  The N x N logits never touch HBM.
 //
-// One CTA = one (batch, head) and NQT query tiles of 128 rows (NQT = 2: two tiles ping-pong so
-// the tensor core works on one tile's MMAs while the other tile is in softmax; NQT = 1: one
-// tile with a double-buffered logits accumulator).  Warp roles (128*NQT + 64 threads, 1 CTA/SM);
-// the two control warps get the HIGHEST warp ids because the SM's warp arbiter prefers them:
-//   warps 0 .. 4*NQT-1   softmax warpgroups, thread <-> query row: one tcgen05.ld round trip brings
-//              the whole 128-column logits row into registers; row max, exp2 with the folded scale
-//              (+ the SAM rel-pos bias in the BIAS kernels), P packed to 16-bit and written back over
-//              the logits' own TMEM columns (tcgen05.st); O is rescaled in TMEM only when the
-//              running max moves by more than 2^8 (exact: the final 1/l uses the same max).
-//              Final 1/l normalisation and 16-byte stores.
-//   warp 4*NQT     TMA producer: Q tiles once, then K/V tiles into a `stages`-deep ring.
-//              Head dims that are not a multiple of 64 (40, 80, 160) are zero-padded for free by
-//              TMA out-of-bounds fill (tensor-map inner extent d, box 64 wide).
-//   warp 4*NQT+1   TMEM allocator + MMA issuer, warp-uniform control flow with one elected lane
-//              (a single-lane branch makes the compiler wrap every MMA in an ELECT/R2UR waterfall):
-//              S = Q K^T (M=128, N=keys, K=d) into TMEM; O += P V (M=128, N=d, K=keys) with P read
-//              straight from TMEM (tcgen05.mma A operand in tensor memory) and V consumed as an
-//              MN-major B operand from its row-major tile.
-// TMEM map (512 columns): NQT=2: S_A 0, S_B 128, O_A 256, O_B 384;  NQT=1: S[0] 0, S[1] 128, O 256.
-// ea_attn_db_kernel (d <= 64, no bias, >= 384 keys): 96-key tiles, so BOTH query tiles have two
-// logits buffers: S[t][buf] at (2t+buf)*96, O[t] at 384 + 64t; 4-stage K/V ring.
+// One CTA = one (batch, head) and a tile of 128 query rows; two warp-groups, warp-group g owns query rows
+// 64g .. 64g+63.  Per 128-key tile:
+//              S = Q K^T with wgmma (A = Q, B = K, both K-major from shared memory) into 64 fp32 registers per
+//              thread; scale (+ the SAM rel-pos bias in the BIAS kernels), mask of missing keys, online softmax
+//              with the running max / sum per row (a row's 128 logits sit on the 4 lanes of a quad); P packed to
+//              16 bit straight from the accumulator layout into the A-operand fragments of the second wgmma,
+//              O += P V (B = V, MN-major from its row-major tile) into DO / 2 registers per thread.  Final 1 / l
+//              normalisation and stores.
+// Thread 0 also drives TMA: the Q tile once, then K/V tiles into a `stages`-deep ring, refilling a stage with the
+// tile `stages` ahead as soon as every warp has released it (a separate producer warp would put three warps on one
+// SM sub-partition and cap every thread at 168 registers: the 192-wide P V accumulator alone is 96).  Head dims that are not a multiple of 64 (40, 80, 160) are zero-padded for free by TMA
+// out-of-bounds fill (tensor-map inner extent d, box 64 wide).
 #include <stdlib.h>
 #include "ea_common.cuh"
 #include "ea_internal.h"
@@ -36,16 +27,14 @@ static constexpr int AT_BQ = 128;
 static constexpr int AT_BKV = 128;
 static constexpr int AT_ATOM = 128 * 128;  // bytes of one 128-row x 64-half swizzled atom
 static constexpr int AT_MAX_STAGES = 4;
+static constexpr int AT_THREADS = 256;   // no separate producer warp: 8 warps may use up to 255 registers a thread
+static constexpr int AT_WARPS = 8;
 
 struct AttnKParams {
   int Nq, Nkv, d, heads;
   int nd;      // ceil(d / 64) atoms along the head dim
   int ksteps;  // ceil(d / 16) MMA K-steps for Q K^T
-  int dpad16;  // d rounded up to 16: MMA N of the PV product
   int stages;
-  int p_smem;  // 1: stage P through shared memory (SS MMA) instead of TMEM (testing fallback)
-  int bias_bytes;  // shared memory for the rel_w rows of the CTA's queries (BIAS kernels), 16-byte multiple
-  int dbg_skip;  // experiment builds: bit0 = skip the PV MMAs, bit1 = skip the S MMAs, bit2 = V K-major view
   float scale_log2;
   ea_half* out;
   long long o_bs, o_ns;
@@ -54,707 +43,217 @@ struct AttnKParams {
   int rel_s;
 };
 
-#ifdef EA_ATTN_TIMING
-// Experiment build only (-DEA_ATTN_TIMING): per-phase clock64 stamps of CTA (0,0,0), softmax warps
-// 4 and 8 (lane 0), KV tiles 8..15; read back with ea_attn_debug_read().
-__device__ long long ea_attn_dbg[2 * 8 * 8];
-__device__ long long ea_attn_dbg_mma[2 * 8 * 4];   // per (tile, kv 8..15): p_ready seen, PV issued, S issued
-#define EA_T(slot)                                                                          \
-  do {                                                                                      \
-    if (dbg_on && j >= 8 && j < 16) ea_attn_dbg[(t * 8 + (j - 8)) * 8 + (slot)] = clock64(); \
-  } while (0)
-#else
-#define EA_T(slot) do {} while (0)
-#endif
-
 __device__ __forceinline__ float ex2_approx(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
 
-// exp2 on the FMA / ALU pipes (Cody-Waite split + degree-3 minimax polynomial on [-0.5, 0.5], max relative error
-// 1.14e-4 - below the 4.9e-4 rounding of the 16-bit P it feeds).  The long self-attention layers are bound by the
-// exp unit (16 MUFU lanes per SM: XU pipe 65 % busy, tensor pipe 21 %, profiles/r02c_misc_ncu_full.txt) while the FMA
-// pipe idles; computing every fourth probability here takes a quarter of the load off the MUFU.  x <= 0; masked keys
-// (x = -inf) clamp to 2^-126 ~ 0.  -DEA_ATTN_EXP_MUFU_ONLY switches it off (A/B).
-__device__ __forceinline__ float ex2_poly(float x) {
-  x = fmaxf(x, -126.f);
-  const float xf = x + 12582912.f;               // 1.5 * 2^23: the integer part lands in the low mantissa bits
-  const float r = x - (xf - 12582912.f);         // fractional part in [-0.5, 0.5]
-  float p = fmaf(0.05459282547f, r, 0.24221783876f);
-  p = fmaf(p, r, 0.69336861372f);
-  p = fmaf(p, r, 1.0f);
-  return __int_as_float(__float_as_int(p) + (__float_as_int(xf) << 23));
+template <int R>
+__device__ __forceinline__ void wgmma_fence_regs_u32(uint32_t (&a)[R][4]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i)
+#pragma unroll
+    for (int k = 0; k < 4; ++k) asm volatile("" : "+r"(a[i][k])::"memory");
 }
 
-__device__ __forceinline__ void tmem_st16_half(uint32_t taddr, const uint32_t (&r)[16]) {
-  tmem_st16(taddr, r);
-}
-
-template <int NQT, bool BIAS>
-__global__ void __launch_bounds__(128 * NQT + 64, 1)
+// DO: width of the P V accumulator (64 / 128 / 192, >= d; the columns past d are TMA zero fill)
+template <int DO, bool BIAS>
+__global__ void __launch_bounds__(AT_THREADS, 1)
 ea_attn_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                const __grid_constant__ CUtensorMap tmV, const AttnKParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                              ~uintptr_t(1023));
-  // layout: Q[NQT][nd] | KV[stages][K nd | V nd] | P[NQT][2] (only if p_smem) | barriers
+  // layout: Q[nd] | KV[stages][K nd | V nd] | rel_w rows (BIAS) | barriers
   uint8_t* sQ = smem;
-  uint8_t* sKV = sQ + NQT * p.nd * AT_ATOM;
+  uint8_t* sKV = sQ + p.nd * AT_ATOM;
   const int kv_stage_bytes = 2 * p.nd * AT_ATOM;
-  uint8_t* sP = sKV + p.stages * kv_stage_bytes;
-  float* rw_s = reinterpret_cast<float*>(sP + (p.p_smem ? NQT * 2 * AT_ATOM : 0));   // [NQT*128][rel_s+1]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(rw_s) + p.bias_bytes);
+  float* rw_s = reinterpret_cast<float*>(sKV + p.stages * kv_stage_bytes);   // [128][rel_s + 1]
+  const int bias_floats = BIAS ? ((AT_BQ * (p.rel_s + 1) + 3) & ~3) : 0;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(rw_s + bias_floats);
   uint64_t* q_full = bars;                      // [1]
   uint64_t* kv_full = bars + 1;                 // [AT_MAX_STAGES]
   uint64_t* kv_empty = kv_full + AT_MAX_STAGES; // [AT_MAX_STAGES]
-  uint64_t* s_full = kv_empty + AT_MAX_STAGES;  // [2]  NQT=2: per tile; NQT=1: per S buffer
-  uint64_t* p_ready = s_full + 2;               // [2]  per tile
-  uint64_t* pv_done = p_ready + 2;              // [2]  per tile
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(pv_done + 2);
 
   pdl_launch_dependents();
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const int qb = blockIdx.x, head = blockIdx.y, b = blockIdx.z;
   const int n_tiles = (p.Nkv + AT_BKV - 1) / AT_BKV;
+  const bool producer = threadIdx.x == 0;
 
-  // Warp roles: softmax warpgroups FIRST (warps 0..4*NQT-1; warp % 4 = TMEM lane quarter), then the
-  // TMA and MMA warps.  The SM's warp arbiter prefers the highest warp id among eligible warps, and
-  // the single MMA-issuing thread must never queue behind the eight busy softmax warps.
-  constexpr int W_TMA = 4 * NQT, W_MMA = 4 * NQT + 1;
-  if (warp == W_TMA && lane == 0) {
+  if (producer) {
     tma_prefetch_desc(&tmQ);
     tma_prefetch_desc(&tmK);
     tma_prefetch_desc(&tmV);
     mbar_init(q_full, 1);
     for (int s = 0; s < AT_MAX_STAGES; ++s) {
       mbar_init(&kv_full[s], 1);
-      mbar_init(&kv_empty[s], 1);
-    }
-    for (int t = 0; t < 2; ++t) {
-      mbar_init(&s_full[t], 1);
-      mbar_init(&p_ready[t], 128);
-      mbar_init(&pv_done[t], 1);
+      mbar_init(&kv_empty[s], AT_WARPS);
     }
     fence_mbar_init();
   }
-  if (warp == W_MMA) tmem_alloc(tmem_slot, 512u);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  pdl_wait();  // everything above overlapped the previous kernel's tail
-
-  if (warp == W_TMA) {
-    // ============================ TMA producer ============================
-    if (lane == 0) {
-      mbar_expect_tx(q_full, (uint32_t)(NQT * p.nd * AT_ATOM));
-      for (int t = 0; t < NQT; ++t)
-        for (int a = 0; a < p.nd; ++a)
-          tma_load_4d(sQ + (t * p.nd + a) * AT_ATOM, &tmQ, q_full, a * 64, head,
-                      (qb * NQT + t) * AT_BQ, b);
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int j = 0; j < n_tiles; ++j) {
-        mbar_wait(&kv_empty[stage], phase ^ 1u);
-        uint8_t* sK = sKV + stage * kv_stage_bytes;
-        uint8_t* sV = sK + p.nd * AT_ATOM;
-        mbar_expect_tx(&kv_full[stage], (uint32_t)kv_stage_bytes);
-        for (int a = 0; a < p.nd; ++a) {
-          tma_load_4d(sK + a * AT_ATOM, &tmK, &kv_full[stage], a * 64, head, j * AT_BKV, b);
-          tma_load_4d(sV + a * AT_ATOM, &tmV, &kv_full[stage], a * 64, head, j * AT_BKV, b);
-        }
-        if (++stage == p.stages) { stage = 0; phase ^= 1u; }
-      }
-    }
-  } else if (warp == W_MMA) {
-    // ============================= MMA issuer =============================
-    // The whole warp runs the schedule in warp-uniform control flow and ONE elected lane issues
-    // (EA_ISSUE): descriptors and TMEM addresses then live in uniform registers.  As a single-lane
-    // branch every UTCHMMA was wrapped in an ELECT/R2UR waterfall and the 11 MMAs of a tile cost
-    // ~1100 clk to issue (tools/exp_attn_timing.py) - three times their execution time.
-#define EA_ISSUE(...) do { if (elect_one()) { __VA_ARGS__; } __syncwarp(); } while (0)
-    {
-      const uint32_t tb = __shfl_sync(0xffffffffu, tmem_base, 0);
-      // Issue loops are kept to a few scalar instructions per MMA (descriptor = base + small add):
-      // a single thread retires about one dependent instruction per 4-5 cycles, and at d = 40 an
-      // MMA itself only takes 24-64 cycles (measured: tools/exp/mma_rate2.cu).
-      const uint32_t idesc_s = umma_idesc(128, 128, 0, 0);
-      const uint32_t idesc_o = umma_idesc(128, (uint32_t)p.dpad16, 0, 1);  // B (=V) MN-major
-      const uint64_t dQ0 = umma_desc_k_sw128(smem_u32(sQ), 1024);
-      const uint64_t dK0 = umma_desc_k_sw128(smem_u32(sKV), 1024);
-      const uint64_t dV0 = umma_desc_mn_sw128(smem_u32(sKV) + (uint32_t)(p.nd * AT_ATOM), AT_ATOM, 1024);
-      const uint64_t dP0 = umma_desc_k_sw128(smem_u32(sP), 1024);
-      const uint32_t q_tile16 = (uint32_t)(p.nd * AT_ATOM) >> 4;
-      const uint32_t kv_stage16 = (uint32_t)kv_stage_bytes >> 4;
-      const int ksteps = p.ksteps;
-      const bool p_smem = p.p_smem != 0;
-      // S_t(j) = Q_t K_j^T into TMEM columns s_col.  K-step ks sits at atom (ks >> 2), +32 B * (ks & 3)
-      auto issue_S = [&](int t, int stage, uint32_t s_col) {
-        uint64_t dq = dQ0 + (uint64_t)(t * q_tile16);
-        uint64_t dk = dK0 + (uint64_t)(stage * kv_stage16);
-        const uint32_t d = tb + s_col;
-        umma_f16_ss(d, dq, dk, idesc_s, 0u);
-        for (int ks = 1; ks < ksteps; ++ks) {
-          const uint32_t step = (ks & 3) ? 2u : (uint32_t)((AT_ATOM >> 4) - 6);
-          dq += step;
-          dk += step;
-          umma_f16_ss(d, dq, dk, idesc_s, 1u);
-        }
-      };
-      // O_t += P_t(j) V_j ; P lives in TMEM columns p_col (16-bit pairs) or in smem tile t
-      auto issue_PV = [&](int t, int stage, uint32_t p_col, uint32_t o_col, bool first) {
-        uint64_t dv = dV0 + (uint64_t)(stage * kv_stage16);
-        const uint32_t d = tb + o_col;
-        uint32_t acc = first ? 0u : 1u;
-        if (p_smem) {
-          uint64_t dp = dP0 + (uint64_t)(t * (2 * AT_ATOM >> 4));
-#pragma unroll
-          for (int ks = 0; ks < AT_BKV / 16; ++ks) {
-            umma_f16_ss(d, dp, dv, idesc_o, acc);
-            acc = 1u;
-            dp += (ks & 3) == 3 ? (uint64_t)((AT_ATOM >> 4) - 6) : 2u;
-            dv += (16 * 128) >> 4;
-          }
-        } else {
-          uint32_t pa = tb + p_col;
-#pragma unroll
-          for (int ks = 0; ks < AT_BKV / 16; ++ks) {
-            umma_f16_ts(d, pa, dv, idesc_o, acc);
-            acc = 1u;
-            pa += 8u;
-            dv += (16 * 128) >> 4;
-          }
-        }
-      };
-      mbar_wait(q_full, 0);
-      if (NQT == 2) {
-        // stage/phase of K/V tile j
-        mbar_wait(&kv_full[0], 0);
-        tc_fence_after();
-        EA_ISSUE(issue_S(0, 0, 0); umma_commit(&s_full[0]); issue_S(1, 0, 128); umma_commit(&s_full[1]));
-        int stage = 0;
-        uint32_t phase = 0;
-        for (int j = 0; j < n_tiles; ++j) {
-          int nstage = stage + 1;
-          uint32_t nphase = phase;
-          if (nstage == p.stages) { nstage = 0; nphase ^= 1u; }
-          const bool more = j + 1 < n_tiles;
-          for (int t = 0; t < 2; ++t) {
-            mbar_wait(&p_ready[t], (uint32_t)(j & 1));
-            tc_fence_after();
-#ifdef EA_ATTN_TIMING
-            const bool md = blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0 && j >= 8 && j < 16 && lane == 0;
-            if (md) ea_attn_dbg_mma[(t * 8 + j - 8) * 4 + 0] = clock64();
-#endif
-            // S_t(j+1) below is queued behind PV_t(j), so "S ready" already implies "PV retired":
-            // pv_done is only needed once, for the epilogue
-            EA_ISSUE(issue_PV(t, stage, (uint32_t)(t * 128), (uint32_t)(256 + t * 128), j == 0);
-                     if (!more) umma_commit(&pv_done[t]);
-                     if (t == 1) umma_commit(&kv_empty[stage]));
-#ifdef EA_ATTN_TIMING
-            if (md) ea_attn_dbg_mma[(t * 8 + j - 8) * 4 + 1] = clock64();
-#endif
-            if (more) {
-              if (t == 0) {
-                mbar_wait(&kv_full[nstage], nphase);
-                tc_fence_after();
-              }
-              EA_ISSUE(issue_S(t, nstage, (uint32_t)(t * 128)); umma_commit(&s_full[t]));
-            }
-#ifdef EA_ATTN_TIMING
-            if (md) ea_attn_dbg_mma[(t * 8 + j - 8) * 4 + 2] = clock64();
-#endif
-          }
-          stage = nstage;
-          phase = nphase;
-        }
-      } else {
-        mbar_wait(&kv_full[0], 0);
-        tc_fence_after();
-        EA_ISSUE(issue_S(0, 0, 0); umma_commit(&s_full[0]));
-        int stage = 0;
-        uint32_t phase = 0;
-        for (int j = 0; j < n_tiles; ++j) {
-          int nstage = stage + 1;
-          uint32_t nphase = phase;
-          if (nstage == p.stages) { nstage = 0; nphase ^= 1u; }
-          const bool more = j + 1 < n_tiles;
-          const uint32_t nbuf = (uint32_t)((j + 1) & 1) * 128u;
-          if (more && p.stages > 1) {  // next logits tile while this one is in softmax
-            mbar_wait(&kv_full[nstage], nphase);
-            tc_fence_after();
-            EA_ISSUE(issue_S(0, nstage, nbuf); umma_commit(&s_full[(j + 1) & 1]));
-          }
-          mbar_wait(&p_ready[0], (uint32_t)(j & 1));
-          tc_fence_after();
-          EA_ISSUE(issue_PV(0, stage, (uint32_t)(j & 1) * 128u, 256u, j == 0); umma_commit(&pv_done[0]);
-                   umma_commit(&kv_empty[stage]));
-          if (more && p.stages == 1) {
-            mbar_wait(&kv_full[nstage], nphase);
-            tc_fence_after();
-            EA_ISSUE(issue_S(0, nstage, nbuf); umma_commit(&s_full[(j + 1) & 1]));
-          }
-          stage = nstage;
-          phase = nphase;
-        }
-      }
-    }
-  } else {
-    // ======================= softmax / correction / epilogue ==============
-    const int t = warp >> 2;        // query tile of this warpgroup
-    const int wq = warp & 3;        // TMEM lane quarter accessible to this warp
-    const int r = wq * 32 + lane;
-    const int q = (qb * NQT + t) * AT_BQ + r;
-    const bool row_ok = q < p.Nq;
-    const uint32_t lane_off = (uint32_t)(wq * 32) << 16;
-    const uint32_t tmem_O = tmem_base + lane_off + (NQT == 2 ? (uint32_t)(256 + t * 128) : 256u);
-    const float LOG2E = 1.4426950408889634f;
-    const float* rh = nullptr;
-    if (BIAS) {
-      const long long bh = (long long)b * p.heads + head;
-      rh = p.rel_h + (bh * p.Nq + (row_ok ? q : 0)) * p.rel_s;
-      const float* rw = p.rel_w + (bh * p.Nq + (row_ok ? q : 0)) * p.rel_s;
-      float* dst = rw_s + (t * AT_BQ + r) * (p.rel_s + 1);
-      for (int i = 0; i < p.rel_s; ++i) dst[i] = row_ok ? __ldg(rw + i) * LOG2E : 0.f;   // own row only
-    }
-    float m_run = -INFINITY;  // running max in the scaled log2 domain
-    float l = 0.f;
-#ifdef EA_ATTN_TIMING
-    const bool dbg_on = blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0 && (warp & 3) == 0 && lane == 0;
-#endif
-    for (int j = 0; j < n_tiles; ++j) {
-      const int sb = (NQT == 2) ? t : (j & 1);
-      const uint32_t sph = (NQT == 2) ? (uint32_t)(j & 1) : (uint32_t)((j >> 1) & 1);
-      EA_T(0);
-      mbar_wait(&s_full[sb], sph);
-      tc_fence_after();
-      EA_T(1);
-      const uint32_t tmem_S = tmem_base + lane_off + (uint32_t)sb * 128u;
-      const int valid = min(AT_BKV, p.Nkv - j * AT_BKV);  // keys of this tile that exist (>= 1)
-      {
-        // ---- whole 128-column logits row in registers: ONE TMEM round trip per tile
-        uint32_t v[4][32];
-        tmem_ld32(tmem_S, v[0]);
-        tmem_ld32(tmem_S + 32u, v[1]);
-        tmem_ld32(tmem_S + 64u, v[2]);
-        tmem_ld32(tmem_S + 96u, v[3]);
-        tmem_ld_wait();
-        EA_T(2);
-        if (BIAS) {
-          // t = s*scale*log2e + (rel_h[q, kh] + rel_w[q, kw])*log2e, written back over v.  rel_w's row
-          // (pre-multiplied by log2e) sits in shared memory, rel_h comes through L1 (2 values/tile
-          // for the 64x64 global grid).
-          const float* rwr = rw_s + (t * AT_BQ + r) * (p.rel_s + 1);
-          const int kk0 = j * AT_BKV;
-          int kh = kk0 / p.rel_s, kw = kk0 - kh * p.rel_s;
-          if ((p.rel_s & 31) == 0) {      // a 32-column chunk never crosses a key row: no branches
-#pragma unroll
-            for (int h = 0; h < 4; ++h) {
-              const float bh_ = __ldg(rh + min(kh, p.rel_s - 1)) * LOG2E;
-#pragma unroll
-              for (int i = 0; i < 32; ++i)
-                v[h][i] = __float_as_uint(fmaf(__uint_as_float(v[h][i]), p.scale_log2, rwr[kw + i] + bh_));
-              kw += 32;
-              if (kw == p.rel_s) { kw = 0; ++kh; }
-            }
-          } else {
-            float bh_ = __ldg(rh + min(kh, p.rel_s - 1)) * LOG2E;
-#pragma unroll
-            for (int h = 0; h < 4; ++h) {
-#pragma unroll
-              for (int i = 0; i < 32; ++i) {
-                v[h][i] = __float_as_uint(fmaf(__uint_as_float(v[h][i]), p.scale_log2, rwr[kw] + bh_));
-                if (++kw == p.rel_s) { kw = 0; ++kh; bh_ = __ldg(rh + min(kh, p.rel_s - 1)) * LOG2E; }
-              }
-            }
-          }
-        }
-        if (valid < AT_BKV) {  // last, partial K/V tile: keys that do not exist get -inf
-#pragma unroll
-          for (int h = 0; h < 4; ++h)
-#pragma unroll
-            for (int i = 0; i < 32; ++i)
-              if (h * 32 + i >= valid) v[h][i] = 0xff800000u;
-        }
-        float mx0 = -INFINITY, mx1 = -INFINITY, mx2 = -INFINITY, mx3 = -INFINITY;
-#pragma unroll
-        for (int i = 0; i < 32; ++i) {
-          mx0 = fmaxf(mx0, __uint_as_float(v[0][i]));
-          mx1 = fmaxf(mx1, __uint_as_float(v[1][i]));
-          mx2 = fmaxf(mx2, __uint_as_float(v[2][i]));
-          mx3 = fmaxf(mx3, __uint_as_float(v[3][i]));
-        }
-        const float m_tile = fmaxf(fmaxf(mx0, mx1), fmaxf(mx2, mx3)) * (BIAS ? 1.f : p.scale_log2);  // scale > 0
-        float alpha = 1.f;
-        const bool need = m_tile > m_run + 8.f;
-        if (need) {
-          alpha = ex2_approx(m_run - m_tile);  // 0 on the first tile (m_run = -inf)
-          m_run = m_tile;
-          l *= alpha;
-        }
-        if (j > 0 && __any_sync(0xffffffffu, need)) {
-          if (NQT == 1) mbar_wait(&pv_done[t], (uint32_t)((j - 1) & 1));  // O holds tiles 0..j-1
-          tc_fence_after();                // (NQT == 2: implied by s_full, see the MMA schedule)
-#pragma unroll 1
-          for (int c = 0; c < p.dpad16; c += 16) {
-            uint32_t o[16];
-            tmem_ld16(tmem_O + (uint32_t)c, o);
-            tmem_ld_wait();
-#pragma unroll
-            for (int i = 0; i < 16; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * alpha);
-            tmem_st16(tmem_O + (uint32_t)c, o);
-          }
-          tmem_st_wait();
-        }
-        const float neg_m = -m_run;
-        EA_T(3);
-        float s0 = 0.f, s1 = 0.f, s2 = 0.f, s3 = 0.f;
-#pragma unroll
-        for (int h = 0; h < 4; ++h) {
-          uint32_t pk[16];
-#pragma unroll
-          for (int i = 0; i < 32; i += 4) {
-            const float sc = BIAS ? 1.f : p.scale_log2;   // BIAS: v already holds the scaled logits
-            const float e0 = ex2_approx(fmaf(__uint_as_float(v[h][i]), sc, neg_m));
-            const float e1 = ex2_approx(fmaf(__uint_as_float(v[h][i + 1]), sc, neg_m));
-            const float e2 = ex2_approx(fmaf(__uint_as_float(v[h][i + 2]), sc, neg_m));
-            const float e3 = ex2_approx(fmaf(__uint_as_float(v[h][i + 3]), sc, neg_m));
-            s0 += e0; s1 += e1; s2 += e2; s3 += e3;
-            pk[i >> 1] = ea_pack2(e0, e1);
-            pk[(i >> 1) + 1] = ea_pack2(e2, e3);
-          }
-          if (p.p_smem) {
-            const int c = h * 32;
-            uint8_t* prow = sP + (t * 2 + (c >> 6)) * AT_ATOM + r * 128;
-#pragma unroll
-            for (int g = 0; g < 4; ++g) {
-              const int c16 = ((c & 63) >> 3) + g;
-              *reinterpret_cast<uint4*>(prow + ((c16 ^ (r & 7)) << 4)) =
-                  make_uint4(pk[4 * g], pk[4 * g + 1], pk[4 * g + 2], pk[4 * g + 3]);
-            }
-          } else {
-            tmem_st16(tmem_S + (uint32_t)(h * 16), pk);  // P over the consumed logits columns
-          }
-        }
-        l += (s0 + s1) + (s2 + s3);
-      }
-      EA_T(4);
-      if (p.p_smem) fence_proxy_async();
-      else tmem_st_wait();
-      tc_fence_before();
-      mbar_arrive(&p_ready[t]);
-      EA_T(5);
-    }
-    // ---- epilogue: O / l
-    mbar_wait(&pv_done[t], NQT == 2 ? 0u : (uint32_t)((n_tiles - 1) & 1));
-    tc_fence_after();
-    const float inv_l = 1.f / l;
-    ea_half* orow = p.out + (long long)b * p.o_bs + (long long)(row_ok ? q : 0) * p.o_ns +
-                    (long long)head * p.d;
-#pragma unroll 1
-    for (int c = 0; c < p.dpad16; c += 16) {
-      uint32_t o[16];
-      tmem_ld16(tmem_O + (uint32_t)c, o);
-      tmem_ld_wait();
-      if (row_ok) {
-#pragma unroll
-        for (int g = 0; g < 2; ++g) {
-          if (c + g * 8 < p.d) {
-            uint4 u = make_uint4(
-                ea_pack2(__uint_as_float(o[g * 8 + 0]) * inv_l, __uint_as_float(o[g * 8 + 1]) * inv_l),
-                ea_pack2(__uint_as_float(o[g * 8 + 2]) * inv_l, __uint_as_float(o[g * 8 + 3]) * inv_l),
-                ea_pack2(__uint_as_float(o[g * 8 + 4]) * inv_l, __uint_as_float(o[g * 8 + 5]) * inv_l),
-                ea_pack2(__uint_as_float(o[g * 8 + 6]) * inv_l, __uint_as_float(o[g * 8 + 7]) * inv_l));
-            *reinterpret_cast<uint4*>(orow + c + g * 8) = u;
-          }
-        }
-      }
-      __syncwarp();
-    }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == W_MMA) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512u);
-  }
-}
-
-// ---------------------------------------------------------------------------------------------
-// ea_attn_db_kernel: the long-sequence, small-head variant (d <= 64, no bias: the 64x64-latent
-// self-attention of SD1.5 with d = 40, 4096 - 16384 keys, where softmax's exp is the bound).
-// Same roles as ea_attn_kernel<2,false>, but the K/V tile is 96 keys so that BOTH query tiles get a
-// DOUBLE-BUFFERED logits accumulator in TMEM (4 x 96 + 2 x 64 columns = 512): S(j+2) is computed
-// while softmax works on S(j), so a softmax warpgroup never waits for the tensor core (with one
-// S buffer per tile it sat idle for the whole P -> PV -> QK^T round trip, ~1000 clk per tile:
-// profiles/r01g_exp_attn_phase_timing.txt).
-static constexpr int DB_BKV = 96;
-static constexpr int DB_KVT = DB_BKV * 128;       // bytes of one 96-row x 64-half swizzled tile
-static constexpr int DB_STAGES = 4;
-
-__global__ void __launch_bounds__(128 * 2 + 64, 1)
-ea_attn_db_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
-                  const __grid_constant__ CUtensorMap tmV, const AttnKParams p) {
-  extern __shared__ __align__(1024) uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
-                                             ~uintptr_t(1023));
-  // layout: Q[2] (16 KB each) | KV[DB_STAGES][K 12 KB | V 12 KB] | barriers
-  uint8_t* sQ = smem;
-  uint8_t* sKV = sQ + 2 * AT_ATOM;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sKV + DB_STAGES * 2 * DB_KVT);
-  uint64_t* q_full = bars;                          // [1]
-  uint64_t* kv_full = bars + 1;                     // [DB_STAGES]
-  uint64_t* kv_empty = kv_full + DB_STAGES;         // [DB_STAGES]
-  uint64_t* s_full = kv_empty + DB_STAGES;          // [2 tiles][2 buffers]
-  uint64_t* p_ready = s_full + 4;                   // [2][2] per (tile, logits buffer): a query tile's
-                                                    // softmax can run two key tiles ahead of the MMA warp
-                                                    // (stalled on the other tile), so one barrier per tile
-                                                    // would be overrun by a whole phase
-  uint64_t* o_done = p_ready + 4;                   // [2]
-  uint64_t* pv_prev = o_done + 2;                   // [2]  PV of the second-to-last tile retired
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(pv_prev + 2);
-
-  pdl_launch_dependents();
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const int qb = blockIdx.x, head = blockIdx.y, b = blockIdx.z;
-  const int n_tiles = (p.Nkv + DB_BKV - 1) / DB_BKV;
-  constexpr int W_TMA = 8, W_MMA = 9;
-
-  if (warp == W_TMA && lane == 0) {
-    tma_prefetch_desc(&tmQ);
-    tma_prefetch_desc(&tmK);
-    tma_prefetch_desc(&tmV);
-    mbar_init(q_full, 1);
-    for (int s = 0; s < DB_STAGES; ++s) {
-      mbar_init(&kv_full[s], 1);
-      mbar_init(&kv_empty[s], 1);
-    }
-    for (int i = 0; i < 4; ++i) mbar_init(&s_full[i], 1);
-    for (int t = 0; t < 2; ++t) {
-      mbar_init(&p_ready[2 * t], 128);
-      mbar_init(&p_ready[2 * t + 1], 128);
-      mbar_init(&o_done[t], 1);
-      mbar_init(&pv_prev[t], 1);
-    }
-    fence_mbar_init();
-  }
-  if (warp == W_MMA) tmem_alloc(tmem_slot, 512u);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   pdl_wait();
-  // TMEM columns: S[t][buf] at (2t + buf) * 96, O[t] at 384 + 64 t
-  if (warp == W_TMA) {
-    if (lane == 0) {
-      mbar_expect_tx(q_full, 2u * AT_ATOM);
-      for (int t = 0; t < 2; ++t)
-        tma_load_4d(sQ + t * AT_ATOM, &tmQ, q_full, 0, head, (qb * 2 + t) * AT_BQ, b);
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int j = 0; j < n_tiles; ++j) {
-        mbar_wait(&kv_empty[stage], phase ^ 1u);
-        uint8_t* sK = sKV + stage * 2 * DB_KVT;
-        mbar_expect_tx(&kv_full[stage], 2u * DB_KVT);
-        tma_load_4d(sK, &tmK, &kv_full[stage], 0, head, j * DB_BKV, b);
-        tma_load_4d(sK + DB_KVT, &tmV, &kv_full[stage], 0, head, j * DB_BKV, b);
-        if (++stage == DB_STAGES) { stage = 0; phase ^= 1u; }
-      }
+  // K/V tile jj into its stage of the ring (thread 0; the stage's previous tile has been released)
+  auto load_kv = [&](int jj) {
+    const int st = jj % p.stages;
+    uint8_t* sK = sKV + st * kv_stage_bytes;
+    uint8_t* sV = sK + p.nd * AT_ATOM;
+    mbar_expect_tx(&kv_full[st], (uint32_t)kv_stage_bytes);
+    for (int a = 0; a < p.nd; ++a) {
+      tma_load_4d(sK + a * AT_ATOM, &tmK, &kv_full[st], a * 64, head, jj * AT_BKV, b);
+      tma_load_4d(sV + a * AT_ATOM, &tmV, &kv_full[st], a * 64, head, jj * AT_BKV, b);
     }
-  } else if (warp == W_MMA) {
-    const uint32_t tb = __shfl_sync(0xffffffffu, tmem_base, 0);
-    const uint32_t idesc_s = umma_idesc(128, DB_BKV, 0, 0);
-    const uint32_t idesc_o = umma_idesc(128, (uint32_t)p.dpad16, 0, 1);
-    const uint64_t dQ0 = umma_desc_k_sw128(smem_u32(sQ), 1024);
-    const uint64_t dK0 = umma_desc_k_sw128(smem_u32(sKV), 1024);
-    const uint64_t dV0 = umma_desc_mn_sw128(smem_u32(sKV) + DB_KVT, DB_KVT, 1024);
-    const int ksteps = p.ksteps;
-    auto issue_S = [&](int t, int stage, int buf) {
-      uint64_t dq = dQ0 + (uint64_t)(t * (AT_ATOM >> 4));
-      uint64_t dk = dK0 + (uint64_t)(stage * (2 * DB_KVT >> 4));
-      const uint32_t d = tb + (uint32_t)((2 * t + buf) * DB_BKV);
-      umma_f16_ss(d, dq, dk, idesc_s, 0u);
-      for (int ks = 1; ks < ksteps; ++ks) {
-        dq += 2; dk += 2;
-        umma_f16_ss(d, dq, dk, idesc_s, 1u);
-      }
-    };
-    auto issue_PV = [&](int t, int stage, int buf, bool first) {
-      uint64_t dv = dV0 + (uint64_t)(stage * (2 * DB_KVT >> 4));
-      const uint32_t d = tb + 384u + (uint32_t)(t * 64);
-      uint32_t pa = tb + (uint32_t)((2 * t + buf) * DB_BKV);
-      uint32_t acc = first ? 0u : 1u;
-#pragma unroll
-      for (int ks = 0; ks < DB_BKV / 16; ++ks) {
-        umma_f16_ts(d, pa, dv, idesc_o, acc);
-        acc = 1u;
-        pa += 8u;
-        dv += (16 * 128) >> 4;
-      }
-    };
-    mbar_wait(q_full, 0);
-    // prologue: S(0) and S(1) of both tiles
-    for (int j = 0; j < 2 && j < n_tiles; ++j) {
-      mbar_wait(&kv_full[j], 0);
-      tc_fence_after();
-      EA_ISSUE(issue_S(0, j, j); umma_commit(&s_full[0 * 2 + j]); issue_S(1, j, j); umma_commit(&s_full[1 * 2 + j]));
-    }
-    int stage = 0;            // stage of K/V tile j
-    uint32_t phase = 0;
-    for (int j = 0; j < n_tiles; ++j) {
-      const int buf = j & 1;
-      const int j2 = j + 2;
-      int st2 = stage + 2;    // stage of tile j + 2
-      uint32_t ph2 = phase;
-      if (st2 >= DB_STAGES) { st2 -= DB_STAGES; ph2 ^= 1u; }
-      for (int t = 0; t < 2; ++t) {
-        mbar_wait(&p_ready[2 * t + buf], (uint32_t)((j >> 1) & 1));
-        tc_fence_after();
-        EA_ISSUE(issue_PV(t, stage, buf, j == 0);
-                 if (j + 1 == n_tiles) umma_commit(&o_done[t]);
-                 if (j + 2 == n_tiles) umma_commit(&pv_prev[t]);
-                 if (t == 1) umma_commit(&kv_empty[stage]));
-        if (j2 < n_tiles) {
-          if (t == 0) {
-            mbar_wait(&kv_full[st2], ph2);
-            tc_fence_after();
-          }
-          EA_ISSUE(issue_S(t, st2, buf); umma_commit(&s_full[t * 2 + buf]));
-        }
-      }
-      if (++stage == DB_STAGES) { stage = 0; phase ^= 1u; }
-    }
-  } else {
-    // ======================= softmax warpgroups (tile t = warp >> 2) =====================
-    const int t = warp >> 2;
-    const int wq = warp & 3;
-    const int r = wq * 32 + lane;
-    const int q = (qb * 2 + t) * AT_BQ + r;
-    const bool row_ok = q < p.Nq;
-    const uint32_t lane_off = (uint32_t)(wq * 32) << 16;
-    const uint32_t tmem_O = tmem_base + lane_off + 384u + (uint32_t)(t * 64);
-    float m_run = -INFINITY;
-    float l = 0.f;
-    for (int j = 0; j < n_tiles; ++j) {
-      const int buf = j & 1;
-      mbar_wait(&s_full[t * 2 + buf], (uint32_t)((j >> 1) & 1));
-      tc_fence_after();
-      const uint32_t tmem_S = tmem_base + lane_off + (uint32_t)((2 * t + buf) * DB_BKV);
-      const int valid = min(DB_BKV, p.Nkv - j * DB_BKV);
-      uint32_t v[3][32];
-      tmem_ld32(tmem_S, v[0]);
-      tmem_ld32(tmem_S + 32u, v[1]);
-      tmem_ld32(tmem_S + 64u, v[2]);
-      tmem_ld_wait();
-      if (valid < DB_BKV) {
-#pragma unroll
-        for (int h = 0; h < 3; ++h)
-#pragma unroll
-          for (int i = 0; i < 32; ++i)
-            if (h * 32 + i >= valid) v[h][i] = 0xff800000u;
-      }
-      float mx0 = -INFINITY, mx1 = -INFINITY, mx2 = -INFINITY;
-#pragma unroll
-      for (int i = 0; i < 32; ++i) {
-        mx0 = fmaxf(mx0, __uint_as_float(v[0][i]));
-        mx1 = fmaxf(mx1, __uint_as_float(v[1][i]));
-        mx2 = fmaxf(mx2, __uint_as_float(v[2][i]));
-      }
-      const float m_tile = fmaxf(fmaxf(mx0, mx1), mx2) * p.scale_log2;
-      float alpha = 1.f;
-      const bool need = m_tile > m_run + 8.f;
-      if (need) {
-        alpha = ex2_approx(m_run - m_tile);
-        m_run = m_tile;
-        l *= alpha;
-      }
-      if (j > 0 && __any_sync(0xffffffffu, need)) {
-        // O must hold tiles 0..j-1: PV(j-1) retires before S(j+1) does (same in-order MMA queue);
-        // on the last tile the epilogue barrier is the only later event
-        if (j + 1 < n_tiles) mbar_wait(&s_full[t * 2 + ((j + 1) & 1)], (uint32_t)(((j + 1) >> 1) & 1));
-        else mbar_wait(&pv_prev[t], 0u);   // last tile: no S(j+1) exists; PV(j-1) signals by itself
-        tc_fence_after();
-#pragma unroll 1
-        for (int c = 0; c < p.dpad16; c += 16) {
-          uint32_t o[16];
-          tmem_ld16(tmem_O + (uint32_t)c, o);
-          tmem_ld_wait();
-#pragma unroll
-          for (int i = 0; i < 16; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * alpha);
-          tmem_st16(tmem_O + (uint32_t)c, o);
-        }
-        tmem_st_wait();
-      }
-      const float neg_m = -m_run;
-      float s0 = 0.f, s1 = 0.f, s2 = 0.f, s3 = 0.f;
-#pragma unroll
-      for (int h = 0; h < 3; ++h) {
-        uint32_t pk[16];
-#pragma unroll
-        for (int i = 0; i < 32; i += 4) {
-          const float e0 = ex2_approx(fmaf(__uint_as_float(v[h][i]), p.scale_log2, neg_m));
-          const float e1 = ex2_approx(fmaf(__uint_as_float(v[h][i + 1]), p.scale_log2, neg_m));
-          const float e2 = ex2_approx(fmaf(__uint_as_float(v[h][i + 2]), p.scale_log2, neg_m));
-#ifdef EA_ATTN_EXP_MUFU_ONLY
-          const float e3 = ex2_approx(fmaf(__uint_as_float(v[h][i + 3]), p.scale_log2, neg_m));
-#else
-          const float e3 = ex2_poly(fmaf(__uint_as_float(v[h][i + 3]), p.scale_log2, neg_m));
-#endif
-          s0 += e0; s1 += e1; s2 += e2; s3 += e3;
-          pk[i >> 1] = ea_pack2(e0, e1);
-          pk[(i >> 1) + 1] = ea_pack2(e2, e3);
-        }
-        tmem_st16(tmem_S + (uint32_t)(h * 16), pk);
-      }
-      l += (s0 + s1) + (s2 + s3);
-      tmem_st_wait();
-      tc_fence_before();
-      mbar_arrive(&p_ready[2 * t + buf]);
-    }
-    mbar_wait(&o_done[t], 0u);
-    tc_fence_after();
-    const float inv_l = 1.f / l;
-    ea_half* orow = p.out + (long long)b * p.o_bs + (long long)(row_ok ? q : 0) * p.o_ns +
-                    (long long)head * p.d;
-#pragma unroll 1
-    for (int c = 0; c < p.dpad16; c += 16) {
-      uint32_t o[16];
-      tmem_ld16(tmem_O + (uint32_t)c, o);
-      tmem_ld_wait();
-      if (row_ok) {
-#pragma unroll
-        for (int g = 0; g < 2; ++g) {
-          if (c + g * 8 < p.d) {
-            uint4 u = make_uint4(
-                ea_pack2(__uint_as_float(o[g * 8 + 0]) * inv_l, __uint_as_float(o[g * 8 + 1]) * inv_l),
-                ea_pack2(__uint_as_float(o[g * 8 + 2]) * inv_l, __uint_as_float(o[g * 8 + 3]) * inv_l),
-                ea_pack2(__uint_as_float(o[g * 8 + 4]) * inv_l, __uint_as_float(o[g * 8 + 5]) * inv_l),
-                ea_pack2(__uint_as_float(o[g * 8 + 6]) * inv_l, __uint_as_float(o[g * 8 + 7]) * inv_l));
-            *reinterpret_cast<uint4*>(orow + c + g * 8) = u;
-          }
-        }
-      }
-      __syncwarp();
-    }
+  };
+  if (producer) {
+    mbar_expect_tx(q_full, (uint32_t)(p.nd * AT_ATOM));
+    for (int a = 0; a < p.nd; ++a) tma_load_4d(sQ + a * AT_ATOM, &tmQ, q_full, a * 64, head, qb * AT_BQ, b);
+    for (int jj = 0; jj < p.stages && jj < n_tiles; ++jj) load_kv(jj);
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == W_MMA) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512u);
+
+  const int wg = warp >> 2, wq = warp & 3;
+  const int g = lane >> 2, t4 = lane & 3;
+  // accumulator layout (ea_wgmma.cuh): this thread holds rows rl (i % 4 < 2) and rl + 8 (i % 4 >= 2) of the tile,
+  // columns 8 (i / 4) + 2 t4 + i % 2
+  const int rl = wg * 64 + wq * 16 + g;
+  const int q_lo = qb * AT_BQ + rl, q_hi = q_lo + 8;
+  const float LOG2E = 1.4426950408889634f;
+  const float* rh_lo = nullptr;
+  const float* rh_hi = nullptr;
+  if (BIAS) {
+    // rel_w rows of the CTA's queries (pre-multiplied by log2e) in shared memory; rel_h comes through L1
+    const long long bh = (long long)b * p.heads + head;
+    for (int idx = threadIdx.x; idx < AT_BQ * p.rel_s; idx += AT_THREADS) {
+      const int row = idx / p.rel_s, i = idx - row * p.rel_s;
+      const int q = qb * AT_BQ + row;
+      rw_s[row * (p.rel_s + 1) + i] = q < p.Nq ? __ldg(p.rel_w + (bh * p.Nq + q) * p.rel_s + i) * LOG2E : 0.f;
+    }
+    rh_lo = p.rel_h + (bh * p.Nq + (q_lo < p.Nq ? q_lo : 0)) * p.rel_s;
+    rh_hi = p.rel_h + (bh * p.Nq + (q_hi < p.Nq ? q_hi : 0)) * p.rel_s;
+    asm volatile("bar.sync 1, 256;" ::: "memory");
+  }
+  const uint64_t dQ0 = gmma_desc_k_sw128(smem_u32(sQ) + (uint32_t)(wg * 64 * 128), 1024);
+  const uint64_t dK0 = gmma_desc_k_sw128(smem_u32(sKV), 1024);
+  const uint64_t dV0 = gmma_desc_mn_sw128(smem_u32(sKV) + (uint32_t)(p.nd * AT_ATOM), AT_ATOM, 1024);
+  const uint32_t kv_stage16 = (uint32_t)kv_stage_bytes >> 4;
+
+  float o[DO / 2];
+#pragma unroll
+  for (int i = 0; i < DO / 2; ++i) o[i] = 0.f;
+  float m_lo = -INFINITY, m_hi = -INFINITY;   // running max in the scaled log2 domain
+  float l_lo = 0.f, l_hi = 0.f;               // this thread's share of the running sum
+  mbar_wait(q_full, 0);
+  int stage = 0;
+  uint32_t phase = 0;
+  for (int j = 0; j < n_tiles; ++j) {
+    mbar_wait(&kv_full[stage], phase);
+    // ---- S = Q K^T.  K-step ks sits at atom (ks >> 2), +32 B * (ks & 3)
+    float s[64];
+    {
+      uint64_t dq = dQ0, dk = dK0 + (uint64_t)(stage * kv_stage16);
+      wgmma_fence();
+      Wgmma<128>::ss(s, dq, dk, 0u);
+      for (int ks = 1; ks < p.ksteps; ++ks) {
+        const uint32_t step = (ks & 3) ? 2u : (uint32_t)((AT_ATOM >> 4) - 6);
+        dq += step;
+        dk += step;
+        Wgmma<128>::ss(s, dq, dk, 1u);
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_regs(s);
+    }
+    // ---- scaled logits (+ bias), missing keys of the last tile -> -inf, row max
+    const int valid = min(AT_BKV, p.Nkv - j * AT_BKV);  // keys of this tile that exist (>= 1)
+    float mx_lo = -INFINITY, mx_hi = -INFINITY;
+#pragma unroll
+    for (int i = 0; i < 64; i += 2) {
+      const int col = 8 * (i >> 2) + 2 * t4;
+      const bool hi = (i >> 1) & 1;
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        float x = s[i + e] * p.scale_log2;
+        if (BIAS) {
+          const int key = j * AT_BKV + col + e;
+          const int kh = key / p.rel_s, kw = key - kh * p.rel_s;
+          x += rw_s[(rl + (hi ? 8 : 0)) * (p.rel_s + 1) + kw] + __ldg((hi ? rh_hi : rh_lo) + min(kh, p.rel_s - 1)) * LOG2E;
+        }
+        if (col + e >= valid) x = -INFINITY;
+        s[i + e] = x;
+        if (hi) mx_hi = fmaxf(mx_hi, x);
+        else mx_lo = fmaxf(mx_lo, x);
+      }
+    }
+    mx_lo = fmaxf(mx_lo, __shfl_xor_sync(0xffffffffu, mx_lo, 1));
+    mx_lo = fmaxf(mx_lo, __shfl_xor_sync(0xffffffffu, mx_lo, 2));
+    mx_hi = fmaxf(mx_hi, __shfl_xor_sync(0xffffffffu, mx_hi, 1));
+    mx_hi = fmaxf(mx_hi, __shfl_xor_sync(0xffffffffu, mx_hi, 2));
+    const float mn_lo = fmaxf(m_lo, mx_lo), mn_hi = fmaxf(m_hi, mx_hi);
+    const float a_lo = ex2_approx(m_lo - mn_lo), a_hi = ex2_approx(m_hi - mn_hi);   // 0 on the first tile
+    m_lo = mn_lo;
+    m_hi = mn_hi;
+    l_lo *= a_lo;
+    l_hi *= a_hi;
+#pragma unroll
+    for (int i = 0; i < DO / 2; ++i) o[i] *= ((i >> 1) & 1) ? a_hi : a_lo;
+    // ---- P = exp2(x - m), packed to 16 bit as the A fragments of the 8 K-steps (16 keys each) of P V
+    uint32_t pa[8][4];
+#pragma unroll
+    for (int kk = 0; kk < 8; ++kk) {
+#pragma unroll
+      for (int h = 0; h < 4; ++h) {
+        const int i = 8 * kk + 2 * h;
+        const float m = (h & 1) ? m_hi : m_lo;
+        const float e0 = ex2_approx(s[i] - m), e1 = ex2_approx(s[i + 1] - m);
+        if (h & 1) l_hi += e0 + e1;
+        else l_lo += e0 + e1;
+        pa[kk][h] = ea_pack2(e0, e1);
+      }
+    }
+    // ---- O += P V ; V K-step kk = 16 key rows = +2048 B
+    {
+      uint64_t dv = dV0 + (uint64_t)(stage * kv_stage16);
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < 8; ++kk) Wgmma<DO>::rs(o, pa[kk], dv + (uint64_t)(kk * ((16 * 128) >> 4)), 1u);
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_regs(o);
+      wgmma_fence_regs_u32(pa);
+    }
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&kv_empty[stage]);
+    if (producer && j + p.stages < n_tiles) {   // every warp has released tile j's stage: refill it
+      mbar_wait(&kv_empty[stage], phase);
+      load_kv(j + p.stages);
+    }
+    if (++stage == p.stages) { stage = 0; phase ^= 1u; }
+  }
+  // ---- epilogue: O / l
+  l_lo += __shfl_xor_sync(0xffffffffu, l_lo, 1);
+  l_lo += __shfl_xor_sync(0xffffffffu, l_lo, 2);
+  l_hi += __shfl_xor_sync(0xffffffffu, l_hi, 1);
+  l_hi += __shfl_xor_sync(0xffffffffu, l_hi, 2);
+  const float inv_lo = 1.f / l_lo, inv_hi = 1.f / l_hi;
+  ea_half* orow_lo = p.out + (long long)b * p.o_bs + (long long)q_lo * p.o_ns + (long long)head * p.d;
+  ea_half* orow_hi = orow_lo + 8 * p.o_ns;
+#pragma unroll
+  for (int i = 0; i < DO / 2; i += 4) {
+    const int col = 8 * (i >> 2) + 2 * t4;
+    if (col < p.d) {
+      if (q_lo < p.Nq) *reinterpret_cast<uint32_t*>(orow_lo + col) = ea_pack2(o[i] * inv_lo, o[i + 1] * inv_lo);
+      if (q_hi < p.Nq) *reinterpret_cast<uint32_t*>(orow_hi + col) = ea_pack2(o[i + 2] * inv_hi, o[i + 3] * inv_hi);
+    }
   }
 }
 
 static int encode_qkv(CUtensorMap* m, const void* base, int d, int heads, int N, int B,
-                      long long ns, long long bs, int box_rows = 128) {
+                      long long ns, long long bs) {
   cuuint64_t dims[4] = {(cuuint64_t)d, (cuuint64_t)heads, (cuuint64_t)N, (cuuint64_t)B};
   cuuint64_t strides[3] = {(cuuint64_t)d * 2, (cuuint64_t)ns * 2, (cuuint64_t)bs * 2};
-  cuuint32_t box[4] = {64, 1, (cuuint32_t)box_rows, 1};
+  cuuint32_t box[4] = {64, 1, 128, 1};
   cuuint32_t estr[4] = {1, 1, 1, 1};
   CUresult r = ea_tmap_encode()(m, EA_TMAP_DTYPE, 4, const_cast<void*>(base), dims, strides, box,
                                 estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
@@ -763,35 +262,25 @@ static int encode_qkv(CUtensorMap* m, const void* base, int d, int heads, int N,
   return r == CUDA_SUCCESS ? 0 : (int)r;
 }
 
-template <int NQT, bool BIAS>
+template <int DO, bool BIAS>
 static int launch_attn(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv,
                        const AttnKParams& p, dim3 grid, int smem_bytes, cudaStream_t stream) {
   static int max_set_dev[EA_MAX_DEV];
   int& max_set = max_set_dev[ea_dev()];
   if (smem_bytes > max_set) {
-    if (cudaFuncSetAttribute(ea_attn_kernel<NQT, BIAS>,
-                             cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes) != cudaSuccess)
-      return EA_ERR_CUDA;
+    const cudaError_t e = cudaFuncSetAttribute(ea_attn_kernel<DO, BIAS>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                               smem_bytes);
+    if (e != cudaSuccess) return ea_cuda_fail(e, "ea_attention: cudaFuncSetAttribute(MaxDynamicSharedMemorySize)");
     max_set = smem_bytes;
   }
-  return ea_launch(ea_attn_kernel<NQT, BIAS>, grid, dim3(128 * NQT + 64), (size_t)smem_bytes, stream,
-                   tq, tk, tv, p) == cudaSuccess ? 0 : EA_ERR_CUDA;
+  const cudaError_t e = ea_launch(ea_attn_kernel<DO, BIAS>, grid, dim3(AT_THREADS), (size_t)smem_bytes, stream,
+                                  tq, tk, tv, p);
+  return e == cudaSuccess ? 0 : ea_cuda_fail(e, "ea_attention: kernel launch");
 }
 
 }  // namespace ea
 
 using namespace ea;
-
-#ifdef EA_ATTN_TIMING
-extern "C" int ea_attn_debug_read(long long* host_out, int n) {
-  if (n > 2 * 8 * 8) n = 2 * 8 * 8;
-  return cudaMemcpyFromSymbol(host_out, ea_attn_dbg, sizeof(long long) * n) == cudaSuccess ? 0 : EA_ERR_CUDA;
-}
-extern "C" int ea_attn_debug_read_mma(long long* host_out, int n) {
-  if (n > 2 * 8 * 4) n = 2 * 8 * 4;
-  return cudaMemcpyFromSymbol(host_out, ea_attn_dbg_mma, sizeof(long long) * n) == cudaSuccess ? 0 : EA_ERR_CUDA;
-}
-#endif
 
 extern "C" int ea_attention(const ea_attn_args* a, void* stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
@@ -804,71 +293,24 @@ extern "C" int ea_attention(const ea_attn_args* a, void* stream_) {
   if ((a->rel_h != nullptr) != (a->rel_w != nullptr)) return EA_ERR_ARG;
   if (a->rel_h && a->rel_s <= 0) return EA_ERR_ARG;
 
-  static const int force_p_smem = [] { const char* e = getenv("EA_ATTN_P_SMEM"); return e && e[0] == '1'; }();
-  static const int force_nqt = [] { const char* e = getenv("EA_ATTN_NQT"); return e ? atoi(e) : 0; }();
-
   AttnKParams p;
   memset(&p, 0, sizeof(p));
   p.Nq = a->Nq; p.Nkv = a->Nkv; p.d = a->d; p.heads = a->heads;
   p.nd = (a->d + 63) / 64;
   p.ksteps = (a->d + 15) / 16;
-  p.dpad16 = p.ksteps * 16;
-  p.p_smem = force_p_smem;
-  static const int dbg_skip = [] { const char* e = getenv("EA_ATTN_SKIP"); return e ? atoi(e) : 0; }();
-  p.dbg_skip = dbg_skip;
   p.scale_log2 = a->scale * 1.4426950408889634f;
   p.out = reinterpret_cast<ea_half*>(a->out);
   p.o_bs = a->o_bs; p.o_ns = a->o_ns;
   p.rel_h = a->rel_h; p.rel_w = a->rel_w; p.rel_s = a->rel_s;
 
-  // long sequences with small heads: double-buffered logits (ea_attn_db_kernel)
-  static const int db_env = [] { const char* e = getenv("EA_ATTN_DB"); return e ? atoi(e) : 1; }();
-  if (db_env && !a->rel_h && a->d <= 64 && !force_p_smem && force_nqt == 0 && a->Nkv >= 4 * DB_BKV &&
-      (db_env == 2 || (long long)((a->Nq + 2 * AT_BQ - 1) / (2 * AT_BQ)) * a->heads * a->B >= 148)) {
-    CUtensorMap tq, tk, tv;
-    if (encode_qkv(&tq, a->q, a->d, a->heads, a->Nq, a->B, a->q_ns, a->q_bs)) return EA_ERR_TMAP;
-    if (encode_qkv(&tk, a->k, a->d, a->heads, a->Nkv, a->B, a->k_ns, a->k_bs, DB_BKV)) return EA_ERR_TMAP;
-    if (encode_qkv(&tv, a->v, a->d, a->heads, a->Nkv, a->B, a->v_ns, a->v_bs, DB_BKV)) return EA_ERR_TMAP;
-    const int smem_bytes = 2 * AT_ATOM + DB_STAGES * 2 * DB_KVT + (1 + 2 * DB_STAGES + 12) * 8 + 16 + 1024;
-    static int db_set_dev[EA_MAX_DEV];
-    int& db_set = db_set_dev[ea_dev()];
-    if (!db_set) {
-      if (cudaFuncSetAttribute(ea_attn_db_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes) !=
-          cudaSuccess)
-        return EA_ERR_CUDA;
-      db_set = 1;
-    }
-    dim3 grid((unsigned)((a->Nq + 2 * AT_BQ - 1) / (2 * AT_BQ)), (unsigned)a->heads, (unsigned)a->B);
-    if (ea_launch(ea_attn_db_kernel, grid, dim3(128 * 2 + 64), (size_t)smem_bytes, stream, tq, tk, tv, p) !=
-        cudaSuccess)
-      return EA_ERR_CUDA;
-    ea_count_launch();
-    return cudaGetLastError() == cudaSuccess ? 0 : EA_ERR_CUDA;
-  }
-
-  // two query tiles per CTA when both accumulators fit TMEM (d <= 128) and there is a second tile
-  int nqt = (a->Nq > AT_BQ && p.dpad16 <= 128) ? 2 : 1;
-  {  // one tile per CTA fills the machine better while two-tile CTAs would leave SMs idle
-    const long long ctas2 = (long long)((a->Nq + 2 * AT_BQ - 1) / (2 * AT_BQ)) * a->heads * a->B;
-    if (nqt == 2 && ctas2 < 148) nqt = 1;
-  }
-  if (force_nqt == 1 || force_nqt == 2) nqt = (force_nqt == 2 && p.dpad16 > 128) ? 1 : force_nqt;
-  const int budget = 225 * 1024 - 1024 - 256;
-  const bool has_bias = a->rel_h != nullptr;
-  auto bias_bytes_for = [&](int n) { return has_bias ? ((n * AT_BQ * (a->rel_s + 1) * 4 + 15) & ~15) : 0; };
-  const int fixed = nqt * p.nd * AT_ATOM + (p.p_smem ? nqt * 2 * AT_ATOM : 0) + bias_bytes_for(nqt);
-  int stages = (budget - fixed) / (2 * p.nd * AT_ATOM);
+  const bool bias = a->rel_h != nullptr;
+  const int budget = 227 * 1024 - 1024 - 256;
+  const int bias_bytes = bias ? ((AT_BQ * (a->rel_s + 1) + 3) & ~3) * 4 : 0;
+  int stages = (budget - p.nd * AT_ATOM - bias_bytes) / (2 * p.nd * AT_ATOM);
   if (stages > AT_MAX_STAGES) stages = AT_MAX_STAGES;
-  if (nqt == 2 && stages < 2) {  // the ping-pong schedule needs two K/V stages
-    nqt = 1;
-    const int fixed1 = p.nd * AT_ATOM + (p.p_smem ? 2 * AT_ATOM : 0) + bias_bytes_for(1);
-    stages = (budget - fixed1) / (2 * p.nd * AT_ATOM);
-    if (stages > AT_MAX_STAGES) stages = AT_MAX_STAGES;
-  }
   if (stages < 1) return EA_ERR_SHAPE;
   const int n_tiles = (a->Nkv + AT_BKV - 1) / AT_BKV;
   if (stages > n_tiles) stages = n_tiles;
-  if (nqt == 2 && stages < 2) stages = 2;
   p.stages = stages;
 
   CUtensorMap tq, tk, tv;
@@ -876,19 +318,17 @@ extern "C" int ea_attention(const ea_attn_args* a, void* stream_) {
   if (encode_qkv(&tk, a->k, a->d, a->heads, a->Nkv, a->B, a->k_ns, a->k_bs)) return EA_ERR_TMAP;
   if (encode_qkv(&tv, a->v, a->d, a->heads, a->Nkv, a->B, a->v_ns, a->v_bs)) return EA_ERR_TMAP;
 
-  p.bias_bytes = bias_bytes_for(nqt);
-  const int smem_bytes = nqt * p.nd * AT_ATOM + p.stages * 2 * p.nd * AT_ATOM +
-                         (p.p_smem ? nqt * 2 * AT_ATOM : 0) + p.bias_bytes +
-                         (1 + 2 * AT_MAX_STAGES + 6) * 8 + 16 + 1024;
-  dim3 grid((unsigned)((a->Nq + AT_BQ * nqt - 1) / (AT_BQ * nqt)), (unsigned)a->heads,
-            (unsigned)a->B);
+  const int smem_bytes = p.nd * AT_ATOM + stages * 2 * p.nd * AT_ATOM + bias_bytes + (1 + 2 * AT_MAX_STAGES) * 8 + 1024;
+  dim3 grid((unsigned)((a->Nq + AT_BQ - 1) / AT_BQ), (unsigned)a->heads, (unsigned)a->B);
   int st;
-  const bool bias = a->rel_h != nullptr;
-  if (nqt == 2) st = bias ? launch_attn<2, true>(tq, tk, tv, p, grid, smem_bytes, stream)
-                          : launch_attn<2, false>(tq, tk, tv, p, grid, smem_bytes, stream);
-  else st = bias ? launch_attn<1, true>(tq, tk, tv, p, grid, smem_bytes, stream)
-                 : launch_attn<1, false>(tq, tk, tv, p, grid, smem_bytes, stream);
+  if (a->d <= 64) st = bias ? launch_attn<64, true>(tq, tk, tv, p, grid, smem_bytes, stream)
+                            : launch_attn<64, false>(tq, tk, tv, p, grid, smem_bytes, stream);
+  else if (a->d <= 128) st = bias ? launch_attn<128, true>(tq, tk, tv, p, grid, smem_bytes, stream)
+                                  : launch_attn<128, false>(tq, tk, tv, p, grid, smem_bytes, stream);
+  else st = bias ? launch_attn<192, true>(tq, tk, tv, p, grid, smem_bytes, stream)
+                 : launch_attn<192, false>(tq, tk, tv, p, grid, smem_bytes, stream);
   if (st) return st;
   ea_count_launch();
-  return cudaGetLastError() == cudaSuccess ? 0 : EA_ERR_CUDA;
+  const cudaError_t e = cudaGetLastError();
+  return e == cudaSuccess ? 0 : ea_cuda_fail(e, "ea_attention: after the kernel launch");
 }

@@ -1,14 +1,15 @@
-// ea_common.cuh — sm_100a PTX wrappers shared by every kernel in this library.
+// ea_common.cuh — sm_90a PTX wrappers shared by every kernel in this library.
 //
-// Everything here is hand-written inline PTX for Blackwell (B200, sm_100a):
-// mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (alloc / mma / commit / ld / st)
-// and the UMMA shared-memory / instruction descriptor encoders.  No CUTLASS.
+// Everything here is hand-written inline PTX for Hopper (H100, sm_90a):
+// mbarrier, TMA (cp.async.bulk.tensor), wgmma (fence / commit / wait) and the wgmma
+// shared-memory descriptor encoders.  No CUTLASS.
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include "ea_wgmma.cuh"
 
 // ---------------------------------------------------------------------------
 // Storage dtype.  fp16 by default (the reference runs fp16 weights/activations
@@ -18,7 +19,6 @@
 #ifdef EA_USE_BF16
 typedef __nv_bfloat16 ea_half;
 typedef __nv_bfloat162 ea_half2;
-#define EA_UMMA_FMT 1u
 #define EA_TMAP_DTYPE CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
 __device__ __forceinline__ float ea_h2f(ea_half h) { return __bfloat162float(h); }
 __device__ __forceinline__ ea_half ea_f2h(float f) { return __float2bfloat16_rn(f); }
@@ -33,7 +33,6 @@ __device__ __forceinline__ float2 ea_unpack2(uint32_t u) {
 #else
 typedef __half ea_half;
 typedef __half2 ea_half2;
-#define EA_UMMA_FMT 0u
 #define EA_TMAP_DTYPE CU_TENSOR_MAP_DATA_TYPE_FLOAT16
 __device__ __forceinline__ float ea_h2f(ea_half h) { return __half2float(h); }
 __device__ __forceinline__ ea_half ea_f2h(float f) { return __float2half_rn(f); }
@@ -151,203 +150,51 @@ __device__ __forceinline__ void tma_load_4d(void* smem, const CUtensorMap* m, ui
       : "memory");
 }
 
-// ------------------------------- tcgen05 -----------------------------------
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+// -------------------------------- wgmma -------------------------------------
+// Warpgroup MMA (sm_90a): 128 threads issue one wgmma.mma_async together; the fp32 accumulator lives in
+// their registers (layout: ea_wgmma.cuh).  fence before the first wgmma that reads registers written by
+// ordinary instructions, commit closes a group, wait<N> leaves at most N groups in flight.
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// Whole-warp (sync.aligned).  ncols: power of two in [32, 512].
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                   smem_u32(smem_dst)),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols)
-               : "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem]; issued by ONE thread.
-__device__ __forceinline__ void umma_f16_ss(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b,
-                                            uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// D[tmem] (+)= A[tmem] * B[smem]; A is a 16-bit matrix living in TMEM.
-__device__ __forceinline__ void umma_f16_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b,
-                                            uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-      "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// All previously issued tcgen05.mma of this thread arrive on `bar` when complete.
-// (implies tcgen05.fence::before_thread_sync)
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                   smem_u32(bar))
-               : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() {
-  asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-}
-// 32 lanes x 32 columns of 32-bit: thread t of the warp receives lane (base_lane + t),
-// columns [col, col+32).  taddr = (lane << 16) | column.
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]),
-        "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-        "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]),
-      "r"(r[8]), "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
+// The accumulator registers are written asynchronously: this empty asm pins every access to them on its side
+// of a wgmma_wait (without it the compiler may read an accumulator before the MMA that writes it completed).
+template <int R>
+__device__ __forceinline__ void wgmma_fence_regs(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// --------------------------- UMMA descriptors ------------------------------
-// Shared-memory matrix descriptor (64-bit), sm_100 layout:
+// --------------------------- wgmma descriptors -------------------------------
+// Shared-memory matrix descriptor (64-bit), sm_90 layout:
 //   [0,14)  start address >> 4        [16,30) leading-dim byte offset >> 4
-//   [32,46) stride-dim byte offset>>4 [46,48) version = 1
-//   [49,52) base offset = 0           [61,64) layout: 0 none, 2 = SW128, 4 = SW64, 6 = SW32
+//   [32,46) stride-dim byte offset>>4 [49,52) base offset = 0
+//   [62,64) layout: 0 none, 1 = SW128, 2 = SW64, 3 = SW32
 //
 // K-major operand, SWIZZLE_128B: rows are 128 B (64 halves) apart, groups of 8 rows are
 // `sbo_bytes` apart (1024 for a dense tile); LBO is unused.  Stepping K by 16 halves inside the
 // 128 B swizzle atom = +32 B on the start address.
-__device__ __forceinline__ uint64_t umma_desc_k_sw128(uint32_t saddr, uint32_t sbo_bytes) {
+__device__ __forceinline__ uint64_t gmma_desc_k_sw128(uint32_t saddr, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr >> 4) & 0x3FFF);
   d |= (uint64_t)1 << 16;  // LBO (ignored for swizzled K-major)
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;  // version
-  d |= (uint64_t)2 << 61;  // SWIZZLE_128B
+  d |= (uint64_t)1 << 62;  // SWIZZLE_128B
   return d;
 }
 // MN-major operand, SWIZZLE_128B: the atom is 64 MN-elements (128 B) x 8 K-rows (1024 B);
 // atoms along MN are `lbo_bytes` apart, groups of 8 K-rows are `sbo_bytes` apart.
-__device__ __forceinline__ uint64_t umma_desc_mn_sw128(uint32_t saddr, uint32_t lbo_bytes,
+__device__ __forceinline__ uint64_t gmma_desc_mn_sw128(uint32_t saddr, uint32_t lbo_bytes,
                                                        uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr >> 4) & 0x3FFF);
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
+  d |= (uint64_t)1 << 62;
   return d;
-}
-// Instruction descriptor (32-bit) for kind::f16, fp32 accumulate.
-//   [4,6) D fmt: 1 = f32   [7,10) A fmt   [10,13) B fmt  (0 = f16, 1 = bf16)
-//   [15] A major (0 = K)   [16] B major (0 = K, 1 = MN)
-//   [17,23) N >> 3         [24,29) M >> 4
-__host__ __device__ __forceinline__ uint32_t umma_idesc(uint32_t M, uint32_t N, uint32_t a_mn,
-                                                        uint32_t b_mn) {
-  uint32_t d = 0;
-  d |= 1u << 4;
-  d |= EA_UMMA_FMT << 7;
-  d |= EA_UMMA_FMT << 10;
-  d |= (a_mn & 1u) << 15;
-  d |= (b_mn & 1u) << 16;
-  d |= ((N >> 3) & 0x3Fu) << 17;
-  d |= ((M >> 4) & 0x1Fu) << 24;
-  return d;
-}
-
-// ------------------------------ CTA pairs (cta_group::2) ---------------------
-// Two CTAs of a cluster (the two SMs of a TPC) run ONE tcgen05.mma with M = 256: each CTA stages its
-// own 128 rows of A and HALF of the B tile, the leader (cluster rank 0) issues the MMA, which reads
-// both CTAs' shared memory at the same offsets and writes each CTA's 128 accumulator rows into that
-// CTA's own TMEM.  Per SM this halves the B bytes TMA has to deliver per MAC.
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// shared::cta address -> shared::cluster address of the same variable in CTA `rank`
-__device__ __forceinline__ uint32_t mapa_shared(uint32_t addr, uint32_t rank) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(addr), "r"(rank));
-  return r;
-}
-// TMA loads whose completion is signalled on an mbarrier of EITHER CTA of the pair (cluster address)
-__device__ __forceinline__ void tma_load_2d_2cta(void* smem, const CUtensorMap* m, uint32_t bar_cluster,
-                                                 int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], "
-      "[%1, {%3, %4}], [%2];" ::"r"(smem_u32(smem)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(bar_cluster), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_4d_2cta(void* smem, const CUtensorMap* m, uint32_t bar_cluster,
-                                                 int c0, int c1, int c2, int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], "
-      "[%1, {%3, %4, %5, %6}], [%2];" ::"r"(smem_u32(smem)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(bar_cluster), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_alloc_2cta(uint32_t* smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                   smem_u32(smem_dst)),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_2cta(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void umma_f16_ss_2cta(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b,
-                                                 uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// arrives on the barrier at the same shared-memory offset in every CTA of `cta_mask`
-__device__ __forceinline__ void umma_commit_2cta(uint64_t* bar, uint16_t cta_mask) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], "
-      "%1;" ::"r"(smem_u32(bar)),
-      "h"(cta_mask)
-      : "memory");
 }
 
 // ------------------------- programmatic dependent launch -------------------
@@ -362,7 +209,7 @@ __device__ __forceinline__ void pdl_launch_dependents() {
 // --------------------------------- math ------------------------------------
 // Compact forms on purpose: these are inlined 32x per epilogue chunk, and with IEEE division / libdevice
 // erff they were HALF of the GEMM kernel's 240 KB of SASS - the epilogue ran out of the instruction
-// cache whenever launches of different shapes alternated (profiles/r01o).
+// cache whenever launches of different shapes alternated.
 __device__ __forceinline__ float mufu_ex2(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));

@@ -1,4 +1,4 @@
-// ea_gemm.cu — the tcgen05 GEMM / implicit-GEMM convolution kernel (sm_100a).
+// ea_gemm.cu — the wgmma GEMM / implicit-GEMM convolution kernel (sm_90a).
 //
 // One kernel serves every dense contraction of the UNet / ControlNet / SAM hot path
 // (SURVEY.md §8a rows R1, R7, R9-R12):
@@ -7,23 +7,21 @@
 //     ResBlock's 1x1 skip convolution folded in as extra K-blocks (openaimodel.py:233-240,274)
 //   * 3x3 stride-2 pad-1 convolutions (Downsample, openaimodel.py:133-159) (mode CONV_S2)
 //
-// Two kernels share the main loop and the fused epilogue:
-//   * ea_gemm_persistent_kernel (default when K is not split): ONE CTA per SM walks the tile list with two TMEM
-//     accumulators - eight epilogue warps drain tile i while the MMA warp accumulates tile i + 1 (the overlap a second
-//     co-resident CTA would give; with 150-200 KB of shared memory per CTA a second one never fits, ncu: 1 block / SM).
-//   * ea_gemm_kernel (one 128 x BN tile per CTA): split-K and CTA-pair (cta_group::2) launches of the small-M,
-//     weight-bound layers; up to 2 CTAs per SM when the stage ring is shallow enough (the planner's `occ`).
-// Roles in both:
-//   TMA producer : A tile (128 rows x 64 halves, SWIZZLE_128B) and B tile (BN x 64) into a `stages`-deep shared-memory
-//                  ring, mbarrier-signalled.  For convolutions the A tile of filter tap (kh,kw) is a 4-D box
-//                  {64ch, bw, bh, bn} of the NHWC tensor shifted by (kh-1, kw-1); the zero padding is TMA out-of-bounds
-//                  fill, no im2col buffer exists.  W-operand loads carry an L2 evict-first hint (see gemm_fill_group).
-//   MMA issuer   : one elected thread issues tcgen05.mma (M=128, N=BN, K=16) x4 per stage, accumulating fp32 in TMEM;
-//                  tcgen05.commit releases stages.  Also allocates TMEM.
-//   epilogue     : tcgen05.ld the accumulator (thread <-> row) into ONE 32-register buffer that is reloaded as soon as
-//                  it has been converted; fused bias / time-embedding row vector / LayerNorm fold / SiLU|GELU|GEGLU /
-//                  scale / residual add / accumulate-into-destination (ControlNet zero-conv residual,
-//                  cldm/cldm.py:34-41) / dual store, rows written as coalesced 128-byte pieces through shared memory.
+// ea_gemm_kernel<BN, NG>: a CTA computes 128 x BN output tiles, one per CTA, or walking a tile list (persistent
+// launches: one CTA per SM).  Roles (288 threads, one CTA per SM):
+//   TMA producer (warp 8, one thread): A tile (128 rows x 64 halves, SWIZZLE_128B) and B tile (BN x 64) into
+//                  a `stages`-deep shared-memory ring, mbarrier-signalled.  For convolutions the A tile of filter tap
+//                  (kh,kw) is a 4-D box {64ch, bw, bh, bn} of the NHWC tensor shifted by (kh-1, kw-1); the zero padding
+//                  is TMA out-of-bounds fill, no im2col buffer exists.  W-operand loads carry an L2 evict-first hint
+//                  (see gemm_fill_group).
+//   consumers    (warp-groups 0-1): warp-group g issues wgmma.mma_async m64nBNk16 x4 per stage for tile rows
+//                  64g .. 64g+63, accumulating fp32 in registers, and releases each stage as soon as the next one's
+//                  MMAs are in flight.  The finished accumulator is staged row-major in shared memory (over the
+//                  drained ring) and the same 256 threads run the fused epilogue with one thread per tile row and the
+//                  two warp-groups on alternating 64-column groups: bias / time-embedding row vector / LayerNorm fold
+//                  / SiLU|GELU|GEGLU / scale / residual add / accumulate-into-destination (ControlNet zero-conv
+//                  residual, cldm/cldm.py:34-41) / dual store, rows written as coalesced 128-byte pieces through
+//                  shared memory.
 #include "ea_common.cuh"
 #include "ea_internal.h"
 
@@ -31,12 +29,22 @@ namespace ea {
 
 static constexpr int BM = 128;
 static constexpr int BK = 64;
-static constexpr int GEMM_THREADS = 192;
-// Warp roles: epilogue warps 0-3 (warp = TMEM lane quarter), TMA producer warp 4, MMA issuer (and
-// TMEM allocator) warp 5.  The two single-thread control warps get the HIGHEST warp ids because the
-// SM's warp arbiter prefers the highest eligible warp id: they must never queue behind epilogue
-// warps that are polling a barrier or storing a tile.
-static constexpr int W_TMA = 4, W_MMA = 5;
+// Warp roles: consumer warps 0-7 (two warp-groups), producer warp 8 (lane 0 issues TMA, lanes 2-31 walk the L2
+// prefetch hint).  Nine warps put three on one SM sub-partition, which caps every thread at 168 registers: the
+// 128-column accumulator (64 of them) fits, the 256-column one (128) spills inside the main loop, so the planner
+// never picks BN = 256 (it remains available as a forced width, ea_gemm_args.force_bn).
+static constexpr int GEMM_THREADS = 288;
+static constexpr int W_TMA = 8;
+static constexpr int EPI_WARPS = 8, EPI_THREADS = 256;
+// Shared memory: the stage ring, which after a tile's last MMA also holds the staged fp32 accumulator
+// ([BM][BN + 4]: the pad keeps the row-per-thread reads conflict-free) and 2 x 4 KB of store / residual staging per
+// consumer warp; then the barriers and the per-column vectors.
+static constexpr int GEMM_SMEM_RING = 216 * 1024;
+__host__ __device__ constexpr int gemm_epi_bytes(int bn) { return BM * (bn + 4) * 4 + 2 * 4096 * EPI_WARPS; }
+__host__ __device__ constexpr int gemm_region_bytes(int bn, int stages) {
+  return stages * (BM * BK * 2 + bn * BK * 2) > gemm_epi_bytes(bn) ? stages * (BM * BK * 2 + bn * BK * 2)
+                                                                    : gemm_epi_bytes(bn);
+}
 
 struct GemmKParams {
   int M, N;
@@ -68,7 +76,6 @@ struct GemmKParams {
   int splits;
   int kb_per_split;
   int no_spin;       // split-K without the sibling wait (concurrent streams)
-  int pair_release;  // stages are released to the producer two at a time (even stage count >= 4)
   float* ws;   // [tiles][splits][128][BN] fp32
   int* cnt;    // [tiles][2]: arrived, done (zero between launches)
   // LayerNorm fold (see ea_gemm_args): producer side / consumer side
@@ -82,7 +89,6 @@ struct GemmKParams {
   long long pf_bytes[EA_GEMM_MAX_PREFETCH];
   int pf_ctas;
   unsigned long long b_policy;   // L2 eviction hint of the W operand's TMA loads (0 = none)
-  int dbg_id;  // experiment builds (-DEA_GEMM_TIMING): launch ordinal for the chain stamps
 };
 
 // One launch can run up to GEMM_MAX_GROUPS independent problems of the SAME shape and launch plan (ea_gemm_grouped):
@@ -112,11 +118,6 @@ __device__ __forceinline__ void tile_origin(const GemmKParams& p, int tm, int& n
   w0 = (r - th * p.tiles_w) * p.bw;
 }
 
-// TMEM allocations are powers of two >= 32 columns
-__host__ __device__ __forceinline__ uint32_t tmem_cols_for(int bn) {
-  return bn <= 32 ? 32u : bn <= 64 ? 64u : bn <= 128 ? 128u : 256u;
-}
-
 struct RowInfo {
   long long m;   // global output row
   bool ok;
@@ -144,8 +145,8 @@ __device__ __forceinline__ RowInfo row_info(const GemmKParams& p, int tm, int r)
   return ri;
 }
 
-// named barrier over the 128 epilogue threads (warps 4-7); barrier 0 is __syncthreads
-__device__ __forceinline__ void epi_bar_sync() { asm volatile("bar.sync 1, 128;" ::: "memory"); }
+// named barrier over the 256 consumer threads (warps 0-7); barrier 0 is __syncthreads
+__device__ __forceinline__ void epi_bar_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
 
 __device__ __forceinline__ int ld_acquire_gpu(const int* p) {
   int v;
@@ -154,17 +155,16 @@ __device__ __forceinline__ int ld_acquire_gpu(const int* p) {
 }
 
 // LayerNorm fold, consumer side: one row's mean / rstd from the producer's per-32-column partial (sum, sumsq) pairs.
-// The loads of a batch of 16 partials are all issued before the first add - a plain loop compiled to one dependent L2
-// round trip per partial (10 for C = 320, 40 for C = 1280: 22 % of all stall samples of the GEGLU launch,
-// profiles/r02c_gemm_ncu_source_hot.txt).  The adds keep their fixed order, so the result stays deterministic.
+// The loads of a batch of 16 partials are all issued before the first add, so they are in flight together instead of
+// one dependent L2 round trip per partial (10 for C = 320, 40 for C = 1280).  The adds keep their fixed order, so the
+// result stays deterministic.
 // L2 prefetch of a later launch's weights (ea_gemm_args.prefetch): lanes `lane0 .. 31` of one warp in each of the first
 // pf_ctas CTAs walk the range line by line.  Issued before the dependency wait - weights are never produced by a
 // predecessor kernel - so HBM works on the next layer while this one computes from L2.
 __device__ __forceinline__ void l2_prefetch_hint(const GemmKParams& p, int cta, int lane, int lane0) {
   if (cta >= p.pf_ctas || lane < lane0) return;
-  // One 128-byte line per instruction through the load/store path (prefetch.global.L2).  NOT cp.async.bulk.prefetch:
-  // bulk prefetches queue in the SM's TMA unit in front of the launch's own operand loads (measured +0.05..0.18 ms per
-  // step, profiles/r02g_weight_prefetch_ab.txt).
+  // One 128-byte line per instruction through the load/store path (prefetch.global.L2), not cp.async.bulk.prefetch:
+  // bulk prefetches queue in the SM's TMA unit in front of the launch's own operand loads.
   const int nl = 32 - lane0;
 #pragma unroll 1
   for (int i = 0; i < EA_GEMM_MAX_PREFETCH; ++i) {
@@ -202,11 +202,10 @@ __device__ __noinline__ float act_call(float x, int act) {
   return act == EA_ACT_SILU ? silu_f(x) : gelu_erf_f(x);
 }
 
-// Coalesced tile stores.  A thread owns one accumulator row, so a direct store instruction touches 32
-// different rows (32 half-written sectors per instruction; measured: the epilogue of a 128x160 tile
-// took 4.9 us, longer than its 5-K-block main loop).  Instead every epilogue warp transposes its
-// 32 rows x 64 columns through a private 4 KB block of the (by then free) stage-0 A tile, XOR-swizzled
-// in 16-byte pieces, and writes each row's 128 bytes with 8 consecutive lanes.
+// Coalesced tile stores.  A thread owns one accumulator row, so a direct store instruction would touch 32
+// different rows (32 half-written sectors per instruction).  Instead every epilogue warp transposes its
+// 32 rows x 64 columns through a private 4 KB staging block in shared memory, XOR-swizzled in 16-byte pieces,
+// and writes each row's 128 bytes with 8 consecutive lanes.
 __device__ __forceinline__ void stage_put32(uint4* stg, int lane, int half, const uint4 (&o)[4]) {
 #pragma unroll
   for (int q = 0; q < 4; ++q) stg[lane * 8 + ((half * 4 + q) ^ (lane & 7))] = o[q];
@@ -216,9 +215,8 @@ __device__ __forceinline__ void stage_flush(const uint4* stg, int lane, ea_half*
                                             int col0, int pieces, int n_limit, long long lin_m0, int M) {
   __syncwarp();
   // Straight-line on purpose: the eight 16-byte pieces of a lane are loaded from the staging block first (8 LDS in
-  // flight) and stored with addresses advanced by a constant row stride.  The rolled version spent ~50 instructions
-  // per 16-byte store on 64-bit multiplies, shuffle-or-linear branches and reconvergence barriers - 22 % of all
-  // instructions a linear GEMM executed (profiles/r02c_gemm_ncu_source_hot.txt).
+  // flight) and stored with addresses advanced by a constant row stride (a rolled loop spends its instructions on
+  // 64-bit multiplies, shuffle-or-linear branches and reconvergence barriers per 16-byte store).
   const int piece = lane & 7, rsub = lane >> 3;
   const int col = col0 + piece * 8;
   const bool col_ok = piece < pieces && col < n_limit;
@@ -451,578 +449,6 @@ __device__ __forceinline__ void epilogue_chunk32(const GemmKParams& p, const Row
   }
 }
 
-#ifdef EA_GEMM_TIMING
-// Experiment build only: clock64 stamps of CTA (0,0,0): producer (slot 0: stage free, 1: TMA issued)
-// and MMA thread (2: operands landed, 3: MMAs + commit issued) for the first 64 K-blocks; slot 4/5 =
-// kernel entry / setup done, 6 = accumulator complete (epilogue start), 7 = epilogue done.
-__device__ long long ea_gemm_dbg[64 * 4 + 8];
-#define EA_GT(idx, slot) do { if (dbg_cta && (idx) < 64 && (threadIdx.x & 31) == 0) ea_gemm_dbg[(idx) * 4 + (slot)] = clock64(); } while (0)
-#define EA_GT1(slot) do { if (dbg_cta) ea_gemm_dbg[256 + (slot)] = clock64(); } while (0)
-// Launch-chain stamps (%globaltimer, ns) per launch ordinal: CTA (0,0,0): 0 entry, 1 setup done,
-// 2 released by griddepcontrol.wait, 3 first operands landed, 4 accumulator complete, 5 epilogue done;
-// grid-wide: 6 = earliest CTA entry, 7 = latest CTA exit.
-__device__ unsigned long long ea_gemm_chain[1024 * 8];
-__device__ __forceinline__ unsigned long long gtimer() {
-  unsigned long long t;
-  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-  return t;
-}
-#define EA_CH(slot) do { if (dbg_cta && p.dbg_id < 1024) ea_gemm_chain[p.dbg_id * 8 + (slot)] = gtimer(); } while (0)
-#else
-#define EA_GT(idx, slot) do {} while (0)
-#define EA_GT1(slot) do {} while (0)
-#define EA_CH(slot) do {} while (0)
-#endif
-
-// TWO = true: CTA pairs (cluster of 2 along M) run tcgen05.mma.cta_group::2 with M = 256; each CTA
-// stages its own A tile and HALF of the B tile (rows tn*BN + rank*BN/2 ...), the leader issues.
-template <bool TWO, int NG>
-__global__ void __launch_bounds__(GEMM_THREADS, 2)
-ea_gemm_kernel(const __grid_constant__ GemmLaunch<NG> L) {
-  // group of this CTA: blockIdx.z = group * splits + split (every group has the same shape and plan)
-  const int n_split0 = L.g[0].p.splits;
-  const int gi = NG == 1 ? 0 : (int)blockIdx.z / n_split0;
-  const int zsplit = NG == 1 ? (int)blockIdx.z : (int)blockIdx.z - gi * n_split0;
-  const GemmGroup& GG = L.g[gi];
-  const GemmKParams& p = GG.p;
-  const CUtensorMap& tmA0 = GG.tmA0;
-  const CUtensorMap& tmA1 = GG.tmA1;
-  const CUtensorMap& tmA2 = GG.tmA2;
-  const CUtensorMap& tmA3 = GG.tmA3;
-  const CUtensorMap& tmAx = GG.tmAx;
-  const CUtensorMap& tmB = GG.tmB;
-  extern __shared__ __align__(1024) uint8_t smem_raw[];
-  // carve: [stages] x (A 16 KB | B BN*128 B), then barriers
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
-                                             ~uintptr_t(1023));
-  const int a_bytes = BM * BK * 2;
-  const int b_rows = TWO ? (p.BN >> 1) : p.BN;     // B rows staged by THIS CTA
-  const int b_bytes = b_rows * BK * 2;
-  const int stage_bytes = a_bytes + b_bytes;
-  const uint32_t rank = TWO ? cluster_ctarank() : 0u;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + p.stages * stage_bytes);
-  uint64_t* empty_bar = full_bar + p.stages;
-  uint64_t* tmem_full_bar = empty_bar + p.stages;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_full_bar + 1);
-  float* cb = reinterpret_cast<float*>((reinterpret_cast<uintptr_t>(tmem_slot + 4) + 15) &
-                                       ~uintptr_t(15));   // [2][256] bias + time-emb row vector
-
-  pdl_launch_dependents();
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const int tm = blockIdx.x;
-  const int tn = blockIdx.y;
-#ifdef EA_GEMM_TIMING
-  const bool dbg_cta = blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0 && gi == 0;
-  if (threadIdx.x == 0) {
-    EA_GT1(0);
-    EA_CH(0);
-    if (p.dbg_id < 1024) atomicMin(&ea_gemm_chain[p.dbg_id * 8 + 6], gtimer());
-  }
-#endif
-  const int nkb_total = p.nkb_main + p.nkb_extra;
-  const int kb0 = zsplit * p.kb_per_split;
-  const int kb1 = min(nkb_total, kb0 + p.kb_per_split);
-
-  if (warp == W_TMA && lane == 0) {
-    tma_prefetch_desc(&tmA0);
-    tma_prefetch_desc(&tmB);
-    if (p.mode == EA_GEMM_CONV_S2 || p.mode == EA_GEMM_CONV_S2A) {
-      tma_prefetch_desc(&tmA1);
-      tma_prefetch_desc(&tmA2);
-      tma_prefetch_desc(&tmA3);
-    }
-    if (p.nkb_extra > 0) tma_prefetch_desc(&tmAx);
-  }
-  if (warp == W_TMA)   // lanes 2..31: the group's L2 prefetch hint, shared by the group's first CTAs
-    l2_prefetch_hint(p, (int)(blockIdx.x + gridDim.x * (blockIdx.y + gridDim.y * zsplit)), lane, 2);
-  if (warp == W_TMA && lane == 1) {
-    for (int s = 0; s < p.stages; ++s) {
-      mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
-    }
-    mbar_init(tmem_full_bar, 1);
-    fence_mbar_init();
-  }
-  if (warp == W_MMA) {
-    if (TWO) tmem_alloc_2cta(tmem_slot, tmem_cols_for(p.BN));
-    else tmem_alloc(tmem_slot, tmem_cols_for(p.BN));
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (TWO) cluster_sync_all();   // the peer's barriers exist before anything signals them
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-#ifdef EA_GEMM_TIMING
-  if (threadIdx.x == 0) EA_CH(1);
-#endif
-  pdl_wait();  // everything above overlapped the previous kernel's tail
-#ifdef EA_GEMM_TIMING
-  if (threadIdx.x == 0) { EA_GT1(1); EA_CH(2); }
-#endif
-
-  if (warp == W_TMA) {
-    // ============================ TMA producer ============================
-    // One thread; the loop body is kept to a handful of scalar instructions (no divisions: the
-    // filter-tap / channel-block position advances incrementally) — a single thread retires roughly
-    // one dependent instruction per 4-5 cycles, so every extra instruction here costs K-block rate.
-    if (lane == 0) {
-      int n0 = 0, h0 = 0, w0 = 0;
-      if (p.mode != EA_GEMM_LINEAR) tile_origin(p, tm, n0, h0, w0);
-      int stage = 0;
-      uint32_t phase = 0;
-      const int bcol = tn * p.BN + (int)rank * b_rows;
-      const bool pair_release = p.pair_release != 0;
-      uint8_t* sa = smem;
-      // TWO: both CTAs signal the LEADER's full barrier (it expects both CTAs' bytes)
-      const uint32_t full0 = TWO ? mapa_shared(smem_u32(&full_bar[0]), 0u) : 0u;
-      const uint32_t tx_bytes = TWO ? 2u * (uint32_t)stage_bytes : (uint32_t)stage_bytes;
-      if (p.mode == EA_GEMM_LINEAR) {
-        const int arow = tm * BM;
-        for (int kb = kb0; kb < kb1; ++kb) {
-          if (!pair_release || !(stage & 1)) mbar_wait(&empty_bar[pair_release ? (stage | 1) : stage], phase ^ 1u);
-          EA_GT(kb - kb0, 0);
-          if (!TWO || rank == 0) mbar_expect_tx(&full_bar[stage], tx_bytes);
-          if (TWO) {
-            tma_load_2d_2cta(sa, &tmA0, full0 + 8u * stage, kb * BK, arow);
-            tma_load_2d_2cta(sa + a_bytes, &tmB, full0 + 8u * stage, kb * BK, bcol);
-          } else {
-            tma_load_2d(sa, &tmA0, &full_bar[stage], kb * BK, arow);
-            tma_load_2d_hint(sa + a_bytes, &tmB, &full_bar[stage], kb * BK, bcol, p.b_policy);
-          }
-          EA_GT(kb - kb0, 1);
-          sa += stage_bytes;
-          if (++stage == p.stages) { stage = 0; phase ^= 1u; sa = smem; }
-        }
-      } else {
-        // position of kb0: tap (kh, kw) and channel block c0 of the main source
-        int tap = kb0 / p.cin_blocks;
-        int c0 = (kb0 - tap * p.cin_blocks) * BK;
-        int kh = tap / 3, kw = tap - kh * 3;
-        const int cin = p.cin_blocks * BK;
-        for (int kb = kb0; kb < kb1; ++kb) {
-          if (!pair_release || !(stage & 1)) mbar_wait(&empty_bar[pair_release ? (stage | 1) : stage], phase ^ 1u);
-          if (!TWO || rank == 0) mbar_expect_tx(&full_bar[stage], tx_bytes);
-          if (TWO) {
-            const uint32_t fb = full0 + 8u * stage;
-            if (kb >= p.nkb_main) tma_load_4d_2cta(sa, &tmAx, fb, (kb - p.nkb_main) * BK, w0, h0, n0);
-            else tma_load_4d_2cta(sa, &tmA0, fb, c0, w0 + kw - 1, h0 + kh - 1, n0);   // CONV_S1 only
-            tma_load_2d_2cta(sa + a_bytes, &tmB, fb, kb * BK, bcol);
-          } else if (kb >= p.nkb_main) {
-            // fused 1x1 skip convolution: centre tap of the raw block input
-            tma_load_4d(sa, &tmAx, &full_bar[stage], (kb - p.nkb_main) * BK, w0, h0, n0);
-          } else if (p.mode == EA_GEMM_CONV_S1) {
-            tma_load_4d(sa, &tmA0, &full_bar[stage], c0, w0 + kw - 1, h0 + kh - 1, n0);
-          } else {
-            // stride 2, pad 1: input row 2*oh + kh - 1 lives in phase ph = (kh != 1) at index oh + dh.
-            // stride 2, pad (0,1,0,1) (CONV_S2A, the VAE encoder's Downsample): input row 2*oh + kh lives in
-            // phase ph = (kh == 1) at index oh + (kh == 2); the bottom / right padding is TMA zero fill.
-            const bool asym = p.mode == EA_GEMM_CONV_S2A;
-            const int ph = asym ? (kh == 1 ? 1 : 0) : (kh == 1 ? 0 : 1);
-            const int dh = asym ? (kh == 2 ? 1 : 0) : (kh == 0 ? -1 : 0);
-            const int pw = asym ? (kw == 1 ? 1 : 0) : (kw == 1 ? 0 : 1);
-            const int dw = asym ? (kw == 2 ? 1 : 0) : (kw == 0 ? -1 : 0);
-            const int sel = ph * 2 + pw;
-            const CUtensorMap* m = sel == 0 ? &tmA0 : sel == 1 ? &tmA1 : sel == 2 ? &tmA2 : &tmA3;
-            tma_load_4d(sa, m, &full_bar[stage], c0, w0 + dw, h0 + dh, n0);
-          }
-          if (!TWO) tma_load_2d_hint(sa + a_bytes, &tmB, &full_bar[stage], kb * BK, bcol, p.b_policy);
-          c0 += BK;
-          if (c0 == cin) { c0 = 0; if (++kw == 3) { kw = 0; ++kh; } }
-          sa += stage_bytes;
-          if (++stage == p.stages) { stage = 0; phase ^= 1u; sa = smem; }
-        }
-      }
-    }
-  } else if (warp == W_MMA) {
-    // ============================ MMA issuer ==============================
-    // One thread; descriptors are advanced with 32-bit adds on the 16-byte-unit address field.
-    // The WHOLE warp runs this loop in warp-uniform control flow and one elected lane issues: the
-    // compiler then keeps the descriptors / addresses in uniform registers.  (Written as a
-    // single-lane branch the loop body compiled to ~110 scalar instructions per K-block with an
-    // ELECT/R2UR "waterfall" around every UTCHMMA, and this thread - not TMA or the tensor core -
-    // set the K-block rate at ~540 clk: tools/exp_gemm_timing.py, profiles/r01f.)
-    if (rank == 0) {
-      const uint32_t tb = __shfl_sync(0xffffffffu, tmem_base, 0);
-      const uint32_t idesc = umma_idesc(TWO ? 2 * BM : BM, (uint32_t)p.BN, 0, 0);
-      const uint64_t d0 = umma_desc_k_sw128(smem_u32(smem), 1024);   // stage 0, A tile
-      const uint32_t st16 = (uint32_t)stage_bytes >> 4, ab16 = (uint32_t)a_bytes >> 4;
-      const int stages = p.stages;
-      const bool pair_release = p.pair_release != 0;
-      uint64_t da = d0;
-      int stage = 0;
-      uint32_t phase = 0;
-      uint32_t acc = 0u;
-      for (int kb = kb0; kb < kb1; ++kb) {
-        mbar_wait(&full_bar[stage], phase);
-        tc_fence_after();
-        EA_GT(kb - kb0, 2);
-#ifdef EA_GEMM_TIMING
-        if (kb == kb0 && lane == 0) EA_CH(3);
-#endif
-        const uint64_t db = da + ab16;
-        const bool release = !pair_release || (stage & 1) || (kb + 1 == kb1);
-        uint64_t* ebar = &empty_bar[pair_release ? (stage | 1) : stage];
-        if (elect_one()) {
-          if (TWO) {
-            umma_f16_ss_2cta(tb, da, db, idesc, acc);
-            umma_f16_ss_2cta(tb, da + 2, db + 2, idesc, 1u);
-            umma_f16_ss_2cta(tb, da + 4, db + 4, idesc, 1u);
-            umma_f16_ss_2cta(tb, da + 6, db + 6, idesc, 1u);
-            if (release) umma_commit_2cta(ebar, (uint16_t)3);  // frees the stage(s) in BOTH CTAs
-          } else {
-            umma_f16_ss(tb, da, db, idesc, acc);
-            umma_f16_ss(tb, da + 2, db + 2, idesc, 1u);
-            umma_f16_ss(tb, da + 4, db + 4, idesc, 1u);
-            umma_f16_ss(tb, da + 6, db + 6, idesc, 1u);
-            if (release) umma_commit(ebar);  // frees the smem stage(s) when these MMAs retire
-          }
-        }
-        __syncwarp();
-        acc = 1u;
-        EA_GT(kb - kb0, 3);
-        da += st16;
-        if (++stage == stages) { stage = 0; phase ^= 1u; da = d0; }
-      }
-      if (elect_one()) {
-        if (TWO) umma_commit_2cta(tmem_full_bar, (uint16_t)3);
-        else umma_commit(tmem_full_bar);
-      }
-      __syncwarp();
-    }
-  } else {
-    // ============================== epilogue ==============================
-    const int wq = warp;                 // TMEM lane quarter
-    const int r = wq * 32 + lane;        // tile row owned by this thread
-    const int et = threadIdx.x;          // 0..127 among the epilogue threads
-    RowInfo ri = row_info(p, tm, r);
-    const int ncol0 = tn * p.BN;
-    const bool geglu = p.act == EA_ACT_GEGLU;
-    const int half_bn = p.BN >> 1;
-    // Fast path (the common case): while the main loop runs, these otherwise idle warps stage
-    // bias (+ the per-image time-embedding row vector) for the tile's columns in shared memory and
-    // pull the first residual chunk into registers, so that after the accumulator is complete the
-    // per-chunk work is TMEM load -> FMA -> 16-byte stores with the NEXT chunk's residual already in
-    // flight (before: four dependent global round trips per 32-column chunk, ~5400 clk per tile).
-    const int b_first = row_info(p, tm, 0).batch, b_last = row_info(p, tm, BM - 1).batch;
-    const bool fast = p.splits == 1 && !geglu && !p.out_f32 && !p.accumulate && !p.row_scale && (b_last - b_first) <= 1;
-    uint4 rres[8];   // next 64-column group of the residual (coalesced layout)
-    const long long lin_m0 = p.mode == EA_GEMM_LINEAR ? (long long)tm * BM + wq * 32 : -1;
-    const bool has_res = p.residual != nullptr;
-    // LayerNorm fold, consumer side: this row's mean / rstd from the producer's per-chunk partials (fixed
-    // summation order: deterministic), while the main loop runs.  out = acc * ln_r + ln_nm * g[n] + c[n].
-    const bool ln = p.ln_stats != nullptr;
-    float ln_r = 1.f, ln_nm = 0.f;
-    if (ln && ri.ok) ln_row_stats(p, ri.m, ln_r, ln_nm);
-    if (fast) {
-      for (int i = et; i < p.BN; i += 128) {
-        const int col = ncol0 + i;
-        float v0 = 0.f, v1 = 0.f;
-        if (col < p.N) {
-          const float bsum = p.bias ? __ldg(p.bias + col) : 0.f;
-          v0 = bsum + (p.rowvec ? __ldg(p.rowvec + (long long)b_first * p.rowvec_ld + col) : 0.f);
-          v1 = ln ? __ldg(p.ln_g + col)       // no row vector with the fold: the second slot carries g[n]
-                  : bsum + (p.rowvec ? __ldg(p.rowvec + (long long)b_last * p.rowvec_ld + col) : 0.f);
-        }
-        cb[i] = v0;
-        cb[256 + i] = v1;
-      }
-      if (has_res) residual_load64(rres, p.residual, p.ldr, lane, ri.m, ri.ok, ncol0, p.BN, p.N, lin_m0, p.M);
-      epi_bar_sync();
-    } else if (geglu && p.splits == 1) {
-      for (int i = et; i < p.BN; i += 128) {
-        const bool in = ncol0 + i < p.N;
-        cb[i] = (p.bias && in) ? __ldg(p.bias + ncol0 + i) : 0.f;
-        if (ln) cb[256 + i] = in ? __ldg(p.ln_g + ncol0 + i) : 0.f;
-      }
-      epi_bar_sync();
-    }
-    mbar_wait(tmem_full_bar, 0);
-    tc_fence_after();
-#ifdef EA_GEMM_TIMING
-    if (threadIdx.x == 0) { EA_GT1(6); EA_CH(4); }
-#endif
-    const uint32_t taddr = tmem_base + ((uint32_t)(wq * 32) << 16);
-    // accumulator complete => every MMA has retired and every TMA load was consumed: stage 0 is free
-    uint4* stg = reinterpret_cast<uint4*>(smem + wq * 4096);
-    uint4* stg2 = reinterpret_cast<uint4*>(smem + 16384 + wq * 4096);   // >= 2 stages of >= 18 KB exist
-    if (fast) {
-      const float* cbr = cb + ((!ln && ri.batch != b_first) ? 256 : 0);
-      // one 32-column chunk: residual hand-off, bias / activation / scale / residual, staging, flush
-      auto process = [&](uint32_t (&v)[32], const int c) {
-        const int n_first = ncol0 + c;
-        const int half = (c >> 5) & 1;
-        if (has_res && half == 0) {
-          // hand the prefetched group to its rows through the second staging block, then put the
-          // next group's loads in flight
-          const int piece = lane & 7, rsub = lane >> 3;
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            const int row = i * 4 + rsub;
-            stg2[row * 8 + (piece ^ (row & 7))] = rres[i];
-          }
-          __syncwarp();
-          if (c + 64 < p.BN)
-            residual_load64(rres, p.residual, p.ldr, lane, ri.m, ri.ok, n_first + 64, p.BN - c - 64, p.N, lin_m0, p.M);
-        }
-        {
-          float f[32];
-          if (ln) {
-#pragma unroll
-            for (int j = 0; j < 32; j += 4) {
-              const float4 b4 = *reinterpret_cast<const float4*>(cb + c + j);
-              const float4 g4 = *reinterpret_cast<const float4*>(cb + 256 + c + j);
-              f[j] = fmaf(__uint_as_float(v[j]), ln_r, fmaf(ln_nm, g4.x, b4.x));
-              f[j + 1] = fmaf(__uint_as_float(v[j + 1]), ln_r, fmaf(ln_nm, g4.y, b4.y));
-              f[j + 2] = fmaf(__uint_as_float(v[j + 2]), ln_r, fmaf(ln_nm, g4.z, b4.z));
-              f[j + 3] = fmaf(__uint_as_float(v[j + 3]), ln_r, fmaf(ln_nm, g4.w, b4.w));
-            }
-          } else {
-#pragma unroll
-            for (int j = 0; j < 32; j += 4) {
-              const float4 b4 = *reinterpret_cast<const float4*>(cbr + c + j);
-              f[j] = __uint_as_float(v[j]) + b4.x;
-              f[j + 1] = __uint_as_float(v[j + 1]) + b4.y;
-              f[j + 2] = __uint_as_float(v[j + 2]) + b4.z;
-              f[j + 3] = __uint_as_float(v[j + 3]) + b4.w;
-            }
-          }
-#ifndef EA_EPI_TWO_BUFFERS
-          // v is dead from here on: the next chunk's tcgen05.ld reuses its registers (see the persistent kernel)
-          if (c + 32 < p.BN) tmem_ld32(taddr + (uint32_t)(c + 32), v);
-#endif
-          if (p.act == EA_ACT_SILU) {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) f[j] = act_call(f[j], EA_ACT_SILU);
-          } else if (p.act == EA_ACT_GELU) {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) f[j] = gelu_erf_f(f[j]);
-          }
-          if (p.out_scale != 1.0f) {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) f[j] *= p.out_scale;
-          }
-#pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            const int slot = lane * 8 + ((half * 4 + q) ^ (lane & 7));
-            if (has_res) {
-              const uint4 rc = stg2[slot];
-              const float2 a = ea_unpack2(rc.x), b = ea_unpack2(rc.y), cc = ea_unpack2(rc.z), d = ea_unpack2(rc.w);
-              f[q * 8 + 0] += a.x; f[q * 8 + 1] += a.y; f[q * 8 + 2] += b.x; f[q * 8 + 3] += b.y;
-              f[q * 8 + 4] += cc.x; f[q * 8 + 5] += cc.y; f[q * 8 + 6] += d.x; f[q * 8 + 7] += d.y;
-            }
-            stg[slot] = make_uint4(ea_pack2(f[q * 8 + 0], f[q * 8 + 1]), ea_pack2(f[q * 8 + 2], f[q * 8 + 3]),
-                                   ea_pack2(f[q * 8 + 4], f[q * 8 + 5]), ea_pack2(f[q * 8 + 6], f[q * 8 + 7]));
-          }
-          if (p.rowstats_out) {
-            // LayerNorm fold, producer side: this row's (sum, sum of squares) over the chunk's 32 stored values
-            float s0 = 0.f, s1 = 0.f, q0 = 0.f, q1 = 0.f;
-#pragma unroll
-            for (int j = 0; j < 32; j += 2) {
-              s0 += f[j]; q0 = fmaf(f[j], f[j], q0);
-              s1 += f[j + 1]; q1 = fmaf(f[j + 1], f[j + 1], q1);
-            }
-            if (ri.ok && n_first < p.N) p.rowstats_out[(size_t)(n_first >> 5) * p.M + ri.m] = make_float2(s0 + s1, q0 + q1);
-          }
-        }
-        if (half == 1 || c + 32 >= p.BN)
-          stage_flush(stg, lane, p.out, p.ldo, p.out2, p.ldo2, ri.m, ri.ok, n_first - half * 32,
-                      half == 1 ? 8 : 4, p.N, lin_m0, p.M);
-      };
-      // TMEM loads are double-buffered: the next chunk's tcgen05.ld is in flight while this chunk is
-      // converted and stored (one warp per SM sub-partition: nothing else hides the load latency)
-      // (one copy of the chunk body: vb is moved into va instead of instantiating `process` twice)
-#ifdef EA_EPI_TWO_BUFFERS
-      uint32_t va[32], vb[32];
-      tmem_ld32(taddr, vb);
-      for (int c = 0; c < p.BN; c += 32) {
-        tmem_ld_wait();
-#pragma unroll
-        for (int j = 0; j < 32; ++j) va[j] = vb[j];
-        if (c + 32 < p.BN) tmem_ld32(taddr + (uint32_t)(c + 32), vb);
-        process(va, c);
-      }
-#else
-      uint32_t va[32];
-      tmem_ld32(taddr, va);
-      for (int c = 0; c < p.BN; c += 32) {
-        tmem_ld_wait();
-        process(va, c);
-      }
-#endif
-    } else
-    if (p.splits == 1) {
-      if (geglu) {
-        // tile columns: [0, BN/2) = value half, [BN/2, BN) = gate half (weights pre-interleaved)
-        for (int c = 0; c < half_bn; c += 32) {
-          uint32_t xv[32], gv[32];
-          tmem_ld32(taddr + (uint32_t)c, xv);
-          tmem_ld32(taddr + (uint32_t)(half_bn + c), gv);
-          tmem_ld_wait();
-          float fx[32], fg[32];
-#pragma unroll
-          for (int j = 0; j < 32; ++j) { fx[j] = __uint_as_float(xv[j]); fg[j] = __uint_as_float(gv[j]); }
-          uint4 o[4];
-          epilogue_geglu32(cb, half_bn, c, fx, fg, o, ln, ln_r, ln_nm);
-          const int half = (c >> 5) & 1;
-          stage_put32(stg, lane, half, o);
-          if (half == 1 || c + 32 >= half_bn)
-            stage_flush(stg, lane, p.out, p.ldo, nullptr, 0, ri.m, ri.ok, (ncol0 >> 1) + c - half * 32,
-                        half == 1 ? 8 : 4, p.N >> 1, lin_m0, p.M);
-        }
-      } else {
-        for (int c = 0; c < p.BN; c += 32) {
-          uint32_t v[32];
-          tmem_ld32(taddr + (uint32_t)c, v);
-          tmem_ld_wait();
-          float f[32];
-#pragma unroll
-          for (int j = 0; j < 32; ++j) f[j] = __uint_as_float(v[j]);
-          epilogue_chunk32(p, ri, ncol0 + c, f);
-          __syncwarp();
-        }
-      }
-    } else {
-      // ---- split-K: publish the fp32 partial tile, wait for the sibling splits, then every
-      //      split CTA reduces and finishes a 1/splits share of the tile's (row, 32-col) units.
-      const int tile_id = tn * gridDim.x + tm;
-      float* wtile = p.ws + (size_t)tile_id * p.splits * (BM * p.BN);
-      float* mine = wtile + (size_t)zsplit * (BM * p.BN);
-      for (int c = 0; c < p.BN; c += 32) {
-        uint32_t v[32];
-        tmem_ld32(taddr + (uint32_t)c, v);
-        tmem_ld_wait();
-        float4* dst = reinterpret_cast<float4*>(mine + (size_t)r * p.BN + c);
-#pragma unroll
-        for (int j = 0; j < 8; ++j)
-          __stcg(dst + j, make_float4(__uint_as_float(v[4 * j]), __uint_as_float(v[4 * j + 1]),
-                                      __uint_as_float(v[4 * j + 2]), __uint_as_float(v[4 * j + 3])));
-      }
-      __threadfence();
-      epi_bar_sync();
-      int* cnt = p.cnt + 2 * tile_id;
-      bool take_all = false;   // no_spin: the LAST split CTA to arrive finishes the whole tile
-      if (p.no_spin) {
-        if (et == 0) *reinterpret_cast<volatile int*>(cb) = atomicAdd(cnt, 1);
-        epi_bar_sync();
-        take_all = *reinterpret_cast<volatile int*>(cb) == p.splits - 1;
-        epi_bar_sync();
-      } else {
-        if (et == 0) {
-          atomicAdd(cnt, 1);
-          uint32_t spins = 0;
-          while (ld_acquire_gpu(cnt) < p.splits) {
-            __nanosleep(40);
-            if (++spins > (1u << 24)) { asm volatile("trap;"); }
-          }
-        }
-        epi_bar_sync();
-      }
-      __threadfence();
-      if (!p.no_spin || take_all) {
-      const int chunks = geglu ? (half_bn >> 5) : (p.BN >> 5);
-      const int units = BM * chunks;
-      const int u0 = take_all ? 0 : (int)(((long long)units * zsplit) / p.splits);
-      const int u1 = take_all ? units : (int)(((long long)units * (zsplit + 1)) / p.splits);
-      // Stage 1 (all 128 threads, float4 granularity, loads of the sibling partials unrolled for
-      // memory-level parallelism) sums this CTA's share into the now-idle pipeline smem; stage 2
-      // runs the fused epilogue on whole 32-column units.  Pieces of <= 128 units (<= 35 KB, the pipeline
-      // stages hold >= 36 KB): every epilogue thread owns one unit in stage 2 (pieces of 64 left half of
-      // them idle and needed twice as many serialized piece rounds: the fix-up of a 128-wide, 3-way split
-      // tile took 20 us, profiles/r01p_exp_step_chain_gemm_in_context.txt).
-      const int segs = geglu ? 2 : 1;                 // 32-float segments per unit (value | gate)
-      const int ustride = segs * 32 + 4;              // padded floats per unit in smem
-      float* stage = reinterpret_cast<float*>(smem);
-      const size_t split_stride = (size_t)BM * p.BN;
-      for (int ub = u0; ub < u1; ub += 128) {
-        const int nu = min(128, u1 - ub);
-        const int nvec4 = nu * segs * 8;
-        for (int idx = et; idx < nvec4; idx += 128) {
-          const int ul = idx / (segs * 8);
-          const int rem = idx - ul * (segs * 8);
-          const int seg = rem >> 3, q = rem & 7;
-          const int u = ub + ul;
-          const int rr = u & (BM - 1);
-          const int c = ((u >> 7) << 5) + seg * half_bn * (geglu ? 1 : 0);
-          const float4* src = reinterpret_cast<const float4*>(wtile + (size_t)rr * p.BN + c) + q;
-          float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
-          int sidx = 0;
-          for (; sidx + 4 <= p.splits; sidx += 4) {
-            float4 v0 = __ldcg(src + (size_t)(sidx + 0) * (split_stride >> 2));
-            float4 v1 = __ldcg(src + (size_t)(sidx + 1) * (split_stride >> 2));
-            float4 v2 = __ldcg(src + (size_t)(sidx + 2) * (split_stride >> 2));
-            float4 v3 = __ldcg(src + (size_t)(sidx + 3) * (split_stride >> 2));
-            acc.x += v0.x; acc.y += v0.y; acc.z += v0.z; acc.w += v0.w;
-            acc.x += v1.x; acc.y += v1.y; acc.z += v1.z; acc.w += v1.w;
-            acc.x += v2.x; acc.y += v2.y; acc.z += v2.z; acc.w += v2.w;
-            acc.x += v3.x; acc.y += v3.y; acc.z += v3.z; acc.w += v3.w;
-          }
-          for (; sidx < p.splits; ++sidx) {
-            float4 v0 = __ldcg(src + (size_t)sidx * (split_stride >> 2));
-            acc.x += v0.x; acc.y += v0.y; acc.z += v0.z; acc.w += v0.w;
-          }
-          *reinterpret_cast<float4*>(stage + ul * ustride + seg * 32 + q * 4) = acc;
-        }
-        epi_bar_sync();
-        if (et < nu) {
-          const int u = ub + et;
-          const int rr = u & (BM - 1);
-          const int c = (u >> 7) << 5;
-          RowInfo r2 = row_info(p, tm, rr);
-          const float4* sp = reinterpret_cast<const float4*>(stage + et * ustride);
-          float f[32];
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            float4 v = sp[j];
-            f[4 * j] = v.x; f[4 * j + 1] = v.y; f[4 * j + 2] = v.z; f[4 * j + 3] = v.w;
-          }
-          if (geglu) {
-            float fg[32];
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              float4 v = sp[8 + j];
-              fg[4 * j] = v.x; fg[4 * j + 1] = v.y; fg[4 * j + 2] = v.z; fg[4 * j + 3] = v.w;
-            }
-            epilogue_geglu32_direct(p, r2, ncol0, half_bn, c, f, fg);
-          } else {
-            epilogue_chunk32(p, r2, ncol0 + c, f);
-          }
-        }
-        epi_bar_sync();
-      }
-      epi_bar_sync();
-      if (et == 0) {
-        if (take_all) {
-          cnt[0] = 0;
-        } else {
-          int old = atomicAdd(cnt + 1, 1);
-          if (old == p.splits - 1) {  // last finisher: re-arm the counters for the next launch
-            cnt[0] = 0;
-            cnt[1] = 0;
-          }
-        }
-      }
-      }  // !no_spin || take_all
-    }
-  }
-
-#ifdef EA_GEMM_TIMING
-  if (threadIdx.x == 0) {
-    EA_GT1(7);
-    EA_CH(5);
-    if (p.dbg_id < 1024) atomicMax(&ea_gemm_chain[p.dbg_id * 8 + 7], gtimer());
-  }
-#endif
-  tc_fence_before();
-  __syncthreads();
-  if (TWO) cluster_sync_all();   // the leader's MMAs read the peer's shared memory until the end
-  if (warp == W_MMA) {
-    tc_fence_after();
-    if (TWO) tmem_dealloc_2cta(tmem_base, tmem_cols_for(p.BN));
-    else tmem_dealloc(tmem_base, tmem_cols_for(p.BN));
-  }
-}
-
 // ------------------------------- host side ---------------------------------
 
 static int encode_2d(CUtensorMap* m, const void* base, uint64_t inner, uint64_t outer,
@@ -1060,397 +486,337 @@ static void conv_geometry(int H, int W, int& bw, int& bh, int& bn) {
   bn = 128 / (bw * bh);
 }
 
-// ---- persistent variant ---------------------------------------------------------------------------
-// The DEFAULT kernel for every launch without split-K / CTA pairs (the 8-warp form; EA_GEMM_PERSIST=0|1|2 and
-// ea_gemm_args.force_persistent override; validated bit-for-bit against the one-tile kernel by
-// tests/test_gpu_gemm_persistent.py).  One CTA per SM walks the tile list (tile -> (tm, tn) with tm
-// fastest, so CTAs working side by side share their weight tile in L2) with TWO TMEM accumulators: the
-// epilogue warps drain tile i while the MMA warp already accumulates tile i+1, the TMA ring runs across
-// tile boundaries, and barrier setup / TMEM allocation / the dependency wait are paid once per SM instead
-// of once per tile.  Scope: no CTA pairs, no split-K, half output, epilogue = fast path or GEGLU (the host
-// only selects this kernel when every tile qualifies).
-// EPI_WG = 2 (force_persistent = 2 / EA_GEMM_PERSIST=2): EIGHT epilogue warps, two per SM sub-partition - the
-// second warp-group takes every other 64-column group of the accumulator.  The one-warp-per-sub-partition
-// epilogue is instruction-latency bound (3-5 us per tile, profiles/r01p_exp_step_chain_gemm_in_context.txt);
-// a second warp on the same scheduler hides it, also for grids of a single wave.
-// Registers (EPI_WG = 2): an SM sub-partition holds 16384 registers = 512 per lane.  Ten warps put three on some
-// sub-partition, which caps every thread at 168 (a launch at 200 is refused: cudaErrorLaunchOutOfResources, round 2
-// session 6) and spilled the double-buffered TMEM drain.  So the block is THREE full warp-groups - epilogue warps
-// 0-7, control warp-group 8-11 (TMA, MMA, two idle warps) - launched at 168 registers, and `setmaxnreg` moves the
-// budget: control warps shrink to 40, epilogue warps grow to 232 (2 x 232 + 40 = 3 x 168, the launch allocation).
-// The pool setmaxnreg draws from is what the LAUNCH allocated (384 x 168), not the whole file: control + 2 x epilogue
-// <= 3 x 168 = 504 per lane.  48 / 232 asked for 1024 registers the pool never had: launch failure / hang (session 8).
-#ifndef EA_PREG_CTRL
-#define EA_PREG_CTRL 40
-#define EA_PREG_EPI 232
-#endif
-static_assert(EA_PREG_CTRL + 2 * EA_PREG_EPI <= 504, "setmaxnreg budget exceeds the launch allocation");
-#ifdef EA_PERSIST_LEGACY_LAYOUT   // A/B: 320 threads, 168 registers for every warp
-template <int EPI_WG> struct PersistShape {
-  static constexpr int kThreads = 64 + 128 * EPI_WG;
-  static constexpr bool kSetMaxNReg = false;
-};
-#else
-template <int EPI_WG> struct PersistShape {
-  static constexpr int kThreads = EPI_WG == 2 ? 384 : 192;
-  static constexpr bool kSetMaxNReg = EPI_WG == 2;
-};
-#endif
-template <int EPI_WG, int NG>
-__global__ void __launch_bounds__(PersistShape<EPI_WG>::kThreads, 1)
-ea_gemm_persistent_kernel(const __grid_constant__ GemmLaunch<NG> L, const int tiles_per_group, const int m_tiles,
-                          const int n_groups) {
-  // the tile list runs over (group, tile): every group has the same shape and plan; `p` below = the shared fields
-  // (group 0), each tile re-binds `p` / the tensor maps to its own group
-  const GemmKParams& p = L.g[0].p;
-  const int num_tiles = tiles_per_group * (NG == 1 ? 1 : n_groups);
-#define EA_PERSIST_TILE_GROUP()                                                    \
+// 32 staged accumulator values of tile row r, columns [c, c + 32)
+__device__ __forceinline__ void acc_ld32(const float* accs, int ld, int r, int c, uint32_t (&v)[32]) {
+  const float4* src = reinterpret_cast<const float4*>(accs + (size_t)r * ld + c);
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    const float4 f = src[j];
+    v[4 * j] = __float_as_uint(f.x); v[4 * j + 1] = __float_as_uint(f.y);
+    v[4 * j + 2] = __float_as_uint(f.z); v[4 * j + 3] = __float_as_uint(f.w);
+  }
+}
+
+// The tile list runs over (group, split, tn, tm) with tm fastest, so CTAs working side by side share their weight
+// tile in L2; every group has the same shape and plan.  `p` below = the shared fields (group 0), each tile re-binds
+// `p` / the tensor maps to its own group.
+#define EA_GEMM_TILE()                                                             \
   const int gi = NG == 1 ? 0 : tile / tiles_per_group;                             \
   const int gtile = NG == 1 ? tile : tile - gi * tiles_per_group;                  \
+  const int zsplit = gtile / mn_tiles;                                             \
+  const int mn = gtile - zsplit * mn_tiles;                                        \
   const GemmGroup& GG = L.g[gi];                                                   \
   const GemmKParams& p = GG.p;                                                     \
-  const int tm = gtile % m_tiles, tn = gtile / m_tiles;
+  const int tm = mn % m_tiles, tn = mn / m_tiles;                                  \
+  const int kb0 = zsplit * p.kb_per_split;                                         \
+  const int kb1 = min(nkb, kb0 + p.kb_per_split);
+
+template <int BN, int NG>
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
+ea_gemm_kernel(const __grid_constant__ GemmLaunch<NG> L, const int tiles_per_group, const int m_tiles,
+               const int n_groups) {
+  const GemmKParams& p0 = L.g[0].p;
+  const int n_tiles = (p0.N + BN - 1) / BN;
+  const int mn_tiles = m_tiles * n_tiles;
+  const int num_tiles = tiles_per_group * (NG == 1 ? 1 : n_groups);
+  const int nkb = p0.nkb_main + p0.nkb_extra;
+  constexpr int a_bytes = BM * BK * 2;
+  constexpr int stage_bytes = a_bytes + BN * BK * 2;
+  constexpr int ACC_LD = BN + 4;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                              ~uintptr_t(1023));
-  const int a_bytes = BM * BK * 2;
-  const int b_bytes = p.BN * BK * 2;
-  const int stage_bytes = a_bytes + b_bytes;
-  constexpr int EPI_WARPS = 4 * EPI_WG, EPI_THREADS = 128 * EPI_WG;
-  constexpr int PW_TMA = EPI_WARPS, PW_MMA = EPI_WARPS + 1;   // control warps keep the highest warp ids
-  // carve: [stages] x (A | B), 4 KB store staging + 4 KB residual staging per epilogue warp, barriers,
-  // TMEM slot, bias
-  uint8_t* stg_base = smem + p.stages * stage_bytes;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(stg_base + 2 * 4096 * EPI_WARPS);
-  uint64_t* empty_bar = full_bar + p.stages;
-  uint64_t* tfull_bar = empty_bar + p.stages;      // [2] accumulator complete
-  uint64_t* tempty_bar = tfull_bar + 2;            // [2] accumulator drained (one arrival per epilogue warp)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty_bar + 2);
-  float* cb = reinterpret_cast<float*>((reinterpret_cast<uintptr_t>(tmem_slot + 4) + 15) &
-                                       ~uintptr_t(15));   // [2 tile parities][2][256]
+  float* accs = reinterpret_cast<float*>(smem);
+  uint8_t* stg_base = smem + BM * ACC_LD * 4;
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + gemm_region_bytes(BN, p0.stages));
+  uint64_t* empty_bar = full_bar + p0.stages;
+  uint64_t* epi_done = empty_bar + p0.stages;       // the staged accumulator has been consumed: the ring is free
+  float* cb = reinterpret_cast<float*>(epi_done + 2);   // [2 tile parities][2][256] per-column vectors
 
   pdl_launch_dependents();
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const int nkb = p.nkb_main + p.nkb_extra;
-  const uint32_t acc_cols = tmem_cols_for(p.BN);
 
-  if (warp == PW_TMA && lane == 0) {
+  if (warp == W_TMA && lane == 0) {
     const int g0 = NG == 1 ? 0 : min((int)blockIdx.x / tiles_per_group, n_groups - 1);
     tma_prefetch_desc(&L.g[g0].tmA0);
     tma_prefetch_desc(&L.g[g0].tmB);
-    if (p.mode == EA_GEMM_CONV_S2 || p.mode == EA_GEMM_CONV_S2A) {
+    if (p0.mode == EA_GEMM_CONV_S2 || p0.mode == EA_GEMM_CONV_S2A) {
       tma_prefetch_desc(&L.g[g0].tmA1);
       tma_prefetch_desc(&L.g[g0].tmA2);
       tma_prefetch_desc(&L.g[g0].tmA3);
     }
-    if (p.nkb_extra > 0) tma_prefetch_desc(&L.g[g0].tmAx);
+    if (p0.nkb_extra > 0) tma_prefetch_desc(&L.g[g0].tmAx);
   }
-  if (warp == PW_TMA) {   // lanes 2..31: every group's L2 prefetch hint, shared by all CTAs of the launch
+  if (warp == W_TMA) {   // lanes 2..31: every group's L2 prefetch hint, shared by the launch's first CTAs
     for (int g = 0; g < (NG == 1 ? 1 : n_groups); ++g) l2_prefetch_hint(L.g[g].p, (int)blockIdx.x, lane, 2);
   }
-  if (warp == PW_TMA && lane == 1) {
-    for (int s = 0; s < p.stages; ++s) {
+  if (warp == W_TMA && lane == 1) {
+    for (int s = 0; s < p0.stages; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
+      mbar_init(&empty_bar[s], EPI_WARPS);
     }
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(&tfull_bar[b], 1);
-      mbar_init(&tempty_bar[b], EPI_WARPS);
-    }
+    mbar_init(epi_done, EPI_WARPS);
     fence_mbar_init();
   }
-  if (warp == PW_MMA) tmem_alloc(tmem_slot, 2u * acc_cols);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  // no code is shared between the two register budgets after this point: each role branch changes its own
+
   if (warp >= EPI_WARPS) {
-  if (PersistShape<EPI_WG>::kSetMaxNReg) asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(EA_PREG_CTRL));
-  pdl_wait();
-  if (warp == PW_TMA) {
+    pdl_wait();
+    if (lane != 0) return;
     // ============================ TMA producer ============================
-    if (lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
-      uint8_t* sa = smem;
-      const int cin = p.cin_blocks * BK;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        EA_PERSIST_TILE_GROUP()
-        const CUtensorMap& tmA0 = GG.tmA0;
-        const CUtensorMap& tmA1 = GG.tmA1;
-        const CUtensorMap& tmA2 = GG.tmA2;
-        const CUtensorMap& tmA3 = GG.tmA3;
-        const CUtensorMap& tmAx = GG.tmAx;
-        const CUtensorMap& tmB = GG.tmB;
-        const int bcol = tn * p.BN;
-        if (p.mode == EA_GEMM_LINEAR) {
-          const int arow = tm * BM;
-          for (int kb = 0; kb < nkb; ++kb) {
-            mbar_wait(&empty_bar[stage], phase ^ 1u);
-            mbar_expect_tx(&full_bar[stage], (uint32_t)stage_bytes);
-            tma_load_2d(sa, &tmA0, &full_bar[stage], kb * BK, arow);
-            tma_load_2d_hint(sa + a_bytes, &tmB, &full_bar[stage], kb * BK, bcol, p.b_policy);
-            sa += stage_bytes;
-            if (++stage == p.stages) { stage = 0; phase ^= 1u; sa = smem; }
-          }
-        } else {
-          int n0, h0, w0;
-          tile_origin(p, tm, n0, h0, w0);
-          int c0 = 0, kh = 0, kw = 0;
-          for (int kb = 0; kb < nkb; ++kb) {
-            mbar_wait(&empty_bar[stage], phase ^ 1u);
-            mbar_expect_tx(&full_bar[stage], (uint32_t)stage_bytes);
-            if (kb >= p.nkb_main) {
-              tma_load_4d(sa, &tmAx, &full_bar[stage], (kb - p.nkb_main) * BK, w0, h0, n0);
-            } else if (p.mode == EA_GEMM_CONV_S1) {
-              tma_load_4d(sa, &tmA0, &full_bar[stage], c0, w0 + kw - 1, h0 + kh - 1, n0);
-            } else {
-              const bool asym = p.mode == EA_GEMM_CONV_S2A;
-              const int ph = asym ? (kh == 1 ? 1 : 0) : (kh == 1 ? 0 : 1);
-              const int dh = asym ? (kh == 2 ? 1 : 0) : (kh == 0 ? -1 : 0);
-              const int pw = asym ? (kw == 1 ? 1 : 0) : (kw == 1 ? 0 : 1);
-              const int dw = asym ? (kw == 2 ? 1 : 0) : (kw == 0 ? -1 : 0);
-              const int sel = ph * 2 + pw;
-              const CUtensorMap* m = sel == 0 ? &tmA0 : sel == 1 ? &tmA1 : sel == 2 ? &tmA2 : &tmA3;
-              tma_load_4d(sa, m, &full_bar[stage], c0, w0 + dw, h0 + dh, n0);
-            }
-            tma_load_2d_hint(sa + a_bytes, &tmB, &full_bar[stage], kb * BK, bcol, p.b_policy);
-            c0 += BK;
-            if (c0 == cin) { c0 = 0; if (++kw == 3) { kw = 0; ++kh; } }
-            sa += stage_bytes;
-            if (++stage == p.stages) { stage = 0; phase ^= 1u; sa = smem; }
-          }
-        }
-      }
-    }
-  } else if (warp == PW_MMA) {
-    // ============================ MMA issuer ==============================
-    const uint32_t tb = __shfl_sync(0xffffffffu, tmem_base, 0);
-    const uint32_t idesc = umma_idesc(BM, (uint32_t)p.BN, 0, 0);
-    const uint64_t d0 = umma_desc_k_sw128(smem_u32(smem), 1024);
-    const uint32_t st16 = (uint32_t)stage_bytes >> 4, ab16 = (uint32_t)a_bytes >> 4;
-    const int stages = p.stages;
-    uint64_t da = d0;
+    // One thread; the loop body is kept to a handful of scalar instructions (no divisions: the filter-tap /
+    // channel-block position advances incrementally).
     int stage = 0;
     uint32_t phase = 0;
-    int abuf = 0;
-    uint32_t aphase = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-      mbar_wait(&tempty_bar[abuf], aphase ^ 1u);      // the epilogue has drained this accumulator
-      tc_fence_after();
-      const uint32_t td = tb + (uint32_t)abuf * acc_cols;
-      uint32_t acc = 0u;
-      for (int kb = 0; kb < nkb; ++kb) {
-        mbar_wait(&full_bar[stage], phase);
-        tc_fence_after();
-        const uint64_t db = da + ab16;
-        if (elect_one()) {
-          umma_f16_ss(td, da, db, idesc, acc);
-          umma_f16_ss(td, da + 2, db + 2, idesc, 1u);
-          umma_f16_ss(td, da + 4, db + 4, idesc, 1u);
-          umma_f16_ss(td, da + 6, db + 6, idesc, 1u);
-          umma_commit(&empty_bar[stage]);
-        }
-        __syncwarp();
-        acc = 1u;
-        da += st16;
-        if (++stage == stages) { stage = 0; phase ^= 1u; da = d0; }
-      }
-      if (elect_one()) umma_commit(&tfull_bar[abuf]);
-      __syncwarp();
-      abuf ^= 1;
-      if (abuf == 0) aphase ^= 1u;
-    }
-  }
-  } else {
-    // ============================== epilogue ==============================
-    if (PersistShape<EPI_WG>::kSetMaxNReg) asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(EA_PREG_EPI));
-    pdl_wait();
-    const int wq = warp & 3;             // TMEM lane quarter = warp id mod 4
-    const int wg = warp >> 2;            // epilogue warp-group: owns the 64-column groups gi with gi % EPI_WG == wg
-    const int r = wq * 32 + lane;
-    const int et = threadIdx.x;          // 0 .. EPI_THREADS-1
-    const bool geglu = p.act == EA_ACT_GEGLU;
-    const int half_bn = p.BN >> 1;
-    uint4* stg = reinterpret_cast<uint4*>(stg_base + warp * 4096);
-    uint4* stg2 = reinterpret_cast<uint4*>(stg_base + 4096 * EPI_WARPS + warp * 4096);
-    constexpr int GSTEP = 64 * EPI_WG;   // column distance between two groups of one warp-group
-    int abuf = 0, it = 0;
-    uint32_t fphase = 0;
+    uint8_t* sa = smem;
+    int it = 0;
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
-      EA_PERSIST_TILE_GROUP()
-      const bool has_res = p.residual != nullptr;
-      const RowInfo ri = row_info(p, tm, r);
-      const int ncol0 = tn * p.BN;
-      float* cbt = cb + (it & 1) * 512;
-      const long long lin_m0 = p.mode == EA_GEMM_LINEAR ? (long long)tm * BM + wq * 32 : -1;
-      const int b_first = row_info(p, tm, 0).batch, b_last = row_info(p, tm, BM - 1).batch;
-      uint4 rres[8];
-      // LayerNorm fold, consumer side (see ea_gemm_kernel)
-      const bool ln = p.ln_stats != nullptr;
-      float ln_r = 1.f, ln_nm = 0.f;
-      if (ln && ri.ok) ln_row_stats(p, ri.m, ln_r, ln_nm);
-      if (!geglu) {
-        for (int i = et; i < p.BN; i += EPI_THREADS) {
-          const int col = ncol0 + i;
-          float v0 = 0.f, v1 = 0.f;
-          if (col < p.N) {
-            const float bsum = p.bias ? __ldg(p.bias + col) : 0.f;
-            v0 = bsum + (p.rowvec ? __ldg(p.rowvec + (long long)b_first * p.rowvec_ld + col) : 0.f);
-            v1 = ln ? __ldg(p.ln_g + col)
-                    : bsum + (p.rowvec ? __ldg(p.rowvec + (long long)b_last * p.rowvec_ld + col) : 0.f);
-          }
-          cbt[i] = v0;
-          cbt[256 + i] = v1;
+      EA_GEMM_TILE()
+      const CUtensorMap& tmA0 = GG.tmA0;
+      const CUtensorMap& tmA1 = GG.tmA1;
+      const CUtensorMap& tmA2 = GG.tmA2;
+      const CUtensorMap& tmA3 = GG.tmA3;
+      const CUtensorMap& tmAx = GG.tmAx;
+      const CUtensorMap& tmB = GG.tmB;
+      if (it > 0) mbar_wait(epi_done, (uint32_t)((it - 1) & 1));   // the previous tile's accumulator is read
+      const int bcol = tn * BN;
+      if (p.mode == EA_GEMM_LINEAR) {
+        const int arow = tm * BM;
+        for (int kb = kb0; kb < kb1; ++kb) {
+          mbar_wait(&empty_bar[stage], phase ^ 1u);
+          mbar_expect_tx(&full_bar[stage], (uint32_t)stage_bytes);
+          tma_load_2d(sa, &tmA0, &full_bar[stage], kb * BK, arow);
+          tma_load_2d_hint(sa + a_bytes, &tmB, &full_bar[stage], kb * BK, bcol, p.b_policy);
+          sa += stage_bytes;
+          if (++stage == p.stages) { stage = 0; phase ^= 1u; sa = smem; }
         }
-        if (has_res && wg * 64 < p.BN)
-          residual_load64(rres, p.residual, p.ldr, lane, ri.m, ri.ok, ncol0 + wg * 64, p.BN - wg * 64, p.N, lin_m0, p.M);
       } else {
-        for (int i = et; i < p.BN; i += EPI_THREADS) {
-          const bool in = ncol0 + i < p.N;
-          cbt[i] = (p.bias && in) ? __ldg(p.bias + ncol0 + i) : 0.f;
-          if (ln) cbt[256 + i] = in ? __ldg(p.ln_g + ncol0 + i) : 0.f;
+        int n0, h0, w0;
+        tile_origin(p, tm, n0, h0, w0);
+        // position of kb0: tap (kh, kw) and channel block c0 of the main source
+        int tap = kb0 / p.cin_blocks;
+        int c0 = (kb0 - tap * p.cin_blocks) * BK;
+        int kh = tap / 3, kw = tap - kh * 3;
+        const int cin = p.cin_blocks * BK;
+        for (int kb = kb0; kb < kb1; ++kb) {
+          mbar_wait(&empty_bar[stage], phase ^ 1u);
+          mbar_expect_tx(&full_bar[stage], (uint32_t)stage_bytes);
+          if (kb >= p.nkb_main) {
+            // fused 1x1 skip convolution: centre tap of the raw block input
+            tma_load_4d(sa, &tmAx, &full_bar[stage], (kb - p.nkb_main) * BK, w0, h0, n0);
+          } else if (p.mode == EA_GEMM_CONV_S1) {
+            tma_load_4d(sa, &tmA0, &full_bar[stage], c0, w0 + kw - 1, h0 + kh - 1, n0);
+          } else {
+            // stride 2, pad 1: input row 2*oh + kh - 1 lives in phase ph = (kh != 1) at index oh + dh.
+            // stride 2, pad (0,1,0,1) (CONV_S2A, the VAE encoder's Downsample): input row 2*oh + kh lives in
+            // phase ph = (kh == 1) at index oh + (kh == 2); the bottom / right padding is TMA zero fill.
+            const bool asym = p.mode == EA_GEMM_CONV_S2A;
+            const int ph = asym ? (kh == 1 ? 1 : 0) : (kh == 1 ? 0 : 1);
+            const int dh = asym ? (kh == 2 ? 1 : 0) : (kh == 0 ? -1 : 0);
+            const int pw = asym ? (kw == 1 ? 1 : 0) : (kw == 1 ? 0 : 1);
+            const int dw = asym ? (kw == 2 ? 1 : 0) : (kw == 0 ? -1 : 0);
+            const int sel = ph * 2 + pw;
+            const CUtensorMap* m = sel == 0 ? &tmA0 : sel == 1 ? &tmA1 : sel == 2 ? &tmA2 : &tmA3;
+            tma_load_4d(sa, m, &full_bar[stage], c0, w0 + dw, h0 + dh, n0);
+          }
+          tma_load_2d_hint(sa + a_bytes, &tmB, &full_bar[stage], kb * BK, bcol, p.b_policy);
+          c0 += BK;
+          if (c0 == cin) { c0 = 0; if (++kw == 3) { kw = 0; ++kh; } }
+          sa += stage_bytes;
+          if (++stage == p.stages) { stage = 0; phase ^= 1u; sa = smem; }
         }
       }
-      asm volatile("bar.sync 1, %0;" ::"n"(EPI_THREADS) : "memory");
-      mbar_wait(&tfull_bar[abuf], fphase);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + ((uint32_t)(wq * 32) << 16) + (uint32_t)abuf * acc_cols;
-      if (!geglu) {
-        const float* cbr = cbt + ((!ln && ri.batch != b_first) ? 256 : 0);
-        // this warp-group's chunks: both halves of the 64-column groups wg, wg + EPI_WG, ...; the next chunk's
-        // tcgen05.ld is in flight while the current one is converted and stored.  ONE copy of the chunk body on
-        // purpose (32 register moves per chunk): alternating two register buffers needs two copies of the ~1500
-        // instruction body, which no longer fit the 32 KB L1.5 instruction cache - measured +0.25 ms per step
-        // (profiles/r02e_ab_epilogue.txt).
-        auto next_chunk = [&](int c) { return ((c & 32) == 0 && c + 32 < p.BN) ? c + 32 : (c & ~63) + GSTEP; };
-        auto process = [&](uint32_t (&v)[32], const int c, const int nc) {
-          const int n_first = ncol0 + c;
-          const int half = (c >> 5) & 1;
-          if (has_res && half == 0) {
-            const int piece = lane & 7, rsub = lane >> 3;
+    }
+    return;
+  }
+
+  // ================================ consumers =================================
+  pdl_wait();
+  const int wg = warp >> 2;            // MMA: tile rows 64 wg ..; epilogue: the 64-column groups gi with gi % 2 == wg
+  const int wq = warp & 3;
+  const int r = wq * 32 + lane;        // epilogue: tile row owned by this thread
+  const int et = threadIdx.x;          // 0 .. EPI_THREADS-1
+  constexpr int GSTEP = 128;           // column distance between two 64-column groups of one warp-group
+  uint4* stg = reinterpret_cast<uint4*>(stg_base + warp * 4096);
+  uint4* stg2 = reinterpret_cast<uint4*>(stg_base + 4096 * EPI_WARPS + warp * 4096);
+  const uint32_t smem0 = smem_u32(smem);
+  int stage = 0;
+  uint32_t phase = 0;
+  int it = 0;
+  for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
+    EA_GEMM_TILE()
+    const bool geglu = p.act == EA_ACT_GEGLU;
+    const int half_bn = BN >> 1;
+    const bool has_res = p.residual != nullptr;
+    const RowInfo ri = row_info(p, tm, r);
+    const int ncol0 = tn * BN;
+    float* cbt = cb + (it & 1) * 512;
+    const long long lin_m0 = p.mode == EA_GEMM_LINEAR ? (long long)tm * BM + wq * 32 : -1;
+    const int b_first = row_info(p, tm, 0).batch, b_last = row_info(p, tm, BM - 1).batch;
+    // Fast path (the common case): before the main loop, bias (+ the per-image time-embedding row vector) for the
+    // tile's columns is staged in shared memory and the first residual chunk is pulled into registers, so that the
+    // per-chunk work after the main loop is load -> FMA -> 16-byte stores with the NEXT chunk's residual in flight.
+    const bool fast = p.splits == 1 && !geglu && !p.out_f32 && !p.accumulate && !p.row_scale && (b_last - b_first) <= 1;
+    uint4 rres[8];   // next 64-column group of the residual (coalesced layout)
+    // LayerNorm fold, consumer side: this row's mean / rstd from the producer's per-chunk partials (fixed
+    // summation order: deterministic).  out = acc * ln_r + ln_nm * g[n] + c[n].
+    const bool ln = p.ln_stats != nullptr;
+    float ln_r = 1.f, ln_nm = 0.f;
+    if (ln && ri.ok) ln_row_stats(p, ri.m, ln_r, ln_nm);
+    if (fast) {
+      for (int i = et; i < BN; i += EPI_THREADS) {
+        const int col = ncol0 + i;
+        float v0 = 0.f, v1 = 0.f;
+        if (col < p.N) {
+          const float bsum = p.bias ? __ldg(p.bias + col) : 0.f;
+          v0 = bsum + (p.rowvec ? __ldg(p.rowvec + (long long)b_first * p.rowvec_ld + col) : 0.f);
+          v1 = ln ? __ldg(p.ln_g + col)       // no row vector with the fold: the second slot carries g[n]
+                  : bsum + (p.rowvec ? __ldg(p.rowvec + (long long)b_last * p.rowvec_ld + col) : 0.f);
+        }
+        cbt[i] = v0;
+        cbt[256 + i] = v1;
+      }
+      if (has_res && wg * 64 < BN)
+        residual_load64(rres, p.residual, p.ldr, lane, ri.m, ri.ok, ncol0 + wg * 64, BN - wg * 64, p.N, lin_m0, p.M);
+    } else if (geglu && p.splits == 1) {
+      for (int i = et; i < BN; i += EPI_THREADS) {
+        const bool in = ncol0 + i < p.N;
+        cbt[i] = (p.bias && in) ? __ldg(p.bias + ncol0 + i) : 0.f;
+        if (ln) cbt[256 + i] = in ? __ldg(p.ln_g + ncol0 + i) : 0.f;
+      }
+    }
+
+    // ---- main loop: the stage of K-block kb is released once the MMAs of kb + 1 are in flight
+    {
+      float acc[BN / 2];
 #pragma unroll
-            for (int i = 0; i < 8; ++i) {
-              const int row = i * 4 + rsub;
-              stg2[row * 8 + (piece ^ (row & 7))] = rres[i];
-            }
-            __syncwarp();
-            if (c + GSTEP < p.BN)
-              residual_load64(rres, p.residual, p.ldr, lane, ri.m, ri.ok, n_first + GSTEP, p.BN - c - GSTEP, p.N, lin_m0, p.M);
+      for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+      int prev = -1;
+      for (int kb = kb0; kb < kb1; ++kb) {
+        mbar_wait(&full_bar[stage], phase);
+        const uint32_t sa = smem0 + (uint32_t)(stage * stage_bytes);
+        const uint64_t da = gmma_desc_k_sw128(sa + (uint32_t)(wg * 64 * 128), 1024);
+        const uint64_t db = gmma_desc_k_sw128(sa + (uint32_t)a_bytes, 1024);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < 4; ++k) Wgmma<BN>::ss(acc, da + 2 * k, db + 2 * k, 1u);
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (prev >= 0) {
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&empty_bar[prev]);
+        }
+        prev = stage;
+        if (++stage == p.stages) { stage = 0; phase ^= 1u; }
+      }
+      wgmma_wait<0>();
+      wgmma_fence_regs(acc);
+      if (prev >= 0) {
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty_bar[prev]);
+      }
+      // every TMA load of this tile has landed and, once both warp-groups are here, every MMA has retired: the ring
+      // is free for the accumulator
+      epi_bar_sync();
+      const int r0 = wg * 64 + wq * 16 + (lane >> 2);
+      float* d0 = accs + (size_t)r0 * ACC_LD + 2 * (lane & 3);
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {
+        *reinterpret_cast<float2*>(d0 + 8 * j) = make_float2(acc[4 * j], acc[4 * j + 1]);
+        *reinterpret_cast<float2*>(d0 + 8 * ACC_LD + 8 * j) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+      }
+    }
+    epi_bar_sync();
+
+    if (fast) {
+      const float* cbr = cbt + ((!ln && ri.batch != b_first) ? 256 : 0);
+      // this warp-group's chunks: both halves of the 64-column groups wg, wg + 2, ...
+      auto next_chunk = [&](int c) { return ((c & 32) == 0 && c + 32 < BN) ? c + 32 : (c & ~63) + GSTEP; };
+      for (int c = wg * 64; c < BN; c = next_chunk(c)) {
+        uint32_t v[32];
+        acc_ld32(accs, ACC_LD, r, c, v);
+        const int n_first = ncol0 + c;
+        const int half = (c >> 5) & 1;
+        if (has_res && half == 0) {
+          // hand the prefetched group to its rows through the second staging block, then put the next group's
+          // loads in flight
+          const int piece = lane & 7, rsub = lane >> 3;
+#pragma unroll
+          for (int i = 0; i < 8; ++i) {
+            const int row = i * 4 + rsub;
+            stg2[row * 8 + (piece ^ (row & 7))] = rres[i];
           }
-          {
-            float f[32];
-            if (ln) {
+          __syncwarp();
+          if (c + GSTEP < BN)
+            residual_load64(rres, p.residual, p.ldr, lane, ri.m, ri.ok, n_first + GSTEP, BN - c - GSTEP, p.N, lin_m0, p.M);
+        }
+        float f[32];
+        if (ln) {
 #pragma unroll
-              for (int j = 0; j < 32; j += 4) {
-                const float4 b4 = *reinterpret_cast<const float4*>(cbt + c + j);
-                const float4 g4 = *reinterpret_cast<const float4*>(cbt + 256 + c + j);
-                f[j] = fmaf(__uint_as_float(v[j]), ln_r, fmaf(ln_nm, g4.x, b4.x));
-                f[j + 1] = fmaf(__uint_as_float(v[j + 1]), ln_r, fmaf(ln_nm, g4.y, b4.y));
-                f[j + 2] = fmaf(__uint_as_float(v[j + 2]), ln_r, fmaf(ln_nm, g4.z, b4.z));
-                f[j + 3] = fmaf(__uint_as_float(v[j + 3]), ln_r, fmaf(ln_nm, g4.w, b4.w));
-              }
-            } else {
-#pragma unroll
-              for (int j = 0; j < 32; j += 4) {
-                const float4 b4 = *reinterpret_cast<const float4*>(cbr + c + j);
-                f[j] = __uint_as_float(v[j]) + b4.x;
-                f[j + 1] = __uint_as_float(v[j + 1]) + b4.y;
-                f[j + 2] = __uint_as_float(v[j + 2]) + b4.z;
-                f[j + 3] = __uint_as_float(v[j + 3]) + b4.w;
-              }
-            }
-#ifndef EA_EPI_TWO_BUFFERS
-            // v is dead from here on: the next chunk's tcgen05.ld goes into the SAME registers and is in flight behind
-            // the activation / pack / staging / flush below - no second buffer, no 32 register moves per chunk
-            if (nc < p.BN) tmem_ld32(taddr + (uint32_t)nc, v);
-#endif
-            if (p.act == EA_ACT_SILU) {
-#pragma unroll
-              for (int j = 0; j < 32; ++j) f[j] = act_call(f[j], EA_ACT_SILU);
-            } else if (p.act == EA_ACT_GELU) {
-#pragma unroll
-              for (int j = 0; j < 32; ++j) f[j] = gelu_erf_f(f[j]);
-            }
-            if (p.out_scale != 1.0f) {
-#pragma unroll
-              for (int j = 0; j < 32; ++j) f[j] *= p.out_scale;
-            }
-#pragma unroll
-            for (int q = 0; q < 4; ++q) {
-              const int slot = lane * 8 + ((half * 4 + q) ^ (lane & 7));
-              if (has_res) {
-                const uint4 rc = stg2[slot];
-                const float2 a = ea_unpack2(rc.x), b = ea_unpack2(rc.y), cc = ea_unpack2(rc.z), d = ea_unpack2(rc.w);
-                f[q * 8 + 0] += a.x; f[q * 8 + 1] += a.y; f[q * 8 + 2] += b.x; f[q * 8 + 3] += b.y;
-                f[q * 8 + 4] += cc.x; f[q * 8 + 5] += cc.y; f[q * 8 + 6] += d.x; f[q * 8 + 7] += d.y;
-              }
-              stg[slot] = make_uint4(ea_pack2(f[q * 8 + 0], f[q * 8 + 1]), ea_pack2(f[q * 8 + 2], f[q * 8 + 3]),
-                                     ea_pack2(f[q * 8 + 4], f[q * 8 + 5]), ea_pack2(f[q * 8 + 6], f[q * 8 + 7]));
-            }
-            if (p.rowstats_out) {   // LayerNorm fold, producer side
-              float s0 = 0.f, s1 = 0.f, q0 = 0.f, q1 = 0.f;
-#pragma unroll
-              for (int j = 0; j < 32; j += 2) {
-                s0 += f[j]; q0 = fmaf(f[j], f[j], q0);
-                s1 += f[j + 1]; q1 = fmaf(f[j + 1], f[j + 1], q1);
-              }
-              if (ri.ok && n_first < p.N) p.rowstats_out[(size_t)(n_first >> 5) * p.M + ri.m] = make_float2(s0 + s1, q0 + q1);
-            }
+          for (int j = 0; j < 32; j += 4) {
+            const float4 b4 = *reinterpret_cast<const float4*>(cbt + c + j);
+            const float4 g4 = *reinterpret_cast<const float4*>(cbt + 256 + c + j);
+            f[j] = fmaf(__uint_as_float(v[j]), ln_r, fmaf(ln_nm, g4.x, b4.x));
+            f[j + 1] = fmaf(__uint_as_float(v[j + 1]), ln_r, fmaf(ln_nm, g4.y, b4.y));
+            f[j + 2] = fmaf(__uint_as_float(v[j + 2]), ln_r, fmaf(ln_nm, g4.z, b4.z));
+            f[j + 3] = fmaf(__uint_as_float(v[j + 3]), ln_r, fmaf(ln_nm, g4.w, b4.w));
           }
-          if (half == 1 || c + 32 >= p.BN)
-            stage_flush(stg, lane, p.out, p.ldo, p.out2, p.ldo2, ri.m, ri.ok, n_first - half * 32,
-                        half == 1 ? 8 : 4, p.N, lin_m0, p.M);
-        };
-        int c = wg * 64;
-#ifdef EA_EPI_TWO_BUFFERS   // A/B: the previous form (second register buffer, copied per chunk)
-        uint32_t va[32], vb[32];
-        if (c < p.BN) tmem_ld32(taddr + (uint32_t)c, vb);
-        while (c < p.BN) {
-          tmem_ld_wait();
+        } else {
 #pragma unroll
-          for (int j = 0; j < 32; ++j) va[j] = vb[j];
-          const int nc = next_chunk(c);
-          if (nc < p.BN) tmem_ld32(taddr + (uint32_t)nc, vb);
-          process(va, c, nc);
-          c = nc;
+          for (int j = 0; j < 32; j += 4) {
+            const float4 b4 = *reinterpret_cast<const float4*>(cbr + c + j);
+            f[j] = __uint_as_float(v[j]) + b4.x;
+            f[j + 1] = __uint_as_float(v[j + 1]) + b4.y;
+            f[j + 2] = __uint_as_float(v[j + 2]) + b4.z;
+            f[j + 3] = __uint_as_float(v[j + 3]) + b4.w;
+          }
         }
-#else
-        uint32_t va[32];
-        if (c < p.BN) tmem_ld32(taddr + (uint32_t)c, va);
-        while (c < p.BN) {
-          tmem_ld_wait();
-          const int nc = next_chunk(c);
-          process(va, c, nc);
-          c = nc;
-        }
-#endif
-      } else if (EPI_WG == 1) {
-        for (int c = 0; c < half_bn; c += 32) {
-          uint32_t xv[32], gv[32];
-          tmem_ld32(taddr + (uint32_t)c, xv);
-          tmem_ld32(taddr + (uint32_t)(half_bn + c), gv);
-          tmem_ld_wait();
-          float fx[32], fg[32];
+        if (p.act == EA_ACT_SILU) {
 #pragma unroll
-          for (int j = 0; j < 32; ++j) { fx[j] = __uint_as_float(xv[j]); fg[j] = __uint_as_float(gv[j]); }
-          uint4 o[4];
-          epilogue_geglu32(cbt, half_bn, c, fx, fg, o, ln, ln_r, ln_nm);
-          const int half = (c >> 5) & 1;
-          stage_put32(stg, lane, half, o);
-          if (half == 1 || c + 32 >= half_bn)
-            stage_flush(stg, lane, p.out, p.ldo, nullptr, 0, ri.m, ri.ok, (ncol0 >> 1) + c - half * 32,
-                        half == 1 ? 8 : 4, p.N >> 1, lin_m0, p.M);
+          for (int j = 0; j < 32; ++j) f[j] = act_call(f[j], EA_ACT_SILU);
+        } else if (p.act == EA_ACT_GELU) {
+#pragma unroll
+          for (int j = 0; j < 32; ++j) f[j] = gelu_erf_f(f[j]);
         }
-      } else {
-        // two warp-groups: the 32-column output chunks alternate between them, each flushed on its own
-        for (int c = wg * 32; c < half_bn; c += 32 * EPI_WG) {
+        if (p.out_scale != 1.0f) {
+#pragma unroll
+          for (int j = 0; j < 32; ++j) f[j] *= p.out_scale;
+        }
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+          const int slot = lane * 8 + ((half * 4 + q) ^ (lane & 7));
+          if (has_res) {
+            const uint4 rc = stg2[slot];
+            const float2 a = ea_unpack2(rc.x), b = ea_unpack2(rc.y), cc = ea_unpack2(rc.z), d = ea_unpack2(rc.w);
+            f[q * 8 + 0] += a.x; f[q * 8 + 1] += a.y; f[q * 8 + 2] += b.x; f[q * 8 + 3] += b.y;
+            f[q * 8 + 4] += cc.x; f[q * 8 + 5] += cc.y; f[q * 8 + 6] += d.x; f[q * 8 + 7] += d.y;
+          }
+          stg[slot] = make_uint4(ea_pack2(f[q * 8 + 0], f[q * 8 + 1]), ea_pack2(f[q * 8 + 2], f[q * 8 + 3]),
+                                 ea_pack2(f[q * 8 + 4], f[q * 8 + 5]), ea_pack2(f[q * 8 + 6], f[q * 8 + 7]));
+        }
+        if (p.rowstats_out) {
+          // LayerNorm fold, producer side: this row's (sum, sum of squares) over the chunk's 32 stored values
+          float s0 = 0.f, s1 = 0.f, q0 = 0.f, q1 = 0.f;
+#pragma unroll
+          for (int j = 0; j < 32; j += 2) {
+            s0 += f[j]; q0 = fmaf(f[j], f[j], q0);
+            s1 += f[j + 1]; q1 = fmaf(f[j + 1], f[j + 1], q1);
+          }
+          if (ri.ok && n_first < p.N) p.rowstats_out[(size_t)(n_first >> 5) * p.M + ri.m] = make_float2(s0 + s1, q0 + q1);
+        }
+        if (half == 1 || c + 32 >= BN)
+          stage_flush(stg, lane, p.out, p.ldo, p.out2, p.ldo2, ri.m, ri.ok, n_first - half * 32,
+                      half == 1 ? 8 : 4, p.N, lin_m0, p.M);
+      }
+    } else if (p.splits == 1) {
+      if (geglu) {
+        // tile columns: [0, BN/2) = value half, [BN/2, BN) = gate half (weights pre-interleaved); the 32-column
+        // output chunks alternate between the two warp-groups, each flushed on its own
+        for (int c = wg * 32; c < half_bn; c += 64) {
           uint32_t xv[32], gv[32];
-          tmem_ld32(taddr + (uint32_t)c, xv);
-          tmem_ld32(taddr + (uint32_t)(half_bn + c), gv);
-          tmem_ld_wait();
+          acc_ld32(accs, ACC_LD, r, c, xv);
+          acc_ld32(accs, ACC_LD, r, half_bn + c, gv);
           float fx[32], fg[32];
 #pragma unroll
           for (int j = 0; j < 32; ++j) { fx[j] = __uint_as_float(xv[j]); fg[j] = __uint_as_float(gv[j]); }
@@ -1462,164 +828,213 @@ ea_gemm_persistent_kernel(const __grid_constant__ GemmLaunch<NG> L, const int ti
           else
             stage_flush(stg, lane, p.out, p.ldo, nullptr, 0, ri.m, ri.ok, (ncol0 >> 1) + c, 4, p.N >> 1, lin_m0, p.M);
         }
+      } else {
+        for (int c = wg * 32; c < BN; c += 64) {
+          uint32_t v[32];
+          acc_ld32(accs, ACC_LD, r, c, v);
+          float f[32];
+#pragma unroll
+          for (int j = 0; j < 32; ++j) f[j] = __uint_as_float(v[j]);
+          epilogue_chunk32(p, ri, ncol0 + c, f);
+          __syncwarp();
+        }
       }
-      // every tcgen05.ld of this accumulator has completed (tmem_ld_wait above): hand it back
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tempty_bar[abuf]);
-      abuf ^= 1;
-      if (abuf == 0) fphase ^= 1u;
+    } else {
+      // ---- split-K: publish the fp32 partial tile, wait for the sibling splits, then every
+      //      split CTA reduces and finishes a 1/splits share of the tile's (row, 32-col) units.
+      const int tile_id = tn * m_tiles + tm;
+      float* wtile = p.ws + (size_t)tile_id * p.splits * (BM * BN);
+      float* mine = wtile + (size_t)zsplit * (BM * BN);
+      for (int c = wg * 32; c < BN; c += 64) {
+        uint32_t v[32];
+        acc_ld32(accs, ACC_LD, r, c, v);
+        float4* dst = reinterpret_cast<float4*>(mine + (size_t)r * BN + c);
+#pragma unroll
+        for (int j = 0; j < 8; ++j)
+          __stcg(dst + j, make_float4(__uint_as_float(v[4 * j]), __uint_as_float(v[4 * j + 1]),
+                                      __uint_as_float(v[4 * j + 2]), __uint_as_float(v[4 * j + 3])));
+      }
+      __threadfence();
+      epi_bar_sync();
+      int* cnt = p.cnt + 2 * tile_id;
+      bool take_all = false;   // no_spin: the LAST split CTA to arrive finishes the whole tile
+      volatile int* flag = reinterpret_cast<volatile int*>(cbt);
+      if (p.no_spin) {
+        if (et == 0) *flag = atomicAdd(cnt, 1);
+        epi_bar_sync();
+        take_all = *flag == p.splits - 1;
+        epi_bar_sync();
+      } else {
+        if (et == 0) {
+          atomicAdd(cnt, 1);
+          uint32_t spins = 0;
+          while (ld_acquire_gpu(cnt) < p.splits) {
+            __nanosleep(40);
+            if (++spins > (1u << 24)) { asm volatile("trap;"); }
+          }
+        }
+        epi_bar_sync();
+      }
+      __threadfence();
+      if (!p.no_spin || take_all) {
+        const int chunks = geglu ? (half_bn >> 5) : (BN >> 5);
+        const int units = BM * chunks;
+        const int u0 = take_all ? 0 : (int)(((long long)units * zsplit) / p.splits);
+        const int u1 = take_all ? units : (int)(((long long)units * (zsplit + 1)) / p.splits);
+        // Stage 1 (all consumer threads, float4 granularity, loads of the sibling partials unrolled for
+        // memory-level parallelism) sums this CTA's share into the (published, now dead) accumulator staging;
+        // stage 2 runs the fused epilogue on whole 32-column units, one per thread.
+        const int segs = geglu ? 2 : 1;                 // 32-float segments per unit (value | gate)
+        const int ustride = segs * 32 + 4;              // padded floats per unit in smem
+        float* stage_f = accs;
+        const size_t split_stride = (size_t)BM * BN;
+        for (int ub = u0; ub < u1; ub += EPI_THREADS) {
+          const int nu = min(EPI_THREADS, u1 - ub);
+          const int nvec4 = nu * segs * 8;
+          for (int idx = et; idx < nvec4; idx += EPI_THREADS) {
+            const int ul = idx / (segs * 8);
+            const int rem = idx - ul * (segs * 8);
+            const int seg = rem >> 3, q = rem & 7;
+            const int u = ub + ul;
+            const int rr = u & (BM - 1);
+            const int c = ((u >> 7) << 5) + seg * half_bn * (geglu ? 1 : 0);
+            const float4* src = reinterpret_cast<const float4*>(wtile + (size_t)rr * BN + c) + q;
+            float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+            int sidx = 0;
+            for (; sidx + 4 <= p.splits; sidx += 4) {
+              float4 v0 = __ldcg(src + (size_t)(sidx + 0) * (split_stride >> 2));
+              float4 v1 = __ldcg(src + (size_t)(sidx + 1) * (split_stride >> 2));
+              float4 v2 = __ldcg(src + (size_t)(sidx + 2) * (split_stride >> 2));
+              float4 v3 = __ldcg(src + (size_t)(sidx + 3) * (split_stride >> 2));
+              acc.x += v0.x; acc.y += v0.y; acc.z += v0.z; acc.w += v0.w;
+              acc.x += v1.x; acc.y += v1.y; acc.z += v1.z; acc.w += v1.w;
+              acc.x += v2.x; acc.y += v2.y; acc.z += v2.z; acc.w += v2.w;
+              acc.x += v3.x; acc.y += v3.y; acc.z += v3.z; acc.w += v3.w;
+            }
+            for (; sidx < p.splits; ++sidx) {
+              float4 v0 = __ldcg(src + (size_t)sidx * (split_stride >> 2));
+              acc.x += v0.x; acc.y += v0.y; acc.z += v0.z; acc.w += v0.w;
+            }
+            *reinterpret_cast<float4*>(stage_f + ul * ustride + seg * 32 + q * 4) = acc;
+          }
+          epi_bar_sync();
+          if (et < nu) {
+            const int u = ub + et;
+            const int rr = u & (BM - 1);
+            const int c = (u >> 7) << 5;
+            RowInfo r2 = row_info(p, tm, rr);
+            const float4* sp = reinterpret_cast<const float4*>(stage_f + et * ustride);
+            float f[32];
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+              float4 v = sp[j];
+              f[4 * j] = v.x; f[4 * j + 1] = v.y; f[4 * j + 2] = v.z; f[4 * j + 3] = v.w;
+            }
+            if (geglu) {
+              float fg[32];
+#pragma unroll
+              for (int j = 0; j < 8; ++j) {
+                float4 v = sp[8 + j];
+                fg[4 * j] = v.x; fg[4 * j + 1] = v.y; fg[4 * j + 2] = v.z; fg[4 * j + 3] = v.w;
+              }
+              epilogue_geglu32_direct(p, r2, ncol0, half_bn, c, f, fg);
+            } else {
+              epilogue_chunk32(p, r2, ncol0 + c, f);
+            }
+          }
+          epi_bar_sync();
+        }
+        epi_bar_sync();
+        if (et == 0) {
+          if (take_all) {
+            cnt[0] = 0;
+          } else {
+            int old = atomicAdd(cnt + 1, 1);
+            if (old == p.splits - 1) {  // last finisher: re-arm the counters for the next launch
+              cnt[0] = 0;
+              cnt[1] = 0;
+            }
+          }
+        }
+      }  // !no_spin || take_all
     }
+    // the staged accumulator has been read: hand the ring back to the producer (its next loads are async-proxy
+    // writes over what this thread wrote and read through the generic proxy)
+    fence_proxy_async();
+    __syncwarp();
+    if (lane == 0) mbar_arrive(epi_done);
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == PW_MMA) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 2u * acc_cols);
-  }
-#undef EA_PERSIST_TILE_GROUP
 }
+#undef EA_GEMM_TILE
 
 // ---- launch planner -------------------------------------------------------------------
-// Picks (BN, stages, CTAs/SM, split-K) for one problem from a small cycle model: per K-block a CTA
-// needs max(MMA time, its share of chip bandwidth, TMA latency / stages in flight); small-M layers
-// (8x8 / 16x16 latents: M = 128 / 512) are weight-streaming bound, so K is split across CTAs until
-// every SM has one deep pipeline, and the partial tiles are combined in-kernel (see the epilogue).
-struct GemmPlan { int BN, stages, splits, kbps, occ; double cost; int two; };
+// Picks (BN, stages, split-K) for one problem from a small cycle model: per K-block a CTA needs max(MMA time,
+// its share of chip bandwidth, TMA latency / stages in flight); small-M layers (8x8 / 16x16 latents: M = 128 / 512)
+// are weight-streaming bound, so K is split across CTAs until every SM has one deep pipeline, and the partial
+// tiles are combined in-kernel (see the epilogue).
+struct GemmPlan { int BN, stages, splits, kbps, occ; double cost; };
 
-// Constants fitted (tools/fit/fit_planner.py, log-RMSE 0.14) to the tile sweep of the step's dominant
-// shapes, profiles/r01n_exp_gemm_sweep.json; the per-launch phases behind them are in
-// profiles/r01n_exp_gemm_chain.txt: a CTA pays ~3800 clk before its first MMA (setup, dependency
-// release, first TMA round trip; +2100 for a CTA pair's cluster syncs) and ~50 clk per accumulator
-// column in the epilogue (+21 with a residual) because ONE warp per SM sub-partition drains TMEM,
-// converts and stores with nothing to hide its instruction latencies.
-static constexpr double PL_LAT = 2100.0, PL_SM_CAP = 57.0, PL_L2 = 8000.0, PL_HBM = 3400.0;
-// Experiment hook: the two split-K constants can be overridden from the environment (EA_PL_SPLIT_COL,
-// EA_PL_SPLIT_FIX) so several settings can be A/B-ed in one GPU session without rebuilding.
-static double pl_env(const char* name, double dflt) {
-  const char* e = getenv(name);
-  return (e && *e) ? atof(e) : dflt;
-}
-static const double PL_SPLIT_COL = pl_env("EA_PL_SPLIT_COL", 8.0);
-static const double PL_SPLIT_FIX = pl_env("EA_PL_SPLIT_FIX", 7000.0);
-static constexpr double PL_START = 3800.0, PL_START_TWO = 2100.0, PL_EPI = 50.0, PL_EPI_RES = 21.0;
+// Per-SM and chip rates in bytes per SM clock, from the H100 SXM data sheet (3.35 TB/s HBM3; fp16 wgmma at
+// 989 TFLOP/s over 132 SMs = 2048 MAC / clk / SM, so a 128 x BN x 64 K-block takes 4 BN clk) and L2 at about 1.6x
+// HBM; the fixed costs (pipeline start ~3800 clk, ~50 clk per accumulator column of epilogue) are not measured
+// per shape on H100.
+static constexpr double PL_LAT = 2100.0, PL_SM_CAP = 57.0, PL_L2 = 3000.0, PL_HBM = 1900.0;
+static constexpr double PL_SPLIT_COL = 8.0, PL_SPLIT_FIX = 7000.0;
+static constexpr double PL_START = 3800.0, PL_EPI = 50.0, PL_EPI_RES = 21.0;
+static constexpr int GEMM_BN[3] = {128, 64, 32};   // the tile widths the planner picks from (see GEMM_THREADS)
 
 // groups: identical problems run by the same launch - they multiply the CTAs (waves, what is left to split K
 // over) but not the reuse of one weight tile across its M-tiles.
-static GemmPlan plan_gemm(int mt, int N, int nkb, int act, long long ws_floats, int n_sm,
-                          bool allow_two, bool has_res = false, int groups = 1) {
+static GemmPlan plan_gemm(int mt, int N, int nkb, int act, long long ws_floats, int n_sm, bool has_res = false,
+                          int groups = 1) {
   const double epi_col = (PL_EPI + (has_res ? PL_EPI_RES : 0.0)) * (act == EA_ACT_GEGLU ? 0.84 : 1.0);
-  // measured on B200 (profiles/r01c): one SM fills shared memory at ~45 B/clk whatever the tile
-  // shape (cuBLAS sits at the same cap with 2-CTA 256x256 tiles), the chip at ~6000 B/clk from L2
-  // and ~3400 B/clk from HBM; a tcgen05 128xBNx16 MMA takes BN/2 clk.
-  GemmPlan best = {0, 0, 1, nkb, 1, 1e30, 0};
-  // CTA pairs (cta_group::2): per SM the TMA stream per K-block shrinks from 16 KB + BN*128 B to
-  // 16 KB + BN*64 B for the same 128 x BN MACs.  Only without split-K and for stride-1 shapes.
-  // 64x64-level projections (M = 8192, N = K = 320: attention out / proj_out with residual): the model picks 96,
-  // the per-shape sweep (profiles/r02f_gemm_shape_sweep.txt) has 128 26 % faster; in the step -0.03 ms (session 13).
-  // EA_PL_N320_BN overrides for A/B.
-  static const int pl_n320_bn = (int)pl_env("EA_PL_N320_BN", 128.0);
-  const int pin_bn = (mt == 64 && N == 320 && nkb == 5 && act != EA_ACT_GEGLU) ? pl_n320_bn : 0;
-  if (allow_two && mt >= 2 && pin_bn == 0) {
-    for (int BN = 256; BN >= 64; BN -= 32) {
-      if (act == EA_ACT_GEGLU && BN != 128) continue;
-      if (N <= BN - 32) continue;
-      const int nt = (N + BN - 1) / BN;
-      const int mt2 = (mt + 1) / 2 * 2;
-      const long long ctas = (long long)mt2 * nt * groups;
-      const int stage_bytes = BM * BK * 2 + (BN / 2) * BK * 2;
-      const int tmem = BN <= 64 ? 64 : BN <= 128 ? 128 : 256;
-      for (int occ = 2; occ >= 1; --occ) {
-        if (occ * tmem > 512) continue;
-        const int avail = (occ == 2 ? 111 : 224) * 1024 - 2048;
-        int st = avail / stage_bytes;
-        if (st > 8) st = 8;
-        if (st > nkb) st = nkb < 2 ? 2 : nkb;
-        if (st < 2 || (occ == 2 && st < 3 && nkb >= 3)) continue;
-        const long long slots = (long long)n_sm * occ;
-        const long long waves = (ctas + slots - 1) / slots;
-        const long long conc = ctas < slots ? ctas : slots;
-        const int per_sm = (int)((conc + n_sm - 1) / n_sm);
-        const double t_mma = 0.5 * BN * 4 * per_sm;
-        const double t_sm = (double)stage_bytes * per_sm / PL_SM_CAP;
-        const double hbm_frac = 1.0 / (double)mt;
-        const double t_chip = (double)conc * (BM * BK * 2.0 / PL_L2 + (BN / 2) * BK * 2.0 * hbm_frac / PL_HBM +
-                                              (BN / 2) * BK * 2.0 * (1.0 - hbm_frac) / PL_L2);
-        const double t_lat = PL_LAT / st;
-        double t_kb = t_mma;
-        if (t_sm > t_kb) t_kb = t_sm;
-        if (t_chip > t_kb) t_kb = t_chip;
-        if (t_lat > t_kb) t_kb = t_lat;
-        const double cost = (double)waves * (PL_START + PL_START_TWO + nkb * t_kb + epi_col * BN);
-        if (cost < best.cost) best = {BN, st, 1, nkb, occ, cost, 1};
-      }
-    }
-  }
-  for (int BN = 256; BN >= 32; BN -= 32) {
+  GemmPlan best = {0, 0, 1, nkb, 1, 1e30};
+  for (int BN : GEMM_BN) {
     if (act == EA_ACT_GEGLU && BN != 128) continue;  // weights are interleaved per 128-row block
     if (BN > 32 && N <= BN - 32) continue;            // a narrower tile covers N just as well
-    if (pin_bn > 0 && BN != pin_bn) continue;
     const int nt = (N + BN - 1) / BN;
     const long long tiles = (long long)mt * nt * groups;
     const int stage_bytes = BM * BK * 2 + BN * BK * 2;
-    const int tmem = BN <= 32 ? 32 : BN <= 64 ? 64 : BN <= 128 ? 128 : 256;
-    for (int occ = 2; occ >= 1; --occ) {
-      if (occ * tmem > 512) continue;
-      const int avail = (occ == 2 ? 111 : 224) * 1024 - 2048;
-      int st = avail / stage_bytes;
-      if (st > 8) st = 8;
-      if (st > nkb) st = nkb < 2 ? 2 : nkb;
-      if (st < 2 || (occ == 2 && st < 3 && nkb >= 3)) continue;
-      const long long slots = (long long)n_sm * occ;
-      for (int pass = 0; pass < 2; ++pass) {
-        int splits = 1, kbps = nkb;
-        if (pass == 1) {
-          if (tiles >= slots || nkb < 8) break;
-          int s_max = (int)(slots / tiles);
-          if (s_max > nkb / 4) s_max = nkb / 4;
-          if (s_max < 2) break;
-          kbps = (nkb + s_max - 1) / s_max;
-          splits = (nkb + kbps - 1) / kbps;  // every split owns at least one K-block
-          if (splits < 2) break;
-          if (tiles > 2048 || tiles * splits * (long long)(BM * BN) > ws_floats) break;
-        }
-        const long long ctas = tiles * splits;
-        const long long waves = (ctas + slots - 1) / slots;
-        const long long conc = ctas < slots ? ctas : slots;
-        const int per_sm = (int)((conc + n_sm - 1) / n_sm);
-        const double t_mma = 0.5 * BN * 4 * per_sm;                       // 4 MMAs (K=16) per K-block
-        const double t_sm = (double)stage_bytes * per_sm / PL_SM_CAP;      // per-SM TMA fill cap
-        const double a_bytes = BM * BK * 2.0, b_bytes = BN * BK * 2.0;
-        const double hbm_frac = 1.0 / (double)mt;                         // weights: HBM once, then L2
-        const double t_chip = (double)conc * (a_bytes / PL_L2 + b_bytes * hbm_frac / PL_HBM +
-                                              b_bytes * (1.0 - hbm_frac) / PL_L2);
-        const double t_lat = PL_LAT / st;
-        double t_kb = t_mma;
-        if (t_sm > t_kb) t_kb = t_sm;
-        if (t_chip > t_kb) t_kb = t_chip;
-        if (t_lat > t_kb) t_kb = t_lat;
-        double cost;
-        if (splits == 1) {
-          cost = (double)waves * (PL_START + kbps * t_kb + epi_col * BN);
-        } else {
-          // fp32 partial store, arrival counter, distributed reduce + fused epilogue (tools/exp_splitk.py,
-          // r01g; the chain stamps of the 8x8 conv put the whole fix-up at ~22k clk for splits = 10, BN = 96)
-          cost = (double)waves * (PL_START + kbps * t_kb + PL_SPLIT_COL * BN) + PL_SPLIT_FIX +
-                 3.0 * (BM * BN * 4.0) / 25.0 + 150.0 * splits;
-        }
-        if (cost < best.cost) best = {BN, st, splits, kbps, occ, cost, 0};
+    int st = GEMM_SMEM_RING / stage_bytes;
+    if (st > 8) st = 8;
+    if (st > nkb) st = nkb < 2 ? 2 : nkb;
+    const long long slots = n_sm;                   // one CTA per SM
+    for (int pass = 0; pass < 2; ++pass) {
+      int splits = 1, kbps = nkb;
+      if (pass == 1) {
+        if (tiles >= slots || nkb < 8) break;
+        int s_max = (int)(slots / tiles);
+        if (s_max > nkb / 4) s_max = nkb / 4;
+        if (s_max < 2) break;
+        kbps = (nkb + s_max - 1) / s_max;
+        splits = (nkb + kbps - 1) / kbps;  // every split owns at least one K-block
+        if (splits < 2) break;
+        if (tiles > 2048 || tiles * splits * (long long)(BM * BN) > ws_floats) break;
       }
+      const long long ctas = tiles * splits;
+      const long long waves = (ctas + slots - 1) / slots;
+      const long long conc = ctas < slots ? ctas : slots;
+      const double t_mma = 4.0 * BN;
+      const double t_sm = (double)stage_bytes / PL_SM_CAP;               // per-SM TMA fill cap
+      const double a_bytes = BM * BK * 2.0, b_bytes = BN * BK * 2.0;
+      const double hbm_frac = 1.0 / (double)mt;                         // weights: HBM once, then L2
+      const double t_chip = (double)conc * (a_bytes / PL_L2 + b_bytes * hbm_frac / PL_HBM +
+                                            b_bytes * (1.0 - hbm_frac) / PL_L2);
+      const double t_lat = PL_LAT / st;
+      double t_kb = t_mma;
+      if (t_sm > t_kb) t_kb = t_sm;
+      if (t_chip > t_kb) t_kb = t_chip;
+      if (t_lat > t_kb) t_kb = t_lat;
+      double cost;
+      if (splits == 1) {
+        cost = (double)waves * (PL_START + kbps * t_kb + epi_col * BN);
+      } else {
+        // fp32 partial store, arrival counter, distributed reduce + fused epilogue
+        cost = (double)waves * (PL_START + kbps * t_kb + PL_SPLIT_COL * BN) + PL_SPLIT_FIX +
+               3.0 * (BM * BN * 4.0) / 25.0 + 150.0 * splits;
+      }
+      if (cost < best.cost) best = {BN, st, splits, kbps, 1, cost};
     }
-  }
-  // Measured deviations from the cost model (profiles/r01r_exp_splitk_sweep.txt, B200, 148 SMs): two shapes of the
-  // 16x16 level where a sweep over (BN, splits) beat the model's pick by 13-14 %.
-  if (ws_floats > 0 && groups == 1 && mt == 4 && N == 1280 && act != EA_ACT_GEGLU) {
-    if (nkb == 80 && best.splits > 1)                       // ff2: 512 x 1280, K = 5120: 24.1 vs 28.0 us
-      best = {64, 8, 1, nkb, 1, best.cost, 0};
-    else if (nkb >= 360 && nkb <= 400 && best.BN == 256 &&  // conv 2560 -> 1280 (+ 1x1 skip): 45.5 vs 52.5 us
-             4LL * mt * 8 * (BM * 160) <= ws_floats)
-      best = {160, 6, 4, (nkb + 3) / 4, 1, best.cost, 0};
   }
   return best;
 }
@@ -1630,33 +1045,13 @@ static int sm_count() { return ea_sm_count(); }
 
 using namespace ea;
 
-#ifdef EA_GEMM_TIMING
-static int g_dbg_launch = 0;
-extern "C" int ea_gemm_chain_reset(void) {
-  static unsigned long long init[1024 * 8];
-  for (int i = 0; i < 1024; ++i)
-    for (int j = 0; j < 8; ++j) init[i * 8 + j] = j == 6 ? ~0ull : 0ull;
-  g_dbg_launch = 0;
-  return cudaMemcpyToSymbol(ea_gemm_chain, init, sizeof(init)) == cudaSuccess ? 0 : EA_ERR_CUDA;
-}
-extern "C" int ea_gemm_chain_read(unsigned long long* host_out, int n_launches) {
-  if (n_launches > 1024) n_launches = 1024;
-  return cudaMemcpyFromSymbol(host_out, ea_gemm_chain, sizeof(unsigned long long) * 8 * n_launches) == cudaSuccess
-             ? 0 : EA_ERR_CUDA;
-}
-extern "C" int ea_gemm_debug_read(long long* host_out, int n) {
-  if (n > 64 * 4 + 8) n = 64 * 4 + 8;
-  return cudaMemcpyFromSymbol(host_out, ea_gemm_dbg, sizeof(long long) * n) == cudaSuccess ? 0 : EA_ERR_CUDA;
-}
-#endif
-
 extern "C" int ea_gemm_plan(int m_tiles, int N, int k_blocks, int act, long long workspace_bytes,
                             int n_sm, int* out5) {
   if (!out5 || m_tiles <= 0 || N <= 0 || k_blocks <= 0) return EA_ERR_ARG;
   const long long ws_floats = workspace_bytes > 65536 ? (workspace_bytes - 65536) / 4 : 0;
-  GemmPlan pl = plan_gemm(m_tiles, N, k_blocks, act, ws_floats, n_sm > 0 ? n_sm : 148, true);
+  GemmPlan pl = plan_gemm(m_tiles, N, k_blocks, act, ws_floats, n_sm > 0 ? n_sm : 132);
   out5[0] = pl.BN; out5[1] = pl.stages; out5[2] = pl.splits; out5[3] = pl.kbps;
-  out5[4] = pl.occ + 10 * pl.two;   // tens digit: 1 = CTA pairs (cta_group::2)
+  out5[4] = pl.occ;   // tens digit (CTA pairs) is always 0 on this architecture
   return pl.BN ? EA_OK : EA_ERR_SHAPE;
 }
 
@@ -1674,9 +1069,6 @@ static int gemm_fill_group(const ea_gemm_args* a, GemmGroup& G, GemmShape& sh) {
   if (a->N % 8 != 0) return EA_ERR_SHAPE;
   GemmKParams& p = G.p;
   memset(&p, 0, sizeof(p));
-#ifdef EA_GEMM_TIMING
-  p.dbg_id = g_dbg_launch++;
-#endif
   p.M = a->M;
   p.N = a->N;
   p.mode = a->mode;
@@ -1700,10 +1092,9 @@ static int gemm_fill_group(const ea_gemm_args* a, GemmGroup& G, GemmShape& sh) {
     p.pf_bytes[i] = a->prefetch[i] ? (a->prefetch_bytes[i] & ~15LL) : 0;
   }
   p.pf_ctas = 0;   // set with the grid
-  // W operand: streamed once per step (3.16 GB through a 126 MB L2) - marked evict-first so that it displaces itself
-  // rather than the activations and skip tensors the following launches read.  EA_GEMM_W_EVICT=0 turns the hint off.
-  static const int w_evict = (int)pl_env("EA_GEMM_W_EVICT", 1.0);
-  p.b_policy = w_evict == 1 ? 0x12F0000000000000ull : w_evict == 2 ? 0x14F0000000000000ull : 0ull;
+  // W operand: streamed once per step (3.16 GB through a 50 MB L2) - marked evict-first so that it displaces itself
+  // rather than the activations and skip tensors the following launches read.
+  p.b_policy = 0x12F0000000000000ull;
   if (a->row_scale && (a->act == EA_ACT_GEGLU || a->rowstats_out || a->ln_stats)) return EA_ERR_ARG;
   sh.ln_any = a->rowstats_out || a->ln_stats;
   if (sh.ln_any) {
@@ -1802,6 +1193,26 @@ static int set_max_smem(K kernel, int bytes, int& cached) {
   return EA_OK;
 }
 
+template <int BN, int NG>
+static cudaError_t launch_gemm(const GemmLaunch<NG>& L, int grid, int smem_bytes, int tiles_per_group, int m_tiles,
+                               int n_groups, cudaStream_t stream, int& rc) {
+  static int cache[EA_MAX_DEV];   // zero-initialised; per device (see ea_internal.h)
+  if ((rc = set_max_smem(ea_gemm_kernel<BN, NG>, smem_bytes, cache[ea_dev()]))) return cudaSuccess;
+  return ea_launch(ea_gemm_kernel<BN, NG>, dim3((unsigned)grid), dim3(GEMM_THREADS), (size_t)smem_bytes, stream, L,
+                   tiles_per_group, m_tiles, n_groups);
+}
+
+template <int NG>
+static cudaError_t launch_gemm_bn(int BN, const GemmLaunch<NG>& L, int grid, int smem_bytes, int tiles_per_group,
+                                  int m_tiles, int n_groups, cudaStream_t stream, int& rc) {
+  switch (BN) {
+    case 32: return launch_gemm<32, NG>(L, grid, smem_bytes, tiles_per_group, m_tiles, n_groups, stream, rc);
+    case 64: return launch_gemm<64, NG>(L, grid, smem_bytes, tiles_per_group, m_tiles, n_groups, stream, rc);
+    case 128: return launch_gemm<128, NG>(L, grid, smem_bytes, tiles_per_group, m_tiles, n_groups, stream, rc);
+    default: return launch_gemm<256, NG>(L, grid, smem_bytes, tiles_per_group, m_tiles, n_groups, stream, rc);
+  }
+}
+
 extern "C" int ea_gemm_grouped(const ea_gemm_args* args, int n_groups, void* stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   if (!args || n_groups < 1 || n_groups > GEMM_MAX_GROUPS) return EA_ERR_ARG;
@@ -1817,103 +1228,50 @@ extern "C" int ea_gemm_grouped(const ea_gemm_args* args, int n_groups, void* str
   }
   const int m_tiles = sh0.m_tiles, nkb = sh0.nkb;
   const bool ln_any = sh0.ln_any;
-  const GemmKParams& p0 = L.g[0].p;
   const int G = n_groups;
   // workspace: [0, 64 KB) arrival counters (int, zero between launches), then fp32 partial tiles
   const long long ws_floats =      // the LayerNorm fold lives in the unsplit epilogues only
       (a->workspace && a->workspace_bytes > 65536 && !ln_any) ? (a->workspace_bytes - 65536) / 4 : 0;
-  static const int two_env = [] { const char* e = getenv("EA_GEMM_2CTA"); return e ? atoi(e) : -1; }();
-  const bool can_two = a->mode != EA_GEMM_CONV_S2 && a->mode != EA_GEMM_CONV_S2A && two_env != 0 && a->force_2cta >= 0;
-  // EA_GEMM_PERSIST: unset / 3 = per-launch choice (below), 0 = never, 1 / 2 = wherever the launch qualifies
-  // (4 / 8 epilogue warps; the A/B switches of profiles/r02a_gemm_breakdown_*).
-  static const int persist_env = [] { const char* e = getenv("EA_GEMM_PERSIST"); return e ? atoi(e) : 3; }();
-  const bool batch_ok =
-      !a->rowvec || (a->mode == EA_GEMM_LINEAR
-                         ? (a->rows_per_batch == 0 || a->rows_per_batch >= BM || a->rows_per_batch == BM / 2)
-                         : p0.bn <= 2);      // a tile may span at most two batch elements (fast epilogue)
-  const bool persist_ok = !a->out_f32 && !a->accumulate && !a->row_scale && a->force_splits <= 1 && a->force_2cta <= 0 &&
-                          (a->act == EA_ACT_GEGLU || batch_ok);
-  bool persist = persist_ok && (a->force_persistent > 0 || (a->force_persistent == 0 && persist_env > 0));
-  const int persist_wg = (a->force_persistent == 2 || (a->force_persistent == 0 && persist_env >= 2)) ? 2 : 1;
+  // force_persistent > 0: one CTA per SM walking the tile list (no split-K); otherwise one tile per CTA
+  const bool persist = a->force_persistent > 0;
   const bool has_res = a->residual != nullptr;
-  GemmPlan plan = plan_gemm(m_tiles, a->N, nkb, a->act, ws_floats, sm_count(), can_two, has_res, G);
-  if (persist && a->force_persistent == 0) {
-    // auto mode: never where the planner splits K (weight-streaming small-M layers; first A/B on hardware: the
-    // unsplit 8x8 convolutions took 50 us instead of 20), and the 4-epilogue-warp variant only for grids of more
-    // than one wave (its gain is the overlap across tiles; the 8-warp variant also speeds up a single tile)
-    const long long tiles0 = (long long)G * m_tiles * ((a->N + plan.BN - 1) / plan.BN);
-    if (plan.splits > 1 || (persist_wg == 1 && tiles0 <= sm_count())) persist = false;
-    if (persist && persist_env == 3) {
-      // Default: the 8-epilogue-warp persistent kernel wherever its tile list balances over the SMs - at most one
-      // wave, or at least two.  Measured per shape on B200 (profiles/r02a_gemm_breakdown_{base,persist2}.json): it
-      // wins 7-27 % on the GEGLU projections, the C x C linears of the 32x32 / 16x16 levels and the long-K
-      // convolutions (sum over a step's 362 launches 6.16 -> 5.86 ms), and loses 6-20 % where 148 < tiles < 296
-      // leaves half the SMs a second tile to do alone (64 x 4 tiles: 8192 x 320 x 320, 8192 x 640 x 5760).
-      const GemmPlan pp = plan.two ? plan_gemm(m_tiles, a->N, nkb, a->act, 0, sm_count(), false, has_res, G) : plan;
-      const long long tiles_p = (long long)G * m_tiles * ((a->N + pp.BN - 1) / pp.BN);
-      if (tiles_p > sm_count() && tiles_p < 2LL * sm_count()) persist = false;
-    }
-  }
-  if (persist && (plan.two || plan.splits > 1))   // the persistent kernel has no CTA pairs and no split-K
-    plan = plan_gemm(m_tiles, a->N, nkb, a->act, 0, sm_count(), false, has_res, G);
-  if (a->force_2cta > 0 && can_two && !plan.two) {  // testing: pair mode with the 1-CTA tile width
-    plan.two = 1; plan.splits = 1; plan.kbps = nkb;
-    if (plan.BN < 64) plan.BN = 64;
-    plan.stages = 3;
-  }
+  GemmPlan plan = plan_gemm(m_tiles, a->N, nkb, a->act, persist ? 0 : ws_floats, sm_count(), has_res, G);
   if (a->force_bn > 0 || a->force_stages > 0 || a->force_splits > 0) {
     if (a->force_bn > 0) plan.BN = a->force_bn;
     const int sb = BM * BK * 2 + plan.BN * BK * 2;
     if (a->force_bn > 0) plan.stages = plan.BN <= 128 ? 3 : 4;
     if (a->force_stages > 0) plan.stages = a->force_stages;
-    if (plan.stages * sb > 224 * 1024) plan.stages = 224 * 1024 / sb;
+    if (plan.stages * sb > GEMM_SMEM_RING) plan.stages = GEMM_SMEM_RING / sb;
     if (plan.stages > nkb) plan.stages = nkb < 2 ? 2 : nkb;
     if (a->force_bn > 0 || a->force_splits > 0) { plan.splits = 1; plan.kbps = nkb; }
-    if (a->force_splits > 1) {
+    if (a->force_splits > 1 && !persist) {
       plan.kbps = (nkb + a->force_splits - 1) / a->force_splits;
       plan.splits = (nkb + plan.kbps - 1) / plan.kbps;
-      plan.two = 0;
     }
-    if (a->force_2cta <= 0 && (a->force_bn > 0 || a->force_splits > 0)) plan.two = 0;
   }
   if (ln_any && plan.splits > 1) return EA_ERR_ARG;
-  const int two = plan.two && plan.splits == 1 && plan.BN >= 64 && plan.BN % 32 == 0;
   const int BN = plan.BN;
-  if (BN < 32 || BN > 256 || BN % 32 != 0) return EA_ERR_ARG;
+  if (BN != 32 && BN != 64 && BN != 128 && BN != 256) return EA_ERR_SHAPE;
   if (a->act == EA_ACT_GEGLU && (a->N % 128 != 0 || BN != 128)) return EA_ERR_SHAPE;
   const int n_tiles = (a->N + BN - 1) / BN;
   const long long tiles = (long long)m_tiles * n_tiles;      // per group
   if (plan.splits > 1 &&
       (!ws_floats || tiles * G > 8192 || tiles * G * plan.splits * (long long)(BM * BN) > ws_floats))
     return EA_ERR_SHAPE;
+  // the spinning split-K fix-up makes split CTAs wait for their siblings: every CTA of the grid must be resident at
+  // once (one per SM; the planner guarantees it, forced test configurations are checked here instead of deadlocking)
+  if (plan.splits > 1 && !a->no_spin && tiles * G * plan.splits > (long long)sm_count()) return EA_ERR_SHAPE;
 
-  // plan-dependent part of every group: tile shape, split-K scratch, the B map
-  const bool persist_launch = persist && !two && plan.splits == 1;
-  int stages = 0, smem_bytes = 0, pair_release = 0;
-  if (persist_launch) {
-    const int sbp = BM * BK * 2 + BN * BK * 2;
-    const int fixed = 32768 * persist_wg + (2 * 8 + 4) * 8 + 32 + 2 * 2 * 256 * 4 + 1024;   // staging, barriers, slot, bias, align
-    stages = (224 * 1024 - fixed) / sbp;
-    if (stages > 8) stages = 8;
-    if (a->force_stages > 0 && a->force_stages < stages) stages = a->force_stages;
-    smem_bytes = stages * sbp + fixed;
-  }
-  const bool use_persist = persist_launch && stages >= 2;
-  if (!use_persist) {
-    const int stage_bytes = BM * BK * 2 + (two ? BN / 2 : BN) * BK * 2;
-    stages = plan.stages;
-    if (stages > 8) stages = 8;
-    if (stages < 2) stages = 2;
-    if (stages >= 5 && (stages & 1) && a->force_stages == 0) --stages;   // even: stages are released in pairs
-    pair_release = (stages >= 4 && stages % 2 == 0) ? 1 : 0;
-    smem_bytes = stages * stage_bytes + (2 * stages + 1) * 8 + 32 + 2 * 256 * 4 + 1024;
-  }
+  int stages = plan.stages;
+  if (stages > 8) stages = 8;
+  if (stages < 2) stages = 2;
+  const int smem_bytes = gemm_region_bytes(BN, stages) + (2 * stages + 2) * 8 + 2 * 2 * 256 * 4 + 1024;
+  const long long tiles_per_group = tiles * plan.splits;
   for (int g = 0; g < G; ++g) {
     GemmKParams& p = L.g[g].p;
     const ea_gemm_args* ag = &args[g];
     p.BN = BN;
     p.stages = stages;
-    p.pair_release = pair_release;
     p.splits = plan.splits;
     p.kb_per_split = plan.kbps;
     p.no_spin = a->no_spin;
@@ -1924,91 +1282,29 @@ extern "C" int ea_gemm_grouped(const ea_gemm_args* args, int n_groups, void* str
     }
     const long long ldw = ag->ldw > 0 ? ag->ldw : sh0.Ktot;
     if (ldw % 8 != 0) return EA_ERR_SHAPE;
-    if (encode_2d(&L.g[g].tmB, ag->w, (uint64_t)sh0.Ktot, (uint64_t)ag->N, (uint64_t)ldw * 2, BK,
-                  (uint32_t)(two ? BN / 2 : BN)))
+    if (encode_2d(&L.g[g].tmB, ag->w, (uint64_t)sh0.Ktot, (uint64_t)ag->N, (uint64_t)ldw * 2, BK, (uint32_t)BN))
       return EA_ERR_TMAP;
   }
   // The evict-first hint on W pays where a weight tile is used within about one wave (<= 64 row tiles per network: the
   // step at 1 image / GPU, SAM).  With thousands of row tiles (VAE: M up to 262144; 4 images / GPU at 64x64) the same
-  // weight tile is re-read wave after wave and the hint cost 0.4-4 % (round 2, session 22): plain loads there.
+  // weight tile is re-read wave after wave: plain loads there.
   if (m_tiles > 64)
     for (int g = 0; g < G; ++g) L.g[g].p.b_policy = 0ull;
-  {   // L2 prefetch hints: how many CTAs share each group's range (the first ones to start)
-    const long long total_p = tiles * G;
-    const long long per_group = two ? (long long)((m_tiles + 1) / 2 * 2) * n_tiles : tiles * plan.splits;
-    const int share = sm_count() / G > 0 ? sm_count() / G : 1;
-    for (int g = 0; g < G; ++g)
-      L.g[g].p.pf_ctas = use_persist ? (int)(total_p < sm_count() ? total_p : sm_count())
-                                     : (int)(per_group < share ? per_group : share);
-  }
-  GemmLaunch<1> L1;
-  if (G == 1) L1.g[0] = L.g[0];
+  const long long total = tiles_per_group * G;
+  const int grid = (int)(persist && total > sm_count() ? sm_count() : total);
+  for (int g = 0; g < G; ++g)   // L2 prefetch hints: the launch's first CTAs share each group's range
+    L.g[g].p.pf_ctas = grid < sm_count() ? grid : sm_count();
 
-  if (use_persist) {
-    static int cache_all[EA_MAX_DEV][3][2];     // zero-initialised; per device (see ea_internal.h)
-    int (*cache_p)[2] = cache_all[ea_dev()];
-    const long long total = tiles * G;
-    const int grid_p = (int)(total < sm_count() ? total : sm_count());
-    cudaError_t lp;
-    int rc;
-    if (persist_wg == 2) {
-      if (G == 1) {
-        if ((rc = set_max_smem(ea_gemm_persistent_kernel<2, 1>, smem_bytes, cache_p[2][0]))) return rc;
-        lp = ea_launch(ea_gemm_persistent_kernel<2, 1>, dim3((unsigned)grid_p), dim3(PersistShape<2>::kThreads), (size_t)smem_bytes,
-                       stream, L1, (int)tiles, m_tiles, G);
-      } else {
-        if ((rc = set_max_smem(ea_gemm_persistent_kernel<2, GEMM_MAX_GROUPS>, smem_bytes, cache_p[2][1]))) return rc;
-        lp = ea_launch(ea_gemm_persistent_kernel<2, GEMM_MAX_GROUPS>, dim3((unsigned)grid_p), dim3(PersistShape<2>::kThreads),
-                       (size_t)smem_bytes, stream, L, (int)tiles, m_tiles, G);
-      }
-    } else {
-      if (G == 1) {
-        if ((rc = set_max_smem(ea_gemm_persistent_kernel<1, 1>, smem_bytes, cache_p[1][0]))) return rc;
-        lp = ea_launch(ea_gemm_persistent_kernel<1, 1>, dim3((unsigned)grid_p), dim3(PersistShape<1>::kThreads), (size_t)smem_bytes,
-                       stream, L1, (int)tiles, m_tiles, G);
-      } else {
-        if ((rc = set_max_smem(ea_gemm_persistent_kernel<1, GEMM_MAX_GROUPS>, smem_bytes, cache_p[1][1]))) return rc;
-        lp = ea_launch(ea_gemm_persistent_kernel<1, GEMM_MAX_GROUPS>, dim3((unsigned)grid_p), dim3(PersistShape<1>::kThreads),
-                       (size_t)smem_bytes, stream, L, (int)tiles, m_tiles, G);
-      }
-    }
-    ea_count_launch();
-    if (lp != cudaSuccess) return ea_cuda_fail(lp, "ea_gemm: persistent kernel launch");
-    const cudaError_t pe = cudaGetLastError();
-    return pe == cudaSuccess ? 0 : ea_cuda_fail(pe, "ea_gemm: after the persistent kernel launch");
-  }
-  if (plan.splits > 1 && !a->no_spin) {
-    // the spinning fix-up makes split CTAs wait for their siblings: every CTA of the grid must be
-    // resident at once, at the occupancy this launch really gets (the planner guarantees it; forced
-    // test configurations are checked here instead of deadlocking)
-    const int tmem_c = tmem_cols_for(BN);
-    const int occ = (2 * (smem_bytes + 1024) <= 227 * 1024 && 2 * tmem_c <= 512) ? 2 : 1;
-    if (tiles * G * plan.splits > (long long)occ * sm_count()) return EA_ERR_SHAPE;
-  }
-  static int cache_k_all[EA_MAX_DEV][2][2];
-  int (*cache_k)[2] = cache_k_all[ea_dev()];
   cudaError_t le;
-  int rc;
-  if (two) {
-    dim3 grid((unsigned)((m_tiles + 1) / 2 * 2), (unsigned)n_tiles, (unsigned)G);   // whole CTA pairs along M
-    if (G == 1) {
-      if ((rc = set_max_smem(ea_gemm_kernel<true, 1>, smem_bytes, cache_k[1][0]))) return rc;
-      le = ea_launch_cluster(ea_gemm_kernel<true, 1>, grid, dim3(GEMM_THREADS), (size_t)smem_bytes, stream, 2u, L1);
-    } else {
-      if ((rc = set_max_smem(ea_gemm_kernel<true, GEMM_MAX_GROUPS>, smem_bytes, cache_k[1][1]))) return rc;
-      le = ea_launch_cluster(ea_gemm_kernel<true, GEMM_MAX_GROUPS>, grid, dim3(GEMM_THREADS), (size_t)smem_bytes, stream,
-                             2u, L);
-    }
+  int rc = EA_OK;
+  if (G == 1) {
+    GemmLaunch<1> L1;
+    L1.g[0] = L.g[0];
+    le = launch_gemm_bn<1>(BN, L1, grid, smem_bytes, (int)tiles_per_group, m_tiles, G, stream, rc);
   } else {
-    dim3 grid((unsigned)m_tiles, (unsigned)n_tiles, (unsigned)(plan.splits * G));
-    if (G == 1) {
-      if ((rc = set_max_smem(ea_gemm_kernel<false, 1>, smem_bytes, cache_k[0][0]))) return rc;
-      le = ea_launch(ea_gemm_kernel<false, 1>, grid, dim3(GEMM_THREADS), (size_t)smem_bytes, stream, L1);
-    } else {
-      if ((rc = set_max_smem(ea_gemm_kernel<false, GEMM_MAX_GROUPS>, smem_bytes, cache_k[0][1]))) return rc;
-      le = ea_launch(ea_gemm_kernel<false, GEMM_MAX_GROUPS>, grid, dim3(GEMM_THREADS), (size_t)smem_bytes, stream, L);
-    }
+    le = launch_gemm_bn<GEMM_MAX_GROUPS>(BN, L, grid, smem_bytes, (int)tiles_per_group, m_tiles, G, stream, rc);
   }
+  if (rc) return rc;
   ea_count_launch();
   if (le != cudaSuccess) return ea_cuda_fail(le, "ea_gemm: kernel launch");
   const cudaError_t ke = cudaGetLastError();

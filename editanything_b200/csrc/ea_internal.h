@@ -26,7 +26,7 @@ int ea_cuda_fail(cudaError_t e, const char* where);
 
 // Programmatic dependent launch (PDL): every kernel of this library calls griddepcontrol.wait before
 // it touches global memory, so consecutive launches on a stream may overlap the next kernel's
-// prologue (barrier init, TMEM allocation, tensor-map prefetch, block scheduling) with the tail of
+// prologue (barrier init, tensor-map prefetch, block scheduling) with the tail of
 // the previous one.  ea_set_pdl(0) / EA_PDL=0 falls back to plain stream serialisation.
 int ea_pdl_enabled();
 #ifdef __CUDACC__

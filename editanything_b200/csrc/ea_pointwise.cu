@@ -1,4 +1,4 @@
-// ea_pointwise.cu — the HBM/L2-bound operators around the tensor-core kernels (sm_100a).
+// ea_pointwise.cu — the HBM/L2-bound operators around the tensor-core kernels (sm_90a).
 // GroupNorm(+SiLU), LayerNorm, small direct convolutions, nearest upsample, the tiny
 // time-embedding linears, the fused out-conv + CFG + DDIM step, and the SAM window helpers.
 // All use 16-byte vector accesses on channels-last data and warp-shuffle reductions.
@@ -89,8 +89,8 @@ gn_fused_kernel(const ea_half* __restrict__ x, long long ldx, int C1,
 #ifndef EA_GN_NO_ASYNC
     if (cached) {
       // every pixel of this thread goes global -> shared memory asynchronously: all of its loads are in flight at
-      // once (ONE L2 round trip) instead of four at a time through registers (the launch was a chain of ~8 round trips
-      // for 11-15 us whatever the tensor size, profiles/r02c_launches.csv)
+      // once (ONE L2 round trip) instead of four at a time through registers (a chain of ~8 round trips whatever the
+      // tensor size)
       for (int pp = p0 + pl; pp < p1; pp += lanes) {
         const uint32_t dst = (uint32_t)__cvta_generic_to_shared(&cache[(pp - p0) * nvec + v]);
         asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst), "l"(src + ((long long)b * HW + pp) * lds) : "memory");
@@ -119,7 +119,7 @@ gn_fused_kernel(const ea_half* __restrict__ x, long long ldx, int C1,
     }
     }
     // per-(pixel lane, channel) partials -> shared memory (no atomics: 480 threads x 16 contended
-    // shared atomics used to cost ~4 us per launch)
+    // shared atomics per launch)
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
       part[(pl * 2 + 0) * C + c + j] = cs[j];
@@ -155,7 +155,7 @@ gn_fused_kernel(const ea_half* __restrict__ x, long long ldx, int C1,
   }  // phase != 2
   // ---- pass 2: y = x * a + b with a = rstd*gamma, b = beta - mean*a (per channel of this thread)
   // the image's 2*groups statistics come back in ONE L2 round trip (per-thread dependent loads of
-  // "its" groups cost several serialized round trips: profiles/r01j_gn_ncu_full.txt)
+  // "its" groups cost several serialized round trips)
   __syncthreads();
   {
     // sum of the image's per-CTA partials in a fixed order: `parts` threads per statistic take every parts-th CTA
@@ -767,8 +767,8 @@ conv_smallcin_kernel(const ea_half* __restrict__ x, const float* __restrict__ w,
   for (int i = threadIdx.x; i < Cout; i += blockDim.x) wsm[nw + i] = bias ? bias[i] : 0.f;
   __syncthreads();
   // A thread owns 8 consecutive output channels of PX = 4 horizontally adjacent pixels: every weight read from
-  // shared memory feeds 4 FMAs (one pixel per thread made the kernel shared-memory-bandwidth bound: 72 us for the
-  // 94 MFLOP of conv_in at 64x64, profiles/r02c_launches_summary.txt), and a persistent grid loads the 46 KB filter
+  // shared memory feeds 4 FMAs (one pixel per thread makes the kernel shared-memory-bandwidth bound), and a
+  // persistent grid loads the 46 KB filter
   // bank once per CTA instead of once per 256 outputs.
   constexpr int PX = 4;
   const int ngrp = Cout >> 3;

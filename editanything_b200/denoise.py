@@ -1,4 +1,4 @@
-"""The per-step engine: ControlNet(s) -> UNet -> CFG -> DDIM on the B200 kernels.
+"""The per-step engine: ControlNet(s) -> UNet -> CFG -> DDIM on the H100 kernels.
 
 This is the seam SURVEY.md §8b calls B3: what
 utils/stable_diffusion_controlnet_inpaint.py:1607-1636 does with `self.controlnet(...)`,
@@ -296,7 +296,7 @@ class DenoiseEngine:
             lat0, xh0, c0 = self.lat.clone(), self.x_half.clone(), self.step_ctr.clone()
             # opt-in experiment (EA_WEIGHT_PREFETCH = look-ahead distance, default 0 = off): the warm-up pass records
             # the step's GEMM sequence and in the captured pass every launch carries a later launch's weights as an L2
-            # prefetch hint (ops.WeightLookahead).  Measured SLOWER in every form (profiles/r02g_weight_prefetch_ab.txt)
+            # prefetch hint (ops.WeightLookahead).  Not measured on H100.
             dist = int(os.environ.get("EA_WEIGHT_PREFETCH", "0"))
             mk = getattr(self.ops, "WeightLookahead", None)
             single = self.runner.lockstep or not self.runner.cns     # launch order = execution order

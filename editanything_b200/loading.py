@@ -9,7 +9,7 @@ Checkpoints are diffusers-layout DIRECTORIES (model_index.json, unet/, vae/, tex
 a ControlNet is config.json + diffusion_pytorch_model.{safetensors,bin}).  There is no network on the deployment
 boxes: hub ids resolve through $EA_MODEL_ROOT/<org>/<name>, $EA_MODEL_ROOT/<org>--<name> or the local HF cache
 (models--<org>--<name>/snapshots/*).  The weights are re-keyed to the ldm/cldm names (editanything_b200.weights)
-and packed into the B200 engines; text encoder and tokenizer come from `transformers`.
+and packed into the H100 engines; text encoder and tokenizer come from `transformers`.
 """
 import glob
 import json

@@ -3,7 +3,7 @@
 Mirrors the reference call contracts (SURVEY.md §8b B3):
     controlnet(sample, t, encoder_hidden_states, controlnet_cond, conditioning_scale) -> residuals
     unet(sample, t, encoder_hidden_states, down_block_additional_residuals, mid_...)  -> eps
-but executes them channels-last on hand-written sm_100a kernels, with the ControlNet residuals
+but executes them channels-last on hand-written sm_90a kernels, with the ControlNet residuals
 never materialised as separate tensors: every zero-conv GEMM accumulates `scale * residual`
 straight into the UNet's skip-concat buffers (cldm/cldm.py:34-41), and CFG + the DDIM update run in
 the epilogue of the final convolution (cldm/ddim_hacked.py:190-231).
@@ -210,7 +210,7 @@ class PackedNet:
                               ksize=3, stride=s, silu=True, ldo=cp)
             else:
                 # layers 2..8 as implicit-GEMM convolutions on the tensor cores (1.5 GFLOP per image on CUDA cores
-                # cost several ms per request; padded to 64-channel multiples they are ~64 GFLOP of tcgen05 work)
+                # cost several ms per request; padded to 64-channel multiples they are ~64 GFLOP of tensor-core work)
                 wp = self.w[p + ".wp"]
                 y = torch.empty(B, Ho, Wo, wp.shape[0], device=self.dev, dtype=self.hdt)
                 o.gemm(x, wp, y.view(B * Ho * Wo, -1), mode=L.EA_GEMM_CONV_S1 if s == 1 else L.EA_GEMM_CONV_S2,
@@ -624,7 +624,7 @@ class UNetRunner:
             self._encoder_lockstep(x_half, embs, ctx_ls, hints, sinks, scales)
         elif concurrent:
             # The UNet encoder and every ControlNet only READ x and write their own activations: run
-            # them on parallel streams (many of their launches cannot fill 148 SMs on their own), join,
+            # them on parallel streams (many of their launches cannot fill 132 SMs on their own), join,
             # then apply the zero-conv accumulations into the shared skip slots on the main stream.
             # Inside the concurrent region GroupNorm / split-K use their variants without inter-CTA
             # waits, and each stream has its own scratch lane.

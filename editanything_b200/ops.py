@@ -1,7 +1,7 @@
 """Thin torch-tensor wrappers over the C ABI (include/editanything_b200.h).
 
 PyTorch is used here only for device memory and streams; every function below launches
-hand-written sm_100a kernels from libea_b200.so on torch's current stream.
+hand-written sm_90a kernels from libea_b200.so on torch's current stream.
 """
 import ctypes as C
 
@@ -128,8 +128,8 @@ class WeightLookahead:
     """L2 prefetch hints for a REPEATED sequence of GEMM launches (one denoising step): the `record` pass notes every
     launch's weight operands; in the `replay` pass launch i carries the weights of launch i + distance (wrapping to the
     next step's first launches) in ea_gemm_args.prefetch, so HBM streams them into L2 while launch i computes.  The
-    step moves 3.16 GB of weights through a 126 MB L2 at an average of only ~0.5 TB/s - HBM idles behind the latency
-    chain of short launches; weight-bound layers (8x8 / 16x16 latents, M = 128 / 512) then start from L2."""
+    step moves 3.16 GB of weights through a 50 MB L2, and HBM idles behind the latency chain of short launches;
+    weight-bound layers (8x8 / 16x16 latents, M = 128 / 512) then start from L2."""
     MIN_BYTES = 1 << 20      # smaller operands arrive within the launch's own first wave anyway
 
     def __init__(self, distance=1, max_m=1 << 30):

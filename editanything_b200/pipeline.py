@@ -1,4 +1,4 @@
-"""`StableDiffusionControlNetInpaintPipeline` on the B200 denoise engine (SURVEY.md §8b B2).
+"""`StableDiffusionControlNetInpaintPipeline` on the H100 denoise engine (SURVEY.md §8b B2).
 
 Same call surface as the reference's diffusers-style pipeline
 (`utils/stable_diffusion_controlnet_inpaint.py:391`, `__call__` `:1131-1703`), so

@@ -11,7 +11,7 @@ in-container HF port transformers/models/sam/modeling_sam.py, "HF:"):
     Block                      HF:954-972            LN -> [pad+window partition] -> attention ->
                                                      [unpartition] + residual -> LN -> MLP + residual
     Attention                  HF:803-831            qkv ea_gemm (+bias) -> decomposed rel-pos terms
-                                                     from the UNSCALED q -> fused tcgen05 attention with the
+                                                     from the UNSCALED q -> fused wgmma attention with the
                                                      rel-pos bias added to the fp32 logits -> proj ea_gemm
     window partition           HF:900-952            zero padding AFTER LayerNorm; padded tokens are
                                                      real keys (k, v = qkv bias), not masked

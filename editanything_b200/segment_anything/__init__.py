@@ -4,7 +4,7 @@ dependency: editany_lora.py:44-66; SURVEY.md §8b row B4):
     from segment_anything import sam_model_registry, SamAutomaticMaskGenerator, SamPredictor      # reference
     from editanything_b200.segment_anything import ...                                             # this backend
 
-`sam_model_registry["default"](checkpoint=path)` builds a `Sam` whose image encoder is the B200 engine
+`sam_model_registry["default"](checkpoint=path)` builds a `Sam` whose image encoder is the H100 engine
 (`editanything_b200.sam.SamEncoderEngine`, built when the model is moved to a CUDA device) and whose prompt encoder /
 mask decoder are PyTorch modules with upstream parameter names, so the official .pth checkpoints load as they are."""
 import torch

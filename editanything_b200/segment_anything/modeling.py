@@ -1,6 +1,6 @@
 """SAM prompt encoder, mask decoder and the `Sam` container (SURVEY.md §8b row B4, §8f N3), in PyTorch.
 
-The image encoder - 5.96 of SAM's ~6 TFLOP per image - is `editanything_b200.sam.SamEncoderEngine` (sm_100a
+The image encoder - 5.96 of SAM's ~6 TFLOP per image - is `editanything_b200.sam.SamEncoderEngine` (sm_90a
 kernels); the prompt encoder and the two-layer two-way mask decoder are a few MFLOP per prompt batch and stay
 PyTorch modules.  Parameter names and tensor layouts follow the upstream `segment_anything` package so the official
 checkpoints (`sam_vit_h_4b8939.pth`, editany_lora.py:54-66,85-87) load with `load_state_dict`; upstream itself is an
@@ -242,7 +242,7 @@ class MaskDecoder(nn.Module):
 
 
 class _EncoderModule(nn.Module):
-    """`sam.image_encoder`: fp32 NCHW [B, 3, S, S] -> fp32 [B, 256, S/16, S/16] on the B200 engine.  The engine is
+    """`sam.image_encoder`: fp32 NCHW [B, 3, S, S] -> fp32 [B, 256, S/16, S/16] on the H100 engine.  The engine is
     built lazily on `.to(cuda device)` from the checkpoint tensors held until then (there is no CPU path)."""
 
     def __init__(self, cfg, state_dict):
@@ -261,7 +261,7 @@ class _EncoderModule(nn.Module):
 
     def forward(self, x):
         if self.engine is None:
-            raise RuntimeError("the SAM image encoder runs on the B200 engine only: call sam.to('cuda') first "
+            raise RuntimeError("the SAM image encoder runs on the H100 engine only: call sam.to('cuda') first "
                                "(there is no CPU fallback)")
         return self.engine(x)
 

@@ -14,7 +14,7 @@ and, for the encode side (`prepare_masked_image_latents`, utils/...inpaint.py:10
     Encoder.forward               model.py:519-543
     Downsample.forward            model.py:79-86     F.pad(x, (0,1,0,1)) -> conv3x3 stride 2 pad 0 (ea_gemm CONV_S2A)
     DiagonalGaussianDistribution  ldm/modules/distributions/distributions.py:24-45  mean, logvar.clamp(-30, 20)
-Execution: channels-last half activations, fp32 accumulation; every 3x3 convolution is the tcgen05
+Execution: channels-last half activations, fp32 accumulation; every 3x3 convolution is the wgmma
 implicit GEMM (ea_gemm CONV_S1), the 1x1 shortcut of a channel-changing ResnetBlock rides along as extra
 K columns of conv2, GroupNorm + swish is one fused launch, and the single-head d = 512 attention is two
 plain GEMMs around a row-softmax kernel (fp32 logits).  The last convolution (128 -> 3) is padded to 8

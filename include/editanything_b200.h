@@ -1,4 +1,4 @@
-/* editanything_b200.h — C ABI of libea_b200.so (B200 / sm_100a only).
+/* editanything_b200.h — C ABI of libea_b200.so (H100 / sm_90a only).
  *
  * The reference (sail-sg/EditAnything @ 8d2db4ae) is pure Python and has no FFI, plugin or
  * operator-registration interface (SURVEY.md §2, §8b): its hot path bottoms out in torch.nn
@@ -49,7 +49,7 @@ void ea_set_pdl(int on);              /* programmatic dependent launch between c
                                          (default on; env EA_PDL=0 disables) */
 void ea_reset_launch_count(void);
 
-/* ---- ea_gemm: tcgen05 GEMM / implicit-GEMM convolution ------------------------------------
+/* ---- ea_gemm: wgmma GEMM / implicit-GEMM convolution --------------------------------------
  * out[M,N] = epilogue( A[M,K] * W[N,K]^T )
  * Replaces: nn.Linear / 1x1 nn.Conv2d / 3x3 nn.Conv2d (stride 1 and 2, pad 1) of
  *   ResBlock._forward            ldm/modules/diffusionmodules/openaimodel.py:254-274
@@ -108,13 +108,10 @@ typedef struct ea_gemm_args {
   int force_bn;              /* 0 = auto; else 32/64/128/256 (testing) */
   int force_stages;          /* 0 = auto */
   int force_splits;          /* 0 = auto; 1 = never split K; n = split K n ways (testing) */
-  int force_2cta;            /* 0 = auto; 1 = CTA pairs (tcgen05 cta_group::2, M = 256); -1 = never */
+  int force_2cta;            /* ignored (kept for ABI compatibility) */
   int no_spin;               /* 1: split-K without the sibling wait - the last split CTA to arrive reduces
                                 the whole tile (required when other streams run kernels concurrently) */
-  int force_persistent;      /* 0 = auto (only with EA_GEMM_PERSIST=1|2 in the environment); 1 = persistent kernel
-                                (one CTA per SM walks the tile list with two TMEM accumulators: EXPERIMENTAL,
-                                see DESIGN.md section 8) when the launch qualifies; 2 = the same with eight
-                                epilogue warps (two per SM sub-partition); -1 = never */
+  int force_persistent;      /* > 0: one CTA per SM walks the tile list (no split-K); 0 / -1 = one tile per CTA */
   /* LayerNorm folded into the GEMMs around it (BasicTransformerBlock norm1/2/3, ldm/modules/attention.py:
    * 263-275): LN(x) W^T = rstd[m] * (x (W*gamma)^T - mean[m] * g) + (W beta + b), g[n] = sum_k (W*gamma)[n,k].
    * The GEMM that PRODUCES x (proj_in / to_out + residual) also writes per-row partial statistics of the
@@ -135,7 +132,7 @@ typedef struct ea_gemm_args {
   const void* prefetch[3];     /* optional L2 prefetch hints: up to EA_GEMM_MAX_PREFETCH ranges of device memory that a LATER */
   long long prefetch_bytes[3]; /* launch will read (its weights) - the first CTAs of this launch issue
                                   cp.async.bulk.prefetch.L2 over them while they work, so HBM streams the next layer's
-                                  weights into the 126 MB L2 behind this layer's math.  Never changes results.
+                                  weights into the 50 MB L2 behind this layer's math.  Never changes results.
                                   NULL / 0 = unused slot. */
   void* workspace;           /* optional device scratch for split-K (small-M, weight-bound layers): */
   long long workspace_bytes; /* first 64 KB = int counters that MUST be zero before the first use

@@ -13,6 +13,8 @@ import sys
 
 import torch
 
+from oracle.make_golden import golden_sample
+
 from editanything_b200.sam_spec import SAM_TINY, SAM_VIT_H, make_sam_state_dict
 from oracle import sam_oracle as S
 
@@ -40,6 +42,10 @@ def run_case(name, spec):
         out = m(img).last_hidden_state
     rec = {"meta": dict(name=name, B=B, weight_seed=wseed, image_seed=iseed, generator="transformers SamVisionEncoder"),
            "embedding": out.to(torch.float16) if cfg.embed_dim >= 1280 else out.clone()}
+    if name == "sam_vit_h":   # files stay below 1 MB: a fixed, seeded sample of 96 of the 256 channels
+        idx = golden_sample(rec["embedding"].shape[1], 96, 1024)
+        rec["embedding"] = rec["embedding"].index_select(1, idx).clone()
+        rec["embedding_index"] = (1, idx)
     torch.save(rec, os.path.join(GOLD, name + ".pt"))
     print(name, tuple(out.shape), float(out.abs().max()), float(out.std()))
 

@@ -11,6 +11,8 @@ import sys
 
 import torch
 
+from oracle.make_golden import golden_sample
+
 from editanything_b200.vae_spec import SD_VAE, VAE_TINY, make_vae_state_dict
 from oracle import vae_oracle as V
 
@@ -36,6 +38,10 @@ def run_case(name, spec):
                         raw_std=float(raw.std())),
            "image": img.to(torch.float16) if side >= 64 else img.clone(),
            "raw_center": raw[:, :, raw.shape[2] // 2 - 8:raw.shape[2] // 2 + 8, raw.shape[3] // 2 - 8:raw.shape[3] // 2 + 8].clone()}
+    if side >= 64:   # files stay below 1 MB: a fixed, seeded sample of half of the image rows
+        idx = golden_sample(rec["image"].shape[2], rec["image"].shape[2] // 2, 512)
+        rec["image"] = rec["image"].index_select(2, idx).clone()
+        rec["image_index"] = (2, idx)
     torch.save(rec, os.path.join(GOLD, name + ".pt"))
     print(name, tuple(img.shape), "raw abs max", float(raw.abs().max()), "raw std", float(raw.std()),
           "fraction clamped", float(((raw / 2 + 0.5) < 0).float().mean() + ((raw / 2 + 0.5) > 1).float().mean()))

@@ -1,16 +1,14 @@
 """`EditAnythingLoraModel.process` (SURVEY.md §8b row B1, editanything_b200/app.py):
-  1. against the REFERENCE's own `process` (the method's source compiled out of /root/reference/editany_lora.py,
-     unmodified; the pipelines replaced by spies): both must hand the pipelines the same tensors, PIL images,
-     scales, generator state - i.e. identical pre-processing, control map, inpaint condition, prompt windows, RNG
-     consumption and tile-pass arguments - and return the same structure;
+  1. against the REFERENCE's own `process` (run once with the pipelines replaced by spies by
+     oracle/make_golden_host.py, which stored bit-exact fingerprints of every pipeline call and of the result in
+     tests/golden/host_reference.pt): both must hand the pipelines the same tensors, PIL images, scales, generator
+     state - i.e. identical pre-processing, control map, inpaint condition, prompt windows, RNG consumption and
+     tile-pass arguments - and return the same structure;
   2. end to end on synthetic tiny networks (engines on the CPU emulation of the operators), replaying an
      `input_data.pkl` synthesised the way the reference's decorator writes it (annotator/util.py:75-93)."""
-import ast
 import os
 import pickle
 import random
-import sys
-import textwrap
 from types import SimpleNamespace
 
 import numpy as np
@@ -19,10 +17,6 @@ import torch
 from PIL import Image
 
 from editanything_b200 import app, host
-
-REF = os.environ.get("EA_REFERENCE_ROOT", "/root/reference")
-needs_ref = pytest.mark.skipif(not os.path.isfile(os.path.join(REF, "editany_lora.py")), reason="reference tree not present")
-
 
 class _Ids(torch.Tensor):
     """input_ids that survive `.to("cuda")` on a CPU-only box."""
@@ -111,76 +105,34 @@ def _model(cls_or_obj, pipe, tile):
     return m
 
 
-def _reference_class():
-    """The reference's EditAnythingLoraModel with ONLY `process`, `get_sam_control` (their unmodified source) and
-    the module-level helpers they call, compiled in a namespace of stand-ins for the absent third-party imports."""
-    if REF not in sys.path:
-        sys.path.insert(0, REF)
-    import annotator.util as U
-    import cv2
-    import einops
-    src = open(os.path.join(REF, "editany_lora.py")).read()
-    tree = ast.parse(src)
-    ns = {"np": np, "torch": torch, "cv2": cv2, "einops": einops, "random": random, "Image": Image, "PIL": __import__("PIL"),
-          "os": os, "HWC3": U.HWC3, "resize_image": U.resize_image, "get_bounding_box": U.get_bounding_box,
-          "seed_everything": host.seed_everything, "StableDiffusionControlNetInpaintMixingPipeline": type("Mix", (), {}),
-          "prepare_mask_image": None, "obtain_generation_model": None}
-    __import__("PIL.Image")
-    for node in tree.body:
-        if isinstance(node, ast.FunctionDef) and node.name in ("show_anns", "make_inpaint_condition", "get_pipeline_embeds"):
-            exec(compile(ast.Module([node], []), "editany_lora.py", "exec"), ns)
-        if isinstance(node, ast.ClassDef) and node.name == "EditAnythingLoraModel":
-            keep = [n for n in node.body if isinstance(n, ast.FunctionDef) and n.name in ("process", "get_sam_control")]
-            for n in keep:
-                n.decorator_list = []          # @torch.inference_mode() / @save_input_to_file: not part of the arithmetic
-            node.body = keep
-            exec(compile(ast.Module([node], []), "editany_lora.py", "exec"), ns)
-    return ns["EditAnythingLoraModel"]
+def run_process(cls):
+    """process() of `cls` with spy pipelines on the fixed inputs: (main pipeline calls, tile calls, result)."""
+    args, kwargs = _inputs()
+    pipe, tile = SpyPipe(), SpyPipe()
+    model = _model(cls, pipe, tile)
+    np.random.seed(5)
+    return pipe.calls, tile.calls, model.process(*args, **kwargs)
 
 
-def _same(a, b, path=""):
-    if torch.is_tensor(a):
-        assert torch.is_tensor(b) and a.dtype == b.dtype and a.shape == b.shape, (path, a.dtype, getattr(b, "dtype", None))
-        assert torch.equal(a.cpu(), b.cpu()), path
-    elif isinstance(a, Image.Image):
-        assert isinstance(b, Image.Image) and a.size == b.size and a.mode == b.mode, path
-        assert np.array_equal(np.array(a), np.array(b)), path
-    elif isinstance(a, np.ndarray):
-        assert np.array_equal(a, b), path
-    elif isinstance(a, (list, tuple)):
-        assert len(a) == len(b), path
-        for i, (x, y) in enumerate(zip(a, b)):
-            _same(x, y, f"{path}[{i}]")
-    elif isinstance(a, torch.Generator):
-        pass
-    else:
-        assert a == b, (path, a, b)
-
-
-@needs_ref
 def test_process_hands_the_pipelines_exactly_what_the_reference_does(monkeypatch):
+    from tests.test_host_semantics_cpu import fingerprint, golden
     monkeypatch.setattr(torch.Tensor, "cuda", lambda self, *a, **k: self)       # the reference hard-codes .cuda()
     monkeypatch.setenv("EA_SAVE_INPUT", "0")
-    args, kwargs = _inputs()
-    ref_pipe, ref_tile = SpyPipe(), SpyPipe()
-    ref = _model(_reference_class(), ref_pipe, ref_tile)
-    np.random.seed(5)
-    r_tile, r_res, r_masks, r_prompt = ref.process(*args, **kwargs)
-    our_pipe, our_tile = SpyPipe(), SpyPipe()
-    ours = _model(app.EditAnythingLoraModel, our_pipe, our_tile)
-    np.random.seed(5)
-    o_tile, o_res, o_masks, o_prompt = ours.process(*args, **kwargs)
-    assert len(ref_pipe.calls) == len(our_pipe.calls) == 1 and len(ref_tile.calls) == len(our_tile.calls) == 2
-    for rc, oc in zip(ref_pipe.calls + ref_tile.calls, our_pipe.calls + our_tile.calls):
+    ref = golden("process")
+    our_pipe_calls, our_tile_calls, (o_tile, o_res, o_masks, o_prompt) = run_process(app.EditAnythingLoraModel)
+    assert len(ref["calls"]) == len(our_pipe_calls) == 1 and len(ref["tile_calls"]) == len(our_tile_calls) == 2
+    for rc, oc in zip(ref["calls"] + ref["tile_calls"], our_pipe_calls + our_tile_calls):
         # the reference forwards the (unused, None-valued) reference-only keywords as well
         extra = {k: v for k, v in rc.items() if k not in oc}
         assert all(v is None or k.startswith(("attention_auto", "gn_auto", "style_fid", "reference_", "ref_")) for k, v in extra.items()), extra
         for k in oc:
-            _same(rc[k], oc[k], k)
-    _same(r_tile, o_tile, "results_tile")
-    _same(r_res, o_res, "results")
-    _same(r_masks, o_masks, "[full_segmask, mask]")
-    assert r_prompt == o_prompt
+            assert fingerprint(oc[k]) == rc[k], k
+    assert fingerprint(o_tile) == ref["results_tile"]
+    assert fingerprint(o_res) == ref["results"]
+    assert fingerprint(o_masks) == ref["masks"]
+    assert o_prompt == ref["prompt"]
+    our_pipe = SimpleNamespace(calls=our_pipe_calls)
+    our_tile = SimpleNamespace(calls=our_tile_calls)
     main = our_pipe.calls[0]
     assert main["controlnet_conditioning_image"][0].dtype == torch.float16
     assert float(main["controlnet_conditioning_image"][0].max()) > 1.5          # the id map is NOT normalised

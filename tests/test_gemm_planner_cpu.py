@@ -1,14 +1,16 @@
 """ea_gemm_plan (no GPU needed): invariants of the launch planner over the GEMM shapes of the
 BASELINE.json configs (SD1.5 512x512 / 1024x1024, SD2.1 768x768 N=4, SAM ViT-H, the VAE): tile widths the
-kernel supports, stage counts that fit shared memory, split-K grids that are fully resident (the
-spinning fix-up waits for sibling CTAs), GEGLU tiles of exactly 128 columns."""
+planner may pick (32 / 64 / 128: the kernel's register budget), one CTA per SM, stage rings that fit the 216 KB
+ring of the kernel's shared memory, split-K grids that are fully resident (the spinning fix-up waits for sibling
+CTAs), GEGLU tiles of exactly 128 columns."""
 import ctypes as C
 import itertools
 
 from editanything_b200 import _lib
 
 WS = 48 * 1024 * 1024 + 65536
-N_SM = 148
+N_SM = 132
+RING = 216 * 1024      # GEMM_SMEM_RING of ea_gemm.cu
 
 
 def _plan(mt, N, kb, act=0, ws=WS):
@@ -30,14 +32,13 @@ def test_plans_are_launchable():
     for M, N, kb in _shapes():
         mt = (M + 127) // 128
         bn, stages, splits, kbps, occ, two = _plan(mt, N, kb)
-        assert 32 <= bn <= 256 and bn % 32 == 0, (M, N, kb, bn)
+        assert bn in (32, 64, 128), (M, N, kb, bn)
         assert bn == 32 or N > bn - 32, "a narrower tile would cover N"
-        assert 2 <= stages <= 8 and occ in (1, 2) and two in (0, 1)
-        stage_bytes = 128 * 128 + (bn // 2 if two else bn) * 128
-        assert stages * stage_bytes <= (111 if occ == 2 else 224) * 1024, (M, N, kb, bn, stages, occ)
+        assert 2 <= stages <= 8 and occ == 1 and two == 0
+        stage_bytes = 128 * 128 + bn * 128
+        assert stages * stage_bytes <= RING, (M, N, kb, bn, stages)
+        assert stages <= max(kb, 2), "no more stages than K-blocks"
         assert splits >= 1 and kbps * splits >= kb and kbps * (splits - 1) < kb, (kb, splits, kbps)
-        if two:
-            assert splits == 1 and bn >= 64 and mt >= 2
         if splits > 1:
             tiles = mt * ((N + bn - 1) // bn)
             assert tiles * splits <= occ * N_SM, ("split CTAs must all be resident", M, N, kb, bn, splits, occ)

@@ -1,6 +1,6 @@
 """-m gpu: the whole request path on CUDA with synthetic tiny weights - what `editany_nogradio.py` does
 (editany_nogradio.py:1-15): build `EditAnythingLoraModel`, replay an `input_data.pkl`, get (refined, output,
-[segmask, mask], prompt) - with the SAM stand-in (`segment_anything` shim: B200 image encoder + PyTorch prompt
+[segmask, mask], prompt) - with the SAM stand-in (`segment_anything` shim: H100 image encoder + PyTorch prompt
 encoder / mask decoder / automatic mask generator), the UniPC scheduler and the shared-UNet tile pipeline."""
 import pickle
 

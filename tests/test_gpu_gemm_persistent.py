@@ -1,6 +1,7 @@
-"""-m gpu: the persistent GEMM variant (ea_gemm_args.force_persistent = 1 | 2; the default for launches whose
-tile list balances over the SMs, DESIGN.md section 4) against the one-tile-per-CTA kernel on the same inputs.  Both compute every output element with the same K order in fp32, so the results
-must agree to the last bit; grids are chosen to give every CTA several tiles (both TMEM accumulators, barrier
+"""-m gpu: the persistent GEMM variant (ea_gemm_args.force_persistent = 1 | 2: one CTA per SM walks the tile list)
+against the one-tile-per-CTA kernel on the same inputs.  Both compute every output element with the same K order in
+fp32, so the results
+must agree to the last bit; grids are chosen to give every CTA several tiles (the ring's barrier
 phase wrap-around) and a ragged last wave."""
 import pytest
 import torch
@@ -18,7 +19,7 @@ def _pair(fn):
     return a, b
 
 
-@pytest.mark.parametrize("variant", [1, 2])      # 1: four epilogue warps, 2: eight (two warp-groups)
+@pytest.mark.parametrize("variant", [1, 2])
 @pytest.mark.parametrize("M,N,K,res,act", [
     (8192, 2560, 320, False, "geglu"),      # 1280 tiles: ~9 per CTA
     (8192, 960, 320, False, "none"),        # qkv at 64x64

@@ -1,7 +1,6 @@
 """-m gpu: the `editany_nogradio.py` flow on CUDA (real kernels, synthetic test-sized checkpoints on disk):
 constructor -> from_pretrained x 2 pipelines + 3 ControlNets -> SAM checkpoint -> input_data.pkl -> process().
-The script text is this repo's wording of the reference's 15-line entry point (the reference file itself is run by
-tests/test_nogradio_cpu.py where /root/reference exists; it does not exist on the GPU box)."""
+The script text is this repo's wording of the reference's 15-line entry point (tests/test_nogradio_cpu.SCRIPT)."""
 import pickle
 
 import numpy as np

@@ -1,6 +1,6 @@
 """The `segment_anything` stand-in (editanything_b200/segment_anything): prompt encoder + two-way mask decoder against
 the in-container HF port of the same network (transformers.models.sam) with the same weights; the automatic mask
-generator's pure helpers; the predictor / generator plumbing with a stub image encoder (the real one is the B200
+generator's pure helpers; the predictor / generator plumbing with a stub image encoder (the real one is the H100
 engine: tests/test_gpu_sam.py).  Upstream `segment_anything` is absent: parity unpinned against it."""
 import numpy as np
 import pytest

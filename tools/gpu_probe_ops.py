@@ -99,39 +99,6 @@ def case_gemm_splitk():
     return res
 
 
-def case_gemm_2cta():
-    """CTA-pair mode (tcgen05 cta_group::2): linear (even / odd number of M tiles, ragged M and N),
-    epilogue variants, and a forced tile width."""
-    import torch
-    from editanything_b200 import ops
-    dt = ops.half_dtype()
-    torch.manual_seed(14)
-    res, worst = {}, 0.0
-    for (M, N, K, bn) in [(256, 256, 256, 0), (1024, 320, 640, 0), (1000, 320, 328, 0), (384, 640, 1280, 0),
-                          (8192, 320, 2880, 160), (2048, 1280, 512, 256), (640, 192, 64, 64)]:
-        a = torch.randn(M, K, device="cuda").to(dt)
-        w = (torch.randn(N, K, device="cuda") / K ** 0.5).to(dt)
-        bias = torch.randn(N, device="cuda")
-        resid = torch.randn(M, N, device="cuda").to(dt)
-        out = torch.full((M, N), 7.0, device="cuda", dtype=dt)
-        ops.gemm(a, w, out, bias=bias, residual=resid, force_2cta=1, force_bn=bn)
-        torch.cuda.synchronize()
-        e = _err(out, a.float() @ w.float().t() + bias + resid.float())
-        res[f"{M}x{N}x{K}/bn{bn}"] = e
-        worst = max(worst, e["max_abs"] / max(1.0, e["ref_max"]))
-    res["max_abs"], res["ref_max"] = worst, 1.0
-    return res
-
-
-def case_conv_2cta():
-    r1 = _conv_case(2, 64, 64, 320, 320, force_2cta=1)
-    r2 = _conv_case(2, 16, 16, 1280, 1280, extra=1920, force_2cta=1)
-    r3 = _conv_case(1, 96, 96, 64, 64, force_2cta=1)
-    r4 = _conv_case(1, 8, 8, 128, 64, force_2cta=1)      # a single M tile: phantom peer tile
-    w = max(r["max_abs"] / max(1.0, r["ref_max"]) for r in (r1, r2, r3, r4))
-    return {"max_abs": w, "ref_max": 1.0, "conv64": r1, "conv16_skip": r2, "conv96": r3, "conv8_b1": r4}
-
-
 def case_concurrent_variants():
     """The no-inter-CTA-wait variants used when several streams run concurrently: two-pass GroupNorm
     and split-K whose last-arriving CTA reduces the tile (ops.set_lane(lane, True))."""
@@ -217,7 +184,7 @@ def case_gemm_accum_scale_dual():
             "ref_max": e1["ref_max"]}
 
 
-def _conv_case(B, H, W, Cin, Cout, stride=1, extra=0, seed=4, force_2cta=0):
+def _conv_case(B, H, W, Cin, Cout, stride=1, extra=0, seed=4):
     import torch
     import torch.nn.functional as F
     from editanything_b200 import ops, _lib as L
@@ -241,7 +208,7 @@ def _conv_case(B, H, W, Cin, Cout, stride=1, extra=0, seed=4, force_2cta=0):
     wp = wp.contiguous()
     out = torch.empty(B * H * W, Cout, device="cuda", dtype=dt)
     ops.gemm(x_nhwc, wp, out, mode=L.EA_GEMM_CONV_S1 if stride == 1 else L.EA_GEMM_CONV_S2,
-             conv=(B, H, W, Cin), a_extra=xe, bias=bias, rowvec=rv, force_2cta=force_2cta)
+             conv=(B, H, W, Cin), a_extra=xe, bias=bias, rowvec=rv)
     torch.cuda.synchronize()
     ref = ref.permute(0, 2, 3, 1).reshape(B * H * W, Cout)
     return _err(out, ref)
@@ -689,10 +656,6 @@ def case_grouped_linear():
 
 def case_grouped_linear_persistent():
     return _grouped_case("linear", seed=32, force_persistent=2)
-
-
-def case_grouped_linear_2cta():
-    return _grouped_case("linear", seed=33, force_persistent=-1, force_2cta=1)
 
 
 def case_grouped_geglu_persistent():
