@@ -14,6 +14,15 @@ The semantics (call order, RNG consumption, dtypes, un-normalised 0..255 control
 PIL mask round trip, one shared generator across the main and the tile pass) follow the reference line by line;
 the code is this package's own.
 
+Base models: SD1.5-style 4-channel UNets, and the 9-channel stabilityai/stable-diffusion-2-inpainting with the SD2.1
+EditAnything ControlNets (sam2groundingdino_edit.py:36-44), e.g.
+
+    EditAnythingLoraModel(base_model_path="stabilityai/stable-diffusion-2-inpainting",
+                          controlmodel_name="LAION Pretrained(v0-4)-SD21", extra_inpaint=False, use_blip=False,
+                          lora_model_path=None)
+
+whose tile pass loads runwayml/stable-diffusion-v1-5 separately (editany_lora.py:395-405).
+
 Not supported here (raise NotImplementedError instead of diverging silently): reference-only mode (`ref_image`),
 `enable_all_generate` (the text-to-image ControlNet pipeline), LoRA merging, the alpha-mixing pipeline.
 """
@@ -88,7 +97,9 @@ def obtain_generation_model(base_model_path, lora_model_path, controlnet_path, g
 
 def obtain_tile_model(base_model_path, lora_model_path, lora_weight=1.0, share_with=None):
     """editany_lora.py:391-423.  `share_with`: a pipeline whose UNet / VAE / text encoder are reused when it was
-    built from the same base model (the tile pass runs the same SD1.5 weights: 1.7 GB of HBM saved)."""
+    built from the same base model directory (the tile pass runs the same SD1.5 weights: 1.7 GB of HBM saved).  An
+    SD2-inpainting main pipeline is not shared: its tile pass runs on SD1.5 (editany_lora.py:395-405)."""
+    from .loading import resolve_model_path
     from .pipeline import ControlNetModel2, StableDiffusionControlNetInpaintPipeline
     from .schedulers import UniPCMultistepScheduler
     if lora_model_path is not None:
@@ -96,6 +107,9 @@ def obtain_tile_model(base_model_path, lora_model_path, lora_weight=1.0, share_w
     controlnet = ControlNetModel2.from_pretrained(TILE_CONTROLNET, torch_dtype=torch.float16)
     if base_model_path in ("runwayml/stable-diffusion-v1-5", "stabilityai/stable-diffusion-2-inpainting"):
         base_model_path = "runwayml/stable-diffusion-v1-5"
+    if share_with is not None and getattr(share_with, "base_model_dir", None) != \
+            os.path.realpath(resolve_model_path(base_model_path)):
+        share_with = None
     pipe = StableDiffusionControlNetInpaintPipeline.from_pretrained(base_model_path, controlnet=controlnet,
                                                                    torch_dtype=torch.float16, safety_checker=None,
                                                                    share_with=share_with)

@@ -13,7 +13,7 @@ import torch
 
 from ._backend import default_ops, engine_call
 from .nets import PackedNet, UNetRunner
-from .unet_spec import UNetConfig
+from .unet_spec import UNetConfig, controlnet_config
 
 
 def ddim_schedule(num_steps, linear_start=0.00085, linear_end=0.012, T=1000):
@@ -33,10 +33,13 @@ class DenoiseEngine:
     def __init__(self, cfg: UNetConfig, unet_sd, controlnet_sds, device, backend=None, unet_packed=None):
         """unet_packed: an already packed UNet (another engine's `.unet`) to share instead of packing `unet_sd`
         again - the reference's tile pipeline runs the same base model as the main one (editany_lora.py:395-405)."""
+        if cfg.in_channels not in (4, 9):
+            raise ValueError(f"the UNet takes 4 latent channels, or 9 (latents, mask, masked-image latents) for an "
+                             f"inpainting base model; got in_channels={cfg.in_channels}")
         self.cfg, self.dev = cfg, device
         self.ops = backend or default_ops()
         self.unet = unet_packed if unet_packed is not None else PackedNet(cfg, "unet", unet_sd, device, backend)
-        self.cns = [PackedNet(cfg, "controlnet", sd, device, backend) for sd in controlnet_sds]
+        self.cns = [PackedNet(controlnet_config(cfg), "controlnet", sd, device, backend) for sd in controlnet_sds]
         self.runner = UNetRunner(self.unet, self.cns, device)
         self.hdt = self.unet.hdt
         self._graph = None
@@ -163,6 +166,28 @@ class DenoiseEngine:
         for buf, r in zip(self.emb_bufs, self._emb_rows(t)):
             buf.copy_(r)
 
+    def _condition(self, mask_n1hw, masked_latents_nchw):
+        """conv_in's contribution of the condition channels of a 9-channel UNet: [B, h, w, mc] (half)."""
+        m = mask_n1hw.to(self.dev, torch.float32)
+        z = masked_latents_nchw.to(self.dev, torch.float32)
+        c = torch.cat([m, z, torch.zeros_like(z[:, :3])], 1).permute(0, 2, 3, 1).contiguous()
+        return self.unet.precompute_condition(c)
+
+    @engine_call
+    def set_unet_condition(self, mask_n1hw, masked_latents_nchw):
+        """The per-request input of a 9-channel (inpainting) UNet: the mask resized to the latents [N, 1, h, w] and
+        the VAE latents of the masked image [N, 4, h, w] (utils/...inpaint.py:1448-1468), for the N images.  They
+        are the same at every step (:1550-1558), so their part of conv_in, bias included, is computed here once;
+        the CFG duplication is done here too.  Each step's conv_in then reads the 4 latent channels only."""
+        if self.unet.x_channels == self.cfg.in_channels:
+            raise ValueError(f"set_unet_condition needs a 9-channel UNet, this one takes {self.cfg.in_channels}")
+        if mask_n1hw.shape[1] != 1 or masked_latents_nchw.shape[1] != 4 or \
+                mask_n1hw.shape[0] != masked_latents_nchw.shape[0] or mask_n1hw.shape[2:] != masked_latents_nchw.shape[2:]:
+            raise ValueError(f"mask {tuple(mask_n1hw.shape)} / masked-image latents {tuple(masked_latents_nchw.shape)}: "
+                             "expected [N, 1, h, w] and [N, 4, h, w]")
+        g = self._condition(mask_n1hw, masked_latents_nchw)
+        self._keep("cond_in", torch.cat([g, g]))
+
     # -- the sampling schedule as device tables -------------------------------------------------
     @engine_call
     def set_schedule(self, timesteps, alphas, alphas_prev, blend=None, multistep=None):
@@ -205,12 +230,20 @@ class DenoiseEngine:
     @engine_call
     def eps(self, x_nchw, t):
         """eps = unet(x, t, ctx, control=sum_k scale_k * controlnet_k(x, hint_k, t, ctx)) as fp32
-        NCHW - the quantity the reference calls `noise_pred` before guidance."""
+        NCHW - the quantity the reference calls `noise_pred` before guidance.  For a 9-channel UNet x is
+        cat([latents, mask, masked-image latents]) (utils/...inpaint.py:1550-1558) and the ControlNets see
+        x[:, :4] (:1607-1615)."""
         B, C, H, W_ = x_nchw.shape
+        if C != self.cfg.in_channels:
+            raise ValueError(f"x has {C} channels, the UNet takes {self.cfg.in_channels}")
+        cond = None
+        if C != self.unet.x_channels:
+            cond = self._condition(x_nchw[:, 4:5], x_nchw[:, 5:9])
+            x_nchw = x_nchw[:, :4]
         xh = x_nchw.to(self.dev).permute(0, 2, 3, 1).contiguous().to(self.hdt)
         self._fill_emb(t)
         xn = self.runner.eps_features(xh, self.t_dev, self.ctx_cache, self.hints, self.scales, self.gn_ws,
-                                      embs=self.emb_bufs, ctx_ls=self.ctx_ls)
+                                      embs=self.emb_bufs, ctx_ls=self.ctx_ls, cond_in=cond)
         eps = torch.empty(B, H, W_, 4, device=self.dev, dtype=torch.float32)
         self.ops.out_cfg_ddim(xn, self.unet.w["out.w"], self.unet.w["out.cb"], eps_out=eps, Nimg=B // 2, H=H,
                               W=W_, C_=self.cfg.model_channels)
@@ -222,11 +255,18 @@ class DenoiseEngine:
         self.ops.step_gather(self.step_ctr, self._sched_cap, [self.coef_tab] + self.emb_tabs,
                              [self.coef_dev] + self.emb_bufs)
         xn = self.runner.eps_features(self.x_half, self.t_dev, self.ctx_cache, self.hints, self.scales, self.gn_ws,
-                                      embs=self.emb_bufs, ctx_ls=self.ctx_ls)
+                                      embs=self.emb_bufs, ctx_ls=self.ctx_ls, cond_in=self._step_cond())
         self.ops.out_cfg_ddim(xn, self.unet.w["out.w"], self.unet.w["out.cb"], latents=self.lat,
                               coef=self.coef_dev, guidance=self.guidance, known=self.known, noise=self.noise,
                               mask=self.mask, lat_half_out=self.x_half, step_counter=self.step_ctr, hist=self.hist,
                               Nimg=self.B // 2, H=H, W=W_, C_=self.cfg.model_channels)
+
+    def _step_cond(self):
+        if self.unet.x_channels == self.cfg.in_channels:
+            return None
+        if getattr(self, "cond_in", None) is None:
+            raise RuntimeError("a 9-channel UNet needs set_unet_condition() before the first step")
+        return self.cond_in
 
     @engine_call
     def begin(self, latents_nchw, guidance, known_nchw=None, mask_n1hw=None, noise_nchw=None, use_graph=True):

@@ -16,6 +16,7 @@ Reference semantics followed (paths relative to the reference root):
     BasicTransformerBlock         ldm/modules/attention.py:271-275
 """
 import os
+from dataclasses import replace
 
 import torch
 
@@ -51,6 +52,8 @@ class PackedNet:
         self.dev = device
         self.hdt = self.ops.half_dtype()
         self.topo = build_topology(cfg, with_decoder=(kind == "unet"))
+        # channels of the per-step input x: the latents only, also for a 9-channel inpainting UNet
+        self.x_channels = 4 if (kind == "unet" and cfg.in_channels == 9) else cfg.in_channels
         sd = state_dict
         self.w = {}
         H, F = self._half, self._f32
@@ -77,7 +80,16 @@ class PackedNet:
         for b in blocks:
             p = b.prefix
             if b.kind == "conv_in":
-                self.w[p + ".w"] = F(sd[p + ".weight"].permute(2, 3, 1, 0))  # [k,k,Cin,Cout]
+                wt = sd[p + ".weight"]
+                if self.x_channels != b.cin:
+                    # 9-channel UNet: conv(cat[x, c], W) + b = conv(x, W_x) + (conv(c, W_c) + b).  W_x (the latent's
+                    # 4 channels) runs every step; W_c (mask + masked-image latents, zero-padded to 8 channels) runs
+                    # once per request in precompute_condition and is added through conv_in's `add`
+                    wc = torch.zeros(wt.shape[0], 8, 3, 3, dtype=wt.dtype, device=wt.device)
+                    wc[:, :b.cin - 4] = wt[:, 4:]
+                    self.w[p + ".wc"] = F(wc.permute(2, 3, 1, 0))
+                    wt = wt[:, :4]
+                self.w[p + ".w"] = F(wt.permute(2, 3, 1, 0))  # [k,k,Cin,Cout]
                 self.w[p + ".b"] = F(sd[p + ".bias"])
             elif b.kind == "res":
                 for n in ("in_layers.0", "out_layers.0"):
@@ -218,6 +230,21 @@ class PackedNet:
                        act=L.EA_ACT_SILU if i != n - 1 else L.EA_ACT_NONE)
             x, cin, Hh, Wh = y, cout, Ho, Wo
         return x
+
+    def precompute_condition(self, c_nhwc):
+        """conv(c, W_c) + b of a 9-channel UNet's conv_in for c = [mask, masked-image latents, 0, 0, 0] (NHWC, 8
+        channels): constant over the denoising loop (utils/...inpaint.py:1550-1558 concatenates the same mask and
+        masked-image latents every step), so it is computed once per request and added to the per-step conv_in."""
+        B, H, W_, C = c_nhwc.shape
+        if self.x_channels == self.cfg.in_channels or C != 8:
+            raise ValueError(f"precompute_condition needs a 9-channel UNet and an 8-channel input, got {C} channels "
+                             f"for in_channels={self.cfg.in_channels}")
+        p = self.topo.input_blocks[0][0].prefix
+        cout = self.cfg.model_channels
+        out = self._new(B, H, W_, cout)
+        self.ops.conv_in(c_nhwc.to(self.hdt).contiguous(), self.w[p + ".wc"], self.w[p + ".b"], out, B=B, H=H, W=W_,
+                         Cin=8, Cout=cout)
+        return out
 
     # ------------------------------------------------------------------ execution
     def _emb(self, t_dev, B):
@@ -422,11 +449,14 @@ class UNetRunner:
         self._streams = []
         self._lane_gn = {}
         # Lockstep: the UNet encoder and the ControlNets as ONE sequence of grouped launches (BlockRunner) instead of
-        # one stream per network.  Needs identical topologies, the LayerNorm fold and at most 3 networks
-        # (ea_gemm_grouped); EA_LOCKSTEP=0 falls back to the concurrent streams (A/B).
+        # one stream per network.  Needs identical topologies (conv_in, run per network, may differ in its input
+        # channels), the LayerNorm fold and at most 3 networks (ea_gemm_grouped); EA_LOCKSTEP=0 falls back to the
+        # concurrent streams (A/B).
         nets = [unet] + self.cns
+        same = replace(unet.cfg, in_channels=0)
         self.lockstep = (os.environ.get("EA_LOCKSTEP", "1") != "0" and 2 <= len(nets) <= 3 and unet.ln_fold
-                         and all(n.cfg == unet.cfg and n.ln_fold for n in nets) and hasattr(self.ops, "gemm_grouped"))
+                         and all(replace(n.cfg, in_channels=0) == same and n.ln_fold for n in nets)
+                         and hasattr(self.ops, "gemm_grouped"))
         self._ls_ws = {}
 
     def _lane_ws(self, B, n):
@@ -437,10 +467,11 @@ class UNetRunner:
         return self._lane_gn[key]
 
     def _encoder(self, net: PackedNet, x_half, emb_all, ctxc, gn_ws, guided_hint=None, sinks=None, scale=1.0,
-                 deferred=None):
+                 deferred=None, cond_in=None):
         """Runs input_blocks + middle.  For the UNet (`sinks` is a dict of concat slots) each skip is
         dual-stored into its decoder concat slot; for a ControlNet each zero-conv accumulates
-        `scale * zero_conv(h)` into the slot instead of materialising the residual."""
+        `scale * zero_conv(h)` into the slot instead of materialising the residual.  cond_in: a 9-channel UNet's
+        conv_in contribution of the condition channels, bias included (PackedNet.precompute_condition)."""
         o, w, topo = net.ops, net.w, net.topo
         B, H, W_, _ = x_half.shape
         is_unet = net.kind == "unet"
@@ -450,7 +481,10 @@ class UNetRunner:
             if layers[0].kind == "conv_in":
                 blk = layers[0]
                 h = net._new(B, H, W_, blk.cout)
-                if blk.cin in (4, 8):
+                if cond_in is not None:
+                    o.conv_in(x_half, w[blk.prefix + ".w"], None, h, B=B, H=H, W=W_, Cin=net.x_channels,
+                              Cout=blk.cout, out2=slot, ldo2=slot.stride(2), add=cond_in)
+                elif blk.cin in (4, 8):
                     o.conv_in(x_half, w[blk.prefix + ".w"], w[blk.prefix + ".b"], h, B=B, H=H, W=W_, Cin=blk.cin,
                               Cout=blk.cout, out2=slot if is_unet else None,
                               ldo2=slot.stride(2) if is_unet else 0, add=guided_hint)
@@ -523,10 +557,11 @@ class UNetRunner:
                     kv[p] = out
         return {"kv": kv, "B": n * B, "L": Lc}
 
-    def _encoder_lockstep(self, x_half, embs, ctx_ls, hints, sinks, scales):
+    def _encoder_lockstep(self, x_half, embs, ctx_ls, hints, sinks, scales, cond_in=None):
         """input_blocks + middle of the UNet and every ControlNet in lockstep (see BlockRunner).  The UNet's skips are
         dual-stored into the decoder's concat slots by the grouped launch itself (out2, network 0); each ControlNet's
-        zero-conv then accumulates `scale * zero_conv(h)` into the same slot (cldm/cldm.py:34-41,293-303)."""
+        zero-conv then accumulates `scale * zero_conv(h)` into the same slot (cldm/cldm.py:34-41,293-303).  cond_in:
+        as in _encoder."""
         o = self.ops
         un = self.unet
         nets = [un] + self.cns
@@ -558,10 +593,13 @@ class UNetRunner:
                 for g, nt in enumerate(nets):
                     hg = h.chunk(n, 0)[g]
                     w = nt.w
-                    if blk.cin in (4, 8):
-                        o.conv_in(x_half, w[blk.prefix + ".w"], w[blk.prefix + ".b"], hg, B=B, H=H, W=W_, Cin=blk.cin,
-                                  Cout=blk.cout, out2=slot if g == 0 else None, ldo2=slot.stride(2) if g == 0 else 0,
-                                  add=hints[g - 1] if g > 0 else None)
+                    if g == 0 and cond_in is not None:
+                        o.conv_in(x_half, w[blk.prefix + ".w"], None, hg, B=B, H=H, W=W_, Cin=nt.x_channels,
+                                  Cout=blk.cout, out2=slot, ldo2=slot.stride(2), add=cond_in)
+                    elif nt.x_channels in (4, 8):
+                        o.conv_in(x_half, w[blk.prefix + ".w"], w[blk.prefix + ".b"], hg, B=B, H=H, W=W_,
+                                  Cin=nt.x_channels, Cout=blk.cout, out2=slot if g == 0 else None,
+                                  ldo2=slot.stride(2) if g == 0 else 0, add=hints[g - 1] if g > 0 else None)
                     else:
                         o.conv_direct(x_half, w[blk.prefix + ".w"], w[blk.prefix + ".b"], hg, B=B, Hin=H, Win=W_,
                                       Cin=blk.cin, Cout=blk.cout, ksize=3, stride=1, add=hints[g - 1] if g > 0 else None)
@@ -605,12 +643,18 @@ class UNetRunner:
         per timestep instead of re-streaming ~93 MB of embedding weights every step."""
         return [n._emb(t_dev, B) for n in [self.unet] + self.cns]
 
-    def eps_features(self, x_half, t_dev, ctx_cache, hints, scales, gn_ws=None, embs=None, ctx_ls=None):
+    def eps_features(self, x_half, t_dev, ctx_cache, hints, scales, gn_ws=None, embs=None, ctx_ls=None, cond_in=None):
         """Runs UNet encoder, ControlNets, UNet decoder; returns the GroupNorm+SiLU'd input of the
-        final convolution [B,H,W,mc] (the out conv itself is fused with CFG/DDIM)."""
+        final convolution [B,H,W,mc] (the out conv itself is fused with CFG/DDIM).  x_half holds the 4 latent
+        channels; a 9-channel UNet also needs cond_in [B,H,W,mc] (PackedNet.precompute_condition)."""
         un = self.unet
         o = self.ops
         B, H, W_, _ = x_half.shape
+        if (un.x_channels != un.cfg.in_channels) != (cond_in is not None):
+            raise ValueError(f"cond_in is required by a {un.cfg.in_channels}-channel UNet exactly when it reads "
+                             "condition channels")
+        if cond_in is not None and tuple(cond_in.shape) != (B, H, W_, un.cfg.model_channels):
+            raise ValueError(f"cond_in {tuple(cond_in.shape)} does not match the latents {(B, H, W_)}")
         if gn_ws is None:
             gn_ws = o.gn_workspace(B, self.dev)
         sinks = self.alloc_sinks(B, H, W_)
@@ -621,7 +665,7 @@ class UNetRunner:
         if self.lockstep and ctx_ls is not None:
             if hasattr(o, "set_lane"):
                 o.set_lane(0, False)
-            self._encoder_lockstep(x_half, embs, ctx_ls, hints, sinks, scales)
+            self._encoder_lockstep(x_half, embs, ctx_ls, hints, sinks, scales, cond_in=cond_in)
         elif concurrent:
             # The UNet encoder and every ControlNet only READ x and write their own activations: run
             # them on parallel streams (many of their launches cannot fill 132 SMs on their own), join,
@@ -636,7 +680,7 @@ class UNetRunner:
             for s in self._streams:
                 s.wait_stream(main)
             o.set_lane(0, True)
-            self._encoder(un, x_half, emb_u, ctx_cache[0], lanes_ws[0], sinks=sinks)
+            self._encoder(un, x_half, emb_u, ctx_cache[0], lanes_ws[0], sinks=sinks, cond_in=cond_in)
             for k, cn in enumerate(self.cns):
                 with torch.cuda.stream(self._streams[k]):
                     o.set_lane(1 + k, True)
@@ -648,7 +692,7 @@ class UNetRunner:
             for a_, w_, out_, kw_ in deferred:
                 o.gemm(a_, w_, out_, **kw_)
         else:
-            self._encoder(un, x_half, emb_u, ctx_cache[0], gn_ws, sinks=sinks)
+            self._encoder(un, x_half, emb_u, ctx_cache[0], gn_ws, sinks=sinks, cond_in=cond_in)
             for k, cn in enumerate(self.cns):
                 emb_c = embs[1 + k]
                 self._encoder(cn, x_half, emb_c, ctx_cache[1 + k], gn_ws, guided_hint=hints[k], sinks=sinks,

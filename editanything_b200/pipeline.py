@@ -9,10 +9,17 @@ scheduler step -> inpaint blend) is ONE fused, CUDA-graph-replayed launch sequen
 `DenoiseEngine`.  Text encoder, tokenizer and VAE stay the caller's PyTorch modules (duck-typed, once
 per image; SURVEY.md §8 R4/R6/R17 "keep in PyTorch").
 
+Both branches of the reference are implemented, selected by `unet.config.in_channels` like there: 4 (any base
+model; the source image is encoded and blended back into the kept region) and 9 (an inpainting base model such as
+stabilityai/stable-diffusion-2-inpainting: the UNet also reads the mask and the latents of the masked image, the
+ControlNets read the 4 latent channels, and there is no blend, so `alignment_ratio` is ignored, :1448-1468,
+:1550-1560, :1647-1664).
+
 Not supported (raises NotImplementedError rather than silently diverging): the reference-only mode
-(`ref_image`, `utils/stable_diffusion_reference.py`), 9-channel inpainting UNets, guess_mode.
+(`ref_image`, `utils/stable_diffusion_reference.py`), guess_mode.
 """
 import math
+import os
 from dataclasses import dataclass
 from types import SimpleNamespace
 from typing import Any, List, Optional
@@ -166,7 +173,7 @@ class StableDiffusionControlNetInpaintPipeline:
         self.safety_checker, self.feature_extractor = safety_checker, feature_extractor
         dt = engine.hdt
         self.unet = _NetStub(engine.cfg.in_channels, dt)
-        self.controlnet = _NetStub(engine.cfg.in_channels, dt, nets=[_NetStub(4, dt) for _ in engine.cns])
+        self.controlnet = _NetStub(4, dt, nets=[_NetStub(4, dt) for _ in engine.cns])
         self.vae_scale_factor = 8 if vae is None else 2 ** (len(vae.config.block_out_channels) - 1)
 
     @classmethod
@@ -178,23 +185,31 @@ class StableDiffusionControlNetInpaintPipeline:
         components may be passed in like diffusers allows (text_encoder=, tokenizer=, vae=, scheduler=).
         `share_with`: another pipeline of the same base model whose packed UNet, VAE, text encoder and tokenizer
         are reused (the tile-refinement pipeline, editany_lora.py:391-423)."""
-        from .loading import load_pipeline_parts
+        from .loading import load_pipeline_parts, resolve_model_path, unet_config_from_diffusers, _read_json
+        from .unet_spec import controlnet_config
         dev = torch.device(device) if device is not None else torch.device("cuda:0" if torch.cuda.is_available() else "cpu")
         cns = [] if controlnet is None else (list(controlnet) if isinstance(controlnet, (list, tuple)) else [controlnet])
+        base_dir = os.path.realpath(resolve_model_path(pretrained_model_name_or_path))
         shared = share_with.engine.unet if share_with is not None else None
         if share_with is not None:
+            ucfg = unet_config_from_diffusers(_read_json(os.path.join(base_dir, "unet", "config.json")))
+            if share_with.engine.cfg != ucfg:
+                raise ValueError(f"share_with runs a UNet {share_with.engine.cfg}, the base model "
+                                 f"'{pretrained_model_name_or_path}' has {ucfg}: nothing can be shared")
             text_encoder = text_encoder or share_with.text_encoder
             tokenizer = tokenizer or share_with.tokenizer
             vae = vae or share_with.vae
         ucfg, usd, vae, text_encoder, tokenizer, sched = load_pipeline_parts(
-            pretrained_model_name_or_path, dev, text_encoder=text_encoder, tokenizer=tokenizer, vae=vae,
-            scheduler=scheduler, unet_packed=shared)
+            base_dir, dev, text_encoder=text_encoder, tokenizer=tokenizer, vae=vae, scheduler=scheduler,
+            unet_packed=shared)
         for c in cns:
-            if c.cfg != ucfg:
+            # the ControlNets of a 9-channel inpainting UNet are 4-channel nets (models/cldm_v21.yaml:44)
+            if c.cfg != controlnet_config(ucfg):
                 raise ValueError(f"ControlNet topology {c.cfg} does not match the UNet {ucfg}")
         eng = DenoiseEngine(ucfg, usd, [c.state_dict_ldm for c in cns], dev, unet_packed=shared)
         pipe = cls(eng, vae=vae, text_encoder=text_encoder, tokenizer=tokenizer, scheduler=sched,
                    safety_checker=safety_checker, feature_extractor=feature_extractor)
+        pipe.base_model_dir = base_dir
         for stub, c in zip(pipe.controlnet.nets, cns):
             stub.config = c.config
         return pipe
@@ -288,8 +303,14 @@ class StableDiffusionControlNetInpaintPipeline:
                 raise ValueError("`image` should be in range [-1, 1]")
             if mask_image.min() < 0 or mask_image.max() > 1:
                 raise ValueError("`mask_image` should be in range [0, 1]")
-        if self.unet.config.in_channels != 4:
-            raise NotImplementedError("9-channel inpainting UNets are not supported by this backend")
+        # :955-979 (a tensor mask has 1 channel, checked above; the reference's latent_channels is the VAE's 4)
+        latent_channels = getattr(getattr(self.vae, "config", None), "latent_channels", 4)
+        expected = latent_channels if self.unet.config.in_channels == 4 else 2 * latent_channels + 1
+        if expected != self.unet.config.in_channels:
+            raise ValueError(f"The config of `pipeline.unet` expects {self.unet.config.in_channels} but received"
+                             f" non inpainting latent channels: {latent_channels}, mask channels: 1, and masked image"
+                             f" channels: {latent_channels}. Please verify the config of `pipeline.unet` and the"
+                             " `mask_image` and `image` inputs.")
 
     def _default_height_width(self, height, width, image):
         """utils/...inpaint.py:1107-1127 (including its shape[3]/shape[2] swap for tensors)."""
@@ -442,16 +463,31 @@ class StableDiffusionControlNetInpaintPipeline:
         timesteps = self.scheduler.timesteps
         lat = self.prepare_latents(N, 4, height, width, edt, generator, latents)
         noise = lat
-        init_lat = self.prepare_masked_image_latents(image, N, edt, generator)
-        mh, mw = mask_image.shape[2], mask_image.shape[3]
-        # NB the reference names these (w, h) but they are (H, W) of the NCHW mask (:1484-1489)
-        m = F.interpolate(mask_image, (mh // 8, mw // 8), mode="nearest").to(lat.dtype)
-        m = 1 - m                                       # 1 = keep the original image
-        if m.shape[0] < N:
-            m = m.repeat(N // m.shape[0], 1, 1, 1)
-
         eng = self.engine
         dev = eng.dev
+        inpaint_unet = self.unet.config.in_channels != 4
+        if inpaint_unet:
+            # 9-channel branch (:1396, :1448-1468): the mask at latent size and the latents of the masked image are
+            # extra UNet inputs; the unmasked image is not encoded and nothing is blended
+            masked_image = image * (mask_image < 0.5)
+            mask_lat = F.interpolate(mask_image, size=(height // self.vae_scale_factor, width // self.vae_scale_factor))
+            mask_lat = mask_lat.to(edt)
+            if mask_lat.shape[0] < N:
+                if N % mask_lat.shape[0] != 0:
+                    raise ValueError("The passed mask and the required batch size don't match.")
+                mask_lat = mask_lat.repeat(N // mask_lat.shape[0], 1, 1, 1)
+            masked_lat = self.prepare_masked_image_latents(masked_image, N, edt, generator)
+            mask_lat, masked_lat = mask_lat.to(dev, torch.float32), masked_lat.to(dev, torch.float32)
+            alignment_ratio = None
+        else:
+            init_lat = self.prepare_masked_image_latents(image, N, edt, generator)
+            mh, mw = mask_image.shape[2], mask_image.shape[3]
+            # NB the reference names these (w, h) but they are (H, W) of the NCHW mask (:1484-1489)
+            m = F.interpolate(mask_image, (mh // 8, mw // 8), mode="nearest").to(lat.dtype)
+            m = 1 - m                                       # 1 = keep the original image
+            if m.shape[0] < N:
+                m = m.repeat(N // m.shape[0], 1, 1, 1)
+
         eng.prepare(prompt_embeds, conds, controlnet_conditioning_scale, guess_mode=guess_mode, cfg_duplicated=do_cfg)
         # fused step: the built-in DDIM, and UniPC (what every reference entry point installs, editany_lora.py:383,418)
         # through its per-step coefficient rows; any other scheduler object runs eng.eps + scheduler.step
@@ -465,7 +501,10 @@ class StableDiffusionControlNetInpaintPipeline:
         # everything below lives on the execution device (the noise was DRAWN on the generator's device above,
         # like diffusers' randn_tensor, then moved - utils/...inpaint.py:998-1012)
         lat = lat.to(dev, torch.float32)
-        noise_d, init_d, m_d = noise.to(dev, torch.float32), init_lat.to(dev, torch.float32), m.to(dev, torch.float32)
+        if inpaint_unet:
+            noise_d = init_d = m_d = None
+        else:
+            noise_d, init_d, m_d = noise.to(dev, torch.float32), init_lat.to(dev, torch.float32), m.to(dev, torch.float32)
         if fused:
             acp = self.scheduler.alphas_cumprod
             coefs = [(float(acp[int(t)]), float(acp[int(t)])) for t in timesteps] if unipc else \
@@ -480,6 +519,8 @@ class StableDiffusionControlNetInpaintPipeline:
             eng.set_schedule([int(t) for t in timesteps], [c[0] for c in coefs], [c[1] for c in coefs],
                              blend=([k[0] for k in k_next], [k[1] for k in k_next], on),
                              multistep=self.scheduler.coefficient_rows() if unipc else None)
+            if inpaint_unet:
+                eng.set_unet_condition(mask_lat, masked_lat)
             eng.begin(lat, guidance_scale, known_nchw=init_d if blend_steps else None,
                       mask_n1hw=m_d if blend_steps else None, noise_nchw=noise_d if blend_steps else None)
             for i, t in enumerate(timesteps):
@@ -490,8 +531,12 @@ class StableDiffusionControlNetInpaintPipeline:
                     eng.blend_now(k_next[i][0], k_next[i][1])
             lat = eng.latents()
         else:
+            if inpaint_unet:
+                cond = torch.cat([torch.cat([mask_lat] * 2), torch.cat([masked_lat] * 2)], 1)
             for i, t in enumerate(timesteps):
                 x_in = self.scheduler.scale_model_input(torch.cat([lat] * 2), t)
+                if inpaint_unet:
+                    x_in = torch.cat([x_in, cond], 1)                                  # :1550-1558
                 eps = eng.eps(x_in, float(t))
                 e = eps[:N] + guidance_scale * (eps[N:] - eps[:N])
                 lat = self.scheduler.step(e, t, lat).prev_sample
@@ -499,7 +544,7 @@ class StableDiffusionControlNetInpaintPipeline:
                     callback(i, t, lat)
                 if i < blend_steps:
                     lat = self.scheduler.add_noise(init_d, noise_d, timesteps[i + 1]) * m_d + lat * (1 - m_d)
-        if alignment_ratio is None or alignment_ratio == 1.0:
+        if not inpaint_unet and (alignment_ratio is None or alignment_ratio == 1.0):
             lat = init_d * m_d + lat * (1 - m_d)                                   # :1658-1664
 
         if output_type == "latent":

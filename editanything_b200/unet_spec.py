@@ -9,7 +9,7 @@ Restated from the reference constructors (no code shared with them):
 Parameter names follow the ldm/cldm state-dict convention so real checkpoints (after the
 diffusers->ldm key map of SURVEY.md App. B) load unchanged.
 """
-from dataclasses import dataclass, field
+from dataclasses import dataclass, field, replace
 from typing import List, Optional, Tuple
 
 import torch
@@ -41,6 +41,16 @@ SD21 = UNetConfig(num_head_channels=64, context_dim=1024, use_linear_in_transfor
 # shape constraint still met: channels multiples of 64)
 TINY = UNetConfig(model_channels=64, num_heads=8, context_dim=64)
 TINY21 = UNetConfig(model_channels=64, num_head_channels=16, context_dim=128, use_linear_in_transformer=True)
+# inpainting base models (stabilityai/stable-diffusion-2-inpainting): the UNet also reads the mask and the VAE latents
+# of the masked image, 4 + 1 + 4 = 9 input channels (utils/stable_diffusion_controlnet_inpaint.py:955-979)
+SD2_INPAINT = replace(SD21, in_channels=9)
+TINY21_INPAINT = replace(TINY21, in_channels=9)
+
+
+def controlnet_config(cfg: UNetConfig) -> UNetConfig:
+    """The ControlNet belonging to a UNet: the same topology on the 4 latent channels only (models/cldm_v21.yaml:44;
+    the 9-channel branch feeds the ControlNets the plain latents, utils/...inpaint.py:1607-1615)."""
+    return replace(cfg, in_channels=4)
 
 HINT_CHANNELS = (16, 16, 32, 32, 96, 96, 256)      # cldm/cldm.py:147-163
 HINT_STRIDES = (1, 1, 2, 1, 2, 1, 2, 1)
