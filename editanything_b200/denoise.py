@@ -29,6 +29,26 @@ def ddim_schedule(num_steps, linear_start=0.00085, linear_end=0.012, T=1000):
     return ts[::-1].copy(), a[::-1].copy(), a_prev[::-1].copy()
 
 
+def _fits(old, new):
+    """Whether `new` can be copied into `old`: the same nesting of lists / dicts, equal plain values, and tensors of
+    the same shape and dtype."""
+    if torch.is_tensor(new):
+        return torch.is_tensor(old) and old.shape == new.shape and old.dtype == new.dtype
+    if isinstance(new, list):
+        return isinstance(old, list) and len(old) == len(new) and all(map(_fits, old, new))
+    if isinstance(new, dict):
+        return isinstance(old, dict) and old.keys() == new.keys() and all(_fits(old[k], new[k]) for k in new)
+    return not torch.is_tensor(old) and old == new
+
+
+def _copy_into(old, new):
+    if torch.is_tensor(new):
+        old.copy_(new)
+    elif isinstance(new, (list, dict)):
+        for k in (new if isinstance(new, dict) else range(len(new))):
+            _copy_into(old[k], new[k])
+
+
 class DenoiseEngine:
     def __init__(self, cfg: UNetConfig, unet_sd, controlnet_sds, device, backend=None, unet_packed=None):
         """unet_packed: an already packed UNet (another engine's `.unet`) to share instead of packing `unet_sd`
@@ -50,15 +70,17 @@ class DenoiseEngine:
 
     # -- per request -------------------------------------------------------------------------
     def _keep(self, name, new):
-        """Store `new` under self.<name>, reusing the existing buffer (same address => a captured
-        CUDA graph stays valid) when shape/dtype match; otherwise invalidate the graph."""
+        """Store `new` (a tensor, or a list / dict of tensors and plain values) under self.<name>, copying it into the
+        existing buffers (same addresses => a captured CUDA graph stays valid) when the structure, plain values and
+        every tensor's shape / dtype match; otherwise adopt it and invalidate the graph."""
         old = getattr(self, name, None)
-        if torch.is_tensor(old) and torch.is_tensor(new) and old.shape == new.shape and old.dtype == new.dtype:
-            old.copy_(new)
-            return old
-        self._graph = None
-        if torch.is_tensor(new) and new.is_inference():
-            new = new.clone()         # a caller under torch.inference_mode(): persistent buffers must be normal tensors
+        if _fits(old, new):
+            _copy_into(old, new)
+            new = old
+        else:
+            self._graph = None
+            if torch.is_tensor(new) and new.is_inference():
+                new = new.clone()     # a caller under torch.inference_mode(): persistent buffers must be normal tensors
         setattr(self, name, new)
         return new
 
@@ -97,25 +119,8 @@ class DenoiseEngine:
         # lockstep (nets.UNetRunner): the encoder-side K/V of all networks live stacked in ctx_ls; only the UNet
         # (whose decoder runs alone) keeps its own per-layer cache
         ls = self.runner.lockstep
-        caches = [n.precompute_context(ctx) for n in (nets[:1] if ls else nets)]
-        new_ls = self.runner.precompute_context_lockstep(ctx) if ls else None
-        old_ls = getattr(self, "ctx_ls", None)
-        if ls and old_ls is not None and old_ls["L"] == new_ls["L"] and old_ls["B"] == new_ls["B"]:
-            for k in old_ls["kv"]:
-                old_ls["kv"][k].copy_(new_ls["kv"][k])
-        else:
-            self.ctx_ls = new_ls
-            if ls:
-                self._graph = None
-        old = getattr(self, "ctx_cache", None)
-        if old is not None and len(old) == len(caches) and all(
-                o["L"] == c["L"] and o["B"] == c["B"] for o, c in zip(old, caches)):
-            for o, c in zip(old, caches):
-                for k in o["kv"]:
-                    o["kv"][k].copy_(c["kv"][k])
-        else:
-            self.ctx_cache = caches
-            self._graph = None
+        self._keep("ctx_cache", [n.precompute_context(ctx) for n in (nets[:1] if ls else nets)])
+        self._keep("ctx_ls", self.runner.precompute_context_lockstep(ctx) if ls else None)
         # cfg_duplicated: the conditioning images are [x; x] (prepare_controlnet_conditioning_image doubles them for
         # classifier-free guidance, utils/...inpaint.py:380-381) - run the hint stack on one half only
         if cfg_duplicated and all(h.shape[0] % 2 == 0 for h in hints):
@@ -125,13 +130,7 @@ class DenoiseEngine:
                 new_hints.append(torch.cat([g, g]))
         else:
             new_hints = [c.precompute_hint(h.to(self.dev)) for c, h in zip(self.cns, hints)]
-        old_h = getattr(self, "hints", None)
-        if old_h is not None and len(old_h) == len(new_hints) and all(o.shape == n.shape for o, n in zip(old_h, new_hints)):
-            for o, n in zip(old_h, new_hints):
-                o.copy_(n)
-        else:
-            self.hints = new_hints
-            self._graph = None
+        self._keep("hints", new_hints)
         lat_hw = (hints[0].shape[-2] // 8, hints[0].shape[-1] // 8) if len(hints) else (0, 0)
         new_scales = [self._norm_scale(s, guess_mode, self.B, lat_hw) for s in scales]
         plain = all(not isinstance(s, dict) for s in new_scales)

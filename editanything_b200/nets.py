@@ -264,11 +264,6 @@ class PackedNet:
     def _new(self, *shape):
         return torch.empty(*shape, device=self.dev, dtype=self.hdt)
 
-    # block execution lives in BlockRunner (one network or several in lockstep)
-    def _run_layers(self, layers, h, emb_all, ctxc, gn_ws, final_out=None, final_out2=None):
-        return BlockRunner([self])._run_layers(layers, h, [emb_all], ctxc, gn_ws, final_out=final_out,
-                                               final_out2=final_out2)
-
 
 class BlockRunner:
     """Executes ResBlocks / SpatialTransformers / resampling convolutions for ONE network or for n networks of
@@ -281,8 +276,13 @@ class BlockRunner:
     def __init__(self, nets):
         self.nets, self.n = list(nets), len(nets)
         n0 = self.nets[0]
-        self.ops, self.cfg, self.dev, self.hdt, self.ln_fold = n0.ops, n0.cfg, n0.dev, n0.hdt, n0.ln_fold
+        self.cfg, self.dev, self.hdt, self.ln_fold = n0.cfg, n0.dev, n0.hdt, n0.ln_fold
         self.emb_off = n0.emb_off
+
+    @property
+    def ops(self):
+        # looked up at every use: a runner lives as long as its networks, whose operator table a caller may swap
+        return self.nets[0].ops
 
     def _new(self, *shape):
         return torch.empty(*shape, device=self.dev, dtype=self.hdt)
@@ -447,7 +447,7 @@ class UNetRunner:
         self.hdt = unet.hdt
         self.concurrent = os.environ.get("EA_CONCURRENT", "1") != "0"
         self._streams = []
-        self._lane_gn = {}
+        self._gn_ws = {}
         # Lockstep: the UNet encoder and the ControlNets as ONE sequence of grouped launches (BlockRunner) instead of
         # one stream per network.  Needs identical topologies (conv_in, run per network, may differ in its input
         # channels), the LayerNorm fold and at most 3 networks (ea_gemm_grouped); EA_LOCKSTEP=0 falls back to the
@@ -455,74 +455,67 @@ class UNetRunner:
         nets = [unet] + self.cns
         same = replace(unet.cfg, in_channels=0)
         self.lockstep = (os.environ.get("EA_LOCKSTEP", "1") != "0" and 2 <= len(nets) <= 3 and unet.ln_fold
-                         and all(replace(n.cfg, in_channels=0) == same and n.ln_fold for n in nets)
-                         and hasattr(self.ops, "gemm_grouped"))
-        self._ls_ws = {}
+                         and all(replace(n.cfg, in_channels=0) == same and n.ln_fold for n in nets))
+        self.solo = [BlockRunner([n]) for n in nets]      # the UNet, then each ControlNet, on its own
+        self.group = BlockRunner(nets) if self.lockstep else None
 
-    def _lane_ws(self, B, n):
-        """One zeroed GroupNorm workspace per concurrent stream."""
+    def _workspaces(self, B, n):
+        """n zeroed GroupNorm workspaces for batch B (one per concurrent stream), allocated once."""
         key = (B, n)
-        if key not in self._lane_gn:
-            self._lane_gn[key] = [self.ops.gn_workspace(B, self.dev) for _ in range(n)]
-        return self._lane_gn[key]
+        if key not in self._gn_ws:
+            self._gn_ws[key] = [self.ops.gn_workspace(B, self.dev) for _ in range(n)]
+        return self._gn_ws[key]
 
-    def _encoder(self, net: PackedNet, x_half, emb_all, ctxc, gn_ws, guided_hint=None, sinks=None, scale=1.0,
-                 deferred=None, cond_in=None):
-        """Runs input_blocks + middle.  For the UNet (`sinks` is a dict of concat slots) each skip is
-        dual-stored into its decoder concat slot; for a ControlNet each zero-conv accumulates
-        `scale * zero_conv(h)` into the slot instead of materialising the residual.  cond_in: a 9-channel UNet's
-        conv_in contribution of the condition channels, bias included (PackedNet.precompute_condition)."""
-        o, w, topo = net.ops, net.w, net.topo
+    def _encoder(self, R: BlockRunner, x_half, embs, ctxc, gn_ws, sinks, hints, scales, cond_in=None, deferred=None):
+        """input_blocks + middle of the networks of R (the UNet, if there, first), stacked along the batch.  embs,
+        hints, scales: one per network of R (hint and scale None for the UNet).  The UNet's skips are dual-stored into
+        the decoder's concat slots; each ControlNet's zero-conv then accumulates `scale * zero_conv(h)` into the same
+        slot instead of materialising the residual (cldm/cldm.py:34-41,293-303), at once or, given `deferred`, later
+        by the caller.  cond_in: a 9-channel UNet's conv_in contribution of the condition channels, bias included
+        (PackedNet.precompute_condition)."""
+        n, nets = R.n, R.nets
+        has_unet = nets[0].kind == "unet"
+        topo = nets[0].topo
         B, H, W_, _ = x_half.shape
-        is_unet = net.kind == "unet"
         h = None
         for i, layers in enumerate(topo.input_blocks):
             slot = sinks["skip"][i]
             if layers[0].kind == "conv_in":
-                blk = layers[0]
-                h = net._new(B, H, W_, blk.cout)
-                if cond_in is not None:
-                    o.conv_in(x_half, w[blk.prefix + ".w"], None, h, B=B, H=H, W=W_, Cin=net.x_channels,
-                              Cout=blk.cout, out2=slot, ldo2=slot.stride(2), add=cond_in)
-                elif blk.cin in (4, 8):
-                    o.conv_in(x_half, w[blk.prefix + ".w"], w[blk.prefix + ".b"], h, B=B, H=H, W=W_, Cin=blk.cin,
-                              Cout=blk.cout, out2=slot if is_unet else None,
-                              ldo2=slot.stride(2) if is_unet else 0, add=guided_hint)
-                else:
-                    o.conv_direct(x_half, w[blk.prefix + ".w"], w[blk.prefix + ".b"], h, B=B, Hin=H, Win=W_,
-                                  Cin=blk.cin, Cout=blk.cout, ksize=3, stride=1, add=guided_hint)
-                    if is_unet:
-                        o.conv_direct(x_half, w[blk.prefix + ".w"], w[blk.prefix + ".b"], slot, B=B, Hin=H, Win=W_,
-                                      Cin=blk.cin, Cout=blk.cout, ksize=3, stride=1, ldo=slot.stride(2))
+                p, cout = layers[0].prefix, layers[0].cout
+                h = R._new(n * B, H, W_, cout)
+                for g, nt in enumerate(nets):
+                    un = nt.kind == "unet"
+                    R.ops.conv_in(x_half, nt.w[p + ".w"], None if un and cond_in is not None else nt.w[p + ".b"],
+                                  h.chunk(n, 0)[g], B=B, H=H, W=W_, Cin=nt.x_channels, Cout=cout,
+                                  out2=slot if un else None, ldo2=slot.stride(2) if un else 0,
+                                  add=cond_in if un else hints[g])
             else:
-                h = net._run_layers(layers, h, emb_all, ctxc, gn_ws, final_out2=slot if is_unet else None)
-            if not is_unet:
-                c = h.shape[-1]
-                M = h.shape[0] * h.shape[1] * h.shape[2]
-                p = f"zero_convs.{i}.0"
-                f, rs = self.zc_scale(scale, i, h.shape)
-                if deferred is not None:   # run after the concurrent streams have joined (shared slots)
-                    deferred.append((h.view(M, c), w[p + ".w"], slot, dict(M=M, bias=w[p + ".b"], out_scale=f, row_scale=rs,
-                                                                        accumulate=True, ldo=slot.stride(2))))
-                else:
-                    o.gemm(h.view(M, c), w[p + ".w"], slot, M=M, bias=w[p + ".b"], out_scale=f, row_scale=rs,
-                           accumulate=True, ldo=slot.stride(2))
-        mid_sink = sinks["mid"]
-        if is_unet:
-            h = net._run_layers(topo.middle, h, emb_all, ctxc, gn_ws, final_out=mid_sink)
-        else:
-            h = net._run_layers(topo.middle, h, emb_all, ctxc, gn_ws)
-            c = h.shape[-1]
-            M = h.shape[0] * h.shape[1] * h.shape[2]
-            f, rs = self.zc_scale(scale, None, h.shape)
-            if deferred is not None:
-                deferred.append((h.view(M, c), w["mid_out.w"], mid_sink, dict(M=M, bias=w["mid_out.b"], out_scale=f,
-                                                                             row_scale=rs, accumulate=True,
-                                                                             ldo=mid_sink.stride(2))))
-            else:
-                o.gemm(h.view(M, c), w["mid_out.w"], mid_sink, M=M, bias=w["mid_out.b"], out_scale=f, row_scale=rs,
-                       accumulate=True, ldo=mid_sink.stride(2))
+                h = R._run_layers(layers, h, embs, ctxc, gn_ws, final_out2=slot if has_unet else None)
+            self._zero_convs(R, h, i, slot, scales, deferred)
+        # the UNet on its own writes the middle output straight into the decoder's first concat; stacked with
+        # ControlNets, its slice of the stacked output is dual-stored there
+        mid = sinks["mid"]
+        h = R._run_layers(topo.middle, h, embs, ctxc, gn_ws, final_out=mid if has_unet and n == 1 else None,
+                          final_out2=mid if has_unet and n > 1 else None)
+        self._zero_convs(R, h, None, mid, scales, deferred)
         return h
+
+    def _zero_convs(self, R, h, i, slot, scales, deferred):
+        """slot += scale * zero_conv_i(h) for every ControlNet of R (i = None: middle_block_out), or the same GEMMs
+        appended to `deferred` as (a, w, out, kwargs)."""
+        c = h.shape[-1]
+        M = h.shape[0] // R.n * h.shape[1] * h.shape[2]
+        p = "mid_out" if i is None else f"zero_convs.{i}.0"
+        for g, nt in enumerate(R.nets):
+            if nt.kind == "unet":
+                continue
+            f, rs = self.zc_scale(scales[g], i, h.shape)
+            call = (h.chunk(R.n, 0)[g].reshape(M, c), nt.w[p + ".w"], slot,
+                    dict(M=M, bias=nt.w[p + ".b"], out_scale=f, row_scale=rs, accumulate=True, ldo=slot.stride(2)))
+            if deferred is not None:
+                deferred.append(call)
+            else:
+                R.ops.gemm(*call[:3], **call[3])
 
     @staticmethod
     def zc_scale(scale, i, shape):
@@ -556,63 +549,6 @@ class UNetRunner:
                     self.ops.gemm_grouped([(ctx2, nt.w[p + ".kv2.w"], out.chunk(n, 0)[g], {}) for g, nt in enumerate(nets)])
                     kv[p] = out
         return {"kv": kv, "B": n * B, "L": Lc}
-
-    def _encoder_lockstep(self, x_half, embs, ctx_ls, hints, sinks, scales, cond_in=None):
-        """input_blocks + middle of the UNet and every ControlNet in lockstep (see BlockRunner).  The UNet's skips are
-        dual-stored into the decoder's concat slots by the grouped launch itself (out2, network 0); each ControlNet's
-        zero-conv then accumulates `scale * zero_conv(h)` into the same slot (cldm/cldm.py:34-41,293-303).  cond_in:
-        as in _encoder."""
-        o = self.ops
-        un = self.unet
-        nets = [un] + self.cns
-        n = len(nets)
-        R = BlockRunner(nets)
-        topo = un.topo
-        B, H, W_, _ = x_half.shape
-        key = (n * B,)
-        if key not in self._ls_ws:
-            self._ls_ws[key] = o.gn_workspace(n * B, self.dev)
-        gn_ws = self._ls_ws[key]
-
-        def zero_convs(h, i, slot):
-            c = h.shape[-1]
-            Mg = B * h.shape[1] * h.shape[2]
-            for k, cn in enumerate(self.cns):
-                pz = f"zero_convs.{i}.0" if i is not None else "mid_out"
-                wz, bz = (cn.w[pz + ".w"], cn.w[pz + ".b"])
-                f, rs = self.zc_scale(scales[k], i, h.shape)
-                o.gemm(h.chunk(n, 0)[1 + k].reshape(Mg, c), wz, slot, M=Mg, bias=bz, out_scale=f, row_scale=rs,
-                       accumulate=True, ldo=slot.stride(2))
-
-        h = None
-        for i, layers in enumerate(topo.input_blocks):
-            slot = sinks["skip"][i]
-            if layers[0].kind == "conv_in":
-                blk = layers[0]
-                h = R._new(n * B, H, W_, blk.cout)
-                for g, nt in enumerate(nets):
-                    hg = h.chunk(n, 0)[g]
-                    w = nt.w
-                    if g == 0 and cond_in is not None:
-                        o.conv_in(x_half, w[blk.prefix + ".w"], None, hg, B=B, H=H, W=W_, Cin=nt.x_channels,
-                                  Cout=blk.cout, out2=slot, ldo2=slot.stride(2), add=cond_in)
-                    elif nt.x_channels in (4, 8):
-                        o.conv_in(x_half, w[blk.prefix + ".w"], w[blk.prefix + ".b"], hg, B=B, H=H, W=W_,
-                                  Cin=nt.x_channels, Cout=blk.cout, out2=slot if g == 0 else None,
-                                  ldo2=slot.stride(2) if g == 0 else 0, add=hints[g - 1] if g > 0 else None)
-                    else:
-                        o.conv_direct(x_half, w[blk.prefix + ".w"], w[blk.prefix + ".b"], hg, B=B, Hin=H, Win=W_,
-                                      Cin=blk.cin, Cout=blk.cout, ksize=3, stride=1, add=hints[g - 1] if g > 0 else None)
-                        if g == 0:
-                            o.conv_direct(x_half, w[blk.prefix + ".w"], w[blk.prefix + ".b"], slot, B=B, Hin=H, Win=W_,
-                                          Cin=blk.cin, Cout=blk.cout, ksize=3, stride=1, ldo=slot.stride(2))
-            else:
-                h = R._run_layers(layers, h, embs, ctx_ls, gn_ws, final_out2=slot)
-            zero_convs(h, i, slot)
-        mid_sink = sinks["mid"]
-        h = R._run_layers(topo.middle, h, embs, ctx_ls, gn_ws, final_out2=mid_sink)
-        zero_convs(h, None, mid_sink)
-        return h
 
     def alloc_sinks(self, B, H, W_):
         """Skip-concat buffers of the decoder: cat_i = [h (C1) | skip_i + control_i (C2)]."""
@@ -660,13 +596,13 @@ class UNetRunner:
         sinks = self.alloc_sinks(B, H, W_)
         if embs is None:
             embs = self.compute_embs(t_dev, B)
-        emb_u = embs[0]
-        concurrent = self.concurrent and len(self.cns) > 0 and hasattr(o, "set_lane") and x_half.is_cuda
+        n = 1 + len(self.cns)
+        hints, scales = [None] + list(hints), [None] + list(scales)     # one per network, UNet first
         if self.lockstep and ctx_ls is not None:
-            if hasattr(o, "set_lane"):
-                o.set_lane(0, False)
-            self._encoder_lockstep(x_half, embs, ctx_ls, hints, sinks, scales, cond_in=cond_in)
-        elif concurrent:
+            o.set_lane(0, False)
+            self._encoder(self.group, x_half, embs, ctx_ls, self._workspaces(n * B, 1)[0], sinks, hints, scales,
+                          cond_in)
+        elif self.concurrent and n > 1 and x_half.is_cuda:
             # The UNet encoder and every ControlNet only READ x and write their own activations: run
             # them on parallel streams (many of their launches cannot fill 132 SMs on their own), join,
             # then apply the zero-conv accumulations into the shared skip slots on the main stream.
@@ -675,28 +611,27 @@ class UNetRunner:
             main = torch.cuda.current_stream()
             if len(self._streams) < len(self.cns):
                 self._streams = [torch.cuda.Stream() for _ in self.cns]
-            lanes_ws = self._lane_ws(B, len(self.cns) + 1)
+            lanes_ws = self._workspaces(B, n)
             deferred = []
             for s in self._streams:
                 s.wait_stream(main)
             o.set_lane(0, True)
-            self._encoder(un, x_half, emb_u, ctx_cache[0], lanes_ws[0], sinks=sinks, cond_in=cond_in)
-            for k, cn in enumerate(self.cns):
-                with torch.cuda.stream(self._streams[k]):
-                    o.set_lane(1 + k, True)
-                    self._encoder(cn, x_half, embs[1 + k], ctx_cache[1 + k], lanes_ws[1 + k], guided_hint=hints[k],
-                                  sinks=sinks, scale=scales[k], deferred=deferred)
+            self._encoder(self.solo[0], x_half, embs[:1], ctx_cache[0], lanes_ws[0], sinks, hints[:1], scales[:1],
+                          cond_in)
+            for g in range(1, n):
+                with torch.cuda.stream(self._streams[g - 1]):
+                    o.set_lane(g, True)
+                    self._encoder(self.solo[g], x_half, embs[g:g + 1], ctx_cache[g], lanes_ws[g], sinks,
+                                  hints[g:g + 1], scales[g:g + 1], deferred=deferred)
             for s in self._streams:
                 main.wait_stream(s)
             o.set_lane(0, False)
             for a_, w_, out_, kw_ in deferred:
                 o.gemm(a_, w_, out_, **kw_)
         else:
-            self._encoder(un, x_half, emb_u, ctx_cache[0], gn_ws, sinks=sinks, cond_in=cond_in)
-            for k, cn in enumerate(self.cns):
-                emb_c = embs[1 + k]
-                self._encoder(cn, x_half, emb_c, ctx_cache[1 + k], gn_ws, guided_hint=hints[k], sinks=sinks,
-                              scale=scales[k])
+            for g, R in enumerate(self.solo):
+                self._encoder(R, x_half, embs[g:g + 1], ctx_cache[g], gn_ws, sinks, hints[g:g + 1], scales[g:g + 1],
+                              cond_in)
         topo = un.topo
         cats = sinks["cats"]
         h = None
@@ -707,7 +642,7 @@ class UNetRunner:
                 dst = nxt[..., :n1]
             else:
                 dst = None
-            h = un._run_layers(layers, cat, emb_u, ctx_cache[0], gn_ws, final_out=dst)
+            h = self.solo[0]._run_layers(layers, cat, embs[:1], ctx_cache[0], gn_ws, final_out=dst)
         mc = un.cfg.model_channels
         xn = un._new(B, H, W_, mc)
         o.groupnorm(h, un.w["out.g"], un.w["out.b"], xn, B=B, HW=H * W_, C_=mc, eps=1e-5, silu=True,

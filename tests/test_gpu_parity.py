@@ -99,6 +99,29 @@ def test_eps_vs_cpu_oracle_fresh_inputs():
         assert (eng.eps(x, t).cpu() - ref).abs().max().item() < EPS_TOL
 
 
+@pytest.mark.parametrize("concurrent", ["1", "0"])
+def test_three_controlnets_vs_cpu_oracle(concurrent, monkeypatch):
+    """Three ControlNets are more networks than one grouped launch takes, so the encoder runs network by network: on
+    one CUDA stream each with the zero-convs applied after the streams join (EA_CONCURRENT=1, the default), or one
+    after another on the current stream (EA_CONCURRENT=0)."""
+    monkeypatch.setenv("EA_CONCURRENT", concurrent)
+    cfg = TINY
+    usd = make_state_dict(cfg, "unet", 71)
+    csds = [make_state_dict(cfg, "controlnet", 72 + i) for i in range(3)]
+    x, ctx, hints = make_inputs(cfg, 2, 16, 13, 8)
+    hints = hints + [hints[0].flip(-1)]
+    scales = [0.5, 1.0, 0.7]
+    eng = DenoiseEngine(cfg, usd, csds, torch.device("cuda:0"))
+    assert not eng.runner.lockstep and eng.runner.concurrent == (concurrent == "1")
+    eng.prepare(ctx, hints, scales)
+    ut, ct = build_topology(cfg), build_topology(cfg, with_decoder=False)
+    for t in (981, 501, 1):
+        with torch.no_grad():
+            ref = O.apply_model(usd, ut, [(sd, ct) for sd in csds], x, torch.full((2,), t), ctx, hints, scales)
+        err = (eng.eps(x, t).cpu() - ref).abs().max().item()
+        assert err < EPS_TOL, (concurrent, t, err)
+
+
 @pytest.mark.parametrize("use_graph", [False, True])
 def test_fused_ddim_loop_matches_oracle_loop(use_graph):
     """5 fused steps (ControlNets -> UNet -> CFG -> DDIM, with the inpaint blend) against the
