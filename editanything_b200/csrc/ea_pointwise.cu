@@ -79,6 +79,25 @@ gn_fused_kernel(const ea_half* __restrict__ x, long long ldx, int C1,
   const ea_half* src;
   long long lds;
   if (c < C1) { src = x + c; lds = ldx; } else { src = x2 + (c - C1); lds = ldx2; }
+  // Shifted statistics: the sums are of (x - k_g), with k_g the value of group g's first channel at the image's first
+  // pixel (the same element for every CTA, so the result stays deterministic).  The one-pass variance
+  // E[(x-k)^2] - E[x-k]^2 then loses precision with (mean - k)^2 / var instead of mean^2 / var, which is large for
+  // groups whose mean sits far from zero relative to their spread.
+  float shift[8];
+  {
+    int gprev = -1;
+    float kv = 0.f;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const int g = (c + j) / cpg;
+      if (g != gprev) {
+        const int ch = g * cpg;
+        kv = ea_h2f(ch < C1 ? x[(long long)b * HW * ldx + ch] : x2[(long long)b * HW * ldx2 + (ch - C1)]);
+        gprev = g;
+      }
+      shift[j] = kv;
+    }
+  }
   if (phase != 2) {
   // ---- pass 1: load (cache) + per-thread, per-channel partial sums (the thread's 8 channels
   //      are fixed, so their groups are too: shared-memory atomics only once, after the loop)
@@ -103,7 +122,11 @@ gn_fused_kernel(const ea_half* __restrict__ x, long long ldx, int C1,
         float2 f0 = ea_unpack2(u.x), f1 = ea_unpack2(u.y), f2 = ea_unpack2(u.z), f3 = ea_unpack2(u.w);
         float vals[8] = {f0.x, f0.y, f1.x, f1.y, f2.x, f2.y, f3.x, f3.y};
 #pragma unroll
-        for (int j = 0; j < 8; ++j) { cs[j] += vals[j]; cq[j] += vals[j] * vals[j]; }
+        for (int j = 0; j < 8; ++j) {
+          const float d = vals[j] - shift[j];
+          cs[j] += d;
+          cq[j] += d * d;
+        }
       }
     } else
 #endif
@@ -115,7 +138,11 @@ gn_fused_kernel(const ea_half* __restrict__ x, long long ldx, int C1,
       float2 f0 = ea_unpack2(u.x), f1 = ea_unpack2(u.y), f2 = ea_unpack2(u.z), f3 = ea_unpack2(u.w);
       float vals[8] = {f0.x, f0.y, f1.x, f1.y, f2.x, f2.y, f3.x, f3.y};
 #pragma unroll
-      for (int j = 0; j < 8; ++j) { cs[j] += vals[j]; cq[j] += vals[j] * vals[j]; }
+      for (int j = 0; j < 8; ++j) {
+        const float d = vals[j] - shift[j];
+        cs[j] += d;
+        cq[j] += d * d;
+      }
     }
     }
     // per-(pixel lane, channel) partials -> shared memory (no atomics: 480 threads x 16 contended
@@ -192,8 +219,9 @@ gn_fused_kernel(const ea_half* __restrict__ x, long long ldx, int C1,
         const int g = (c + j) / cpg;
         if (g != gprev) {
           const float s = sh[g * 2], q = sh[g * 2 + 1];
-          mean = s * inv_n;
-          rstd = rsqrtf(fmaxf(q * inv_n - mean * mean, 0.f) + eps);
+          const float dm = s * inv_n;                  // mean of (x - k_g)
+          mean = shift[j] + dm;
+          rstd = rsqrtf(fmaxf(q * inv_n - dm * dm, 0.f) + eps);
           gprev = g;
         }
         av[j] = rstd * gm[j];
