@@ -23,9 +23,22 @@ EditAnything ControlNets (sam2groundingdino_edit.py:36-44), e.g.
 
 whose tile pass loads runwayml/stable-diffusion-v1-5 separately (editany_lora.py:395-405).
 
+LoRA: `lora_model_path` names a kohya `.safetensors` file merged at `lora_weight` into the UNet and the text
+encoder of the generation and the tile pipeline before their weights are packed (editany_lora.py:378-381, 413-416;
+editanything_b200.lora), e.g. the reference's "Beauty Edit" setup (editany_beauty.py:54-64)
+
+    EditAnythingLoraModel(base_model_path=".../chilloutmix_NiPrunedFp32Fix",
+                          lora_model_path=".../cuteGirlMix4_v10.safetensors", use_blip=True, extra_inpaint=True,
+                          lora_weight=0.5)
+
+Like the reference, a rebuild of the generation pipeline for another ControlNet (`condition_model`) merges the LoRA
+at weight 1.0: it does not pass `lora_weight` on (editany_lora.py:660-666).  `load_lora_weights(pipe, path,
+multiplier, device, dtype)` merges further files into a built pipeline.
+
 Not supported here (raise NotImplementedError instead of diverging silently): reference-only mode (`ref_image`),
-`enable_all_generate` (the text-to-image ControlNet pipeline), LoRA merging, the alpha-mixing pipeline.
+`enable_all_generate` (the text-to-image ControlNet pipeline), the alpha-mixing pipeline.
 """
+import copy
 import os
 import random
 from collections import OrderedDict
@@ -75,6 +88,44 @@ def init_sam_model(sam_generator=None, mask_predictor=None):
             SamPredictor(sam) if mask_predictor is None else mask_predictor)
 
 
+def _lora_list(lora_model_path, lora_weight):
+    """The reference merges one LoRA file at `lora_weight` when a path is given (editany_lora.py:378-381, 413-416)."""
+    return None if lora_model_path is None else [(lora_model_path, lora_weight)]
+
+
+def load_lora_weights(pipeline, checkpoint_path, multiplier, device, dtype):
+    """editany_lora.py:197-329 on an already built pipeline: merge one kohya `.safetensors` file, or a list of them
+    in order, at `multiplier` into the UNet and the text encoder.  `device` and `dtype` are the reference's (it
+    reads the file onto `device` and computes the delta in `dtype`, always "cpu" and torch.float32 at its call
+    sites); here the delta is always fp32 on the CPU, added to the fp16 weights with one rounding.
+    The packed UNet cannot take a delta, so the base UNet is re-read from `pipeline.base_model_dir`, the LoRA list
+    the pipeline already carries and then the new files are merged, and the UNet is packed again on the engine's
+    backend; the packed ControlNets are kept.  The text encoder is merged in place, or in a copy when another
+    pipeline shares it (a tile pipeline built with `share_with`), so that one is not changed.  Every entry is
+    checked before the pipeline changes.  Returns the pipeline."""
+    from . import lora as L
+    from .denoise import DenoiseEngine
+    from .loading import load_weights
+    from .weights import diffusers_to_ldm
+    paths = [checkpoint_path] if isinstance(checkpoint_path, str) else list(checkpoint_path)
+    new = L.normalize([(p, multiplier) for p in paths])
+    eng = pipeline.engine
+    usd = load_weights(os.path.join(pipeline.base_model_dir, "unet"))
+    L.merge(pipeline.lora, unet_sd=usd)
+    shared = pipeline.text_encoder_shared
+    text_encoder = copy.deepcopy(pipeline.text_encoder) if shared else pipeline.text_encoder
+    entries = L.plan(new, list(usd), {k: v.shape for k, v in usd.items()}, text_encoder)
+    with torch.no_grad():
+        L.apply([e for e in entries if e[0] == "unet"], usd)
+        engine = DenoiseEngine(eng.cfg, diffusers_to_ldm(usd, "unet", eng.cfg), [], eng.dev, backend=eng.ops,
+                               controlnets_packed=eng.cns)
+        L.apply([e for e in entries if e[0] != "unet"])
+    pipeline.engine, pipeline.text_encoder = engine, text_encoder
+    pipeline.text_encoder_shared = False
+    pipeline.lora = pipeline.lora + new
+    return pipeline
+
+
 def obtain_generation_model(base_model_path, lora_model_path, controlnet_path, generation_only=False,
                             extra_inpaint=True, lora_weight=1.0):
     """editany_lora.py:343-388: SAM-ControlNet (+ inpaint-ControlNet) pipeline with the UniPC scheduler."""
@@ -82,13 +133,12 @@ def obtain_generation_model(base_model_path, lora_model_path, controlnet_path, g
     from .schedulers import UniPCMultistepScheduler
     if generation_only and extra_inpaint:
         raise NotImplementedError("enable_all_generate: the text-to-image ControlNet pipeline is outside the hot path")
-    if lora_model_path is not None:
-        raise NotImplementedError("LoRA merging (editany_lora.py:197-329) is not implemented: merge offline")
     controlnet = [ControlNetModel2.from_pretrained(controlnet_path, torch_dtype=torch.float16)]
     if (not generation_only) and extra_inpaint:
         controlnet.append(ControlNetModel.from_pretrained(INPAINT_CONTROLNET, torch_dtype=torch.float16))
     pipe = StableDiffusionControlNetInpaintPipeline.from_pretrained(base_model_path, controlnet=controlnet,
-                                                                   torch_dtype=torch.float16, safety_checker=None)
+                                                                   torch_dtype=torch.float16, safety_checker=None,
+                                                                   lora=_lora_list(lora_model_path, lora_weight))
     pipe.scheduler = UniPCMultistepScheduler.from_config(pipe.scheduler.config)
     pipe.enable_xformers_memory_efficient_attention()
     pipe.enable_model_cpu_offload()
@@ -97,13 +147,12 @@ def obtain_generation_model(base_model_path, lora_model_path, controlnet_path, g
 
 def obtain_tile_model(base_model_path, lora_model_path, lora_weight=1.0, share_with=None):
     """editany_lora.py:391-423.  `share_with`: a pipeline whose UNet / VAE / text encoder are reused when it was
-    built from the same base model directory (the tile pass runs the same SD1.5 weights: 1.7 GB of HBM saved).  An
+    built from the same base model directory (the tile pass runs the same SD1.5 weights: 1.7 GB of HBM saved); the
+    UNet and text encoder only when it also carries the same LoRA list, so nothing is merged twice.  An
     SD2-inpainting main pipeline is not shared: its tile pass runs on SD1.5 (editany_lora.py:395-405)."""
     from .loading import resolve_model_path
     from .pipeline import ControlNetModel2, StableDiffusionControlNetInpaintPipeline
     from .schedulers import UniPCMultistepScheduler
-    if lora_model_path is not None:
-        raise NotImplementedError("LoRA merging (editany_lora.py:197-329) is not implemented: merge offline")
     controlnet = ControlNetModel2.from_pretrained(TILE_CONTROLNET, torch_dtype=torch.float16)
     if base_model_path in ("runwayml/stable-diffusion-v1-5", "stabilityai/stable-diffusion-2-inpainting"):
         base_model_path = "runwayml/stable-diffusion-v1-5"
@@ -112,7 +161,8 @@ def obtain_tile_model(base_model_path, lora_model_path, lora_weight=1.0, share_w
         share_with = None
     pipe = StableDiffusionControlNetInpaintPipeline.from_pretrained(base_model_path, controlnet=controlnet,
                                                                    torch_dtype=torch.float16, safety_checker=None,
-                                                                   share_with=share_with)
+                                                                   share_with=share_with,
+                                                                   lora=_lora_list(lora_model_path, lora_weight))
     pipe.scheduler = UniPCMultistepScheduler.from_config(pipe.scheduler.config)
     pipe.enable_xformers_memory_efficient_attention()
     pipe.enable_model_cpu_offload()

@@ -50,16 +50,20 @@ def _copy_into(old, new):
 
 
 class DenoiseEngine:
-    def __init__(self, cfg: UNetConfig, unet_sd, controlnet_sds, device, backend=None, unet_packed=None):
+    def __init__(self, cfg: UNetConfig, unet_sd, controlnet_sds, device, backend=None, unet_packed=None,
+                 controlnets_packed=None):
         """unet_packed: an already packed UNet (another engine's `.unet`) to share instead of packing `unet_sd`
-        again - the reference's tile pipeline runs the same base model as the main one (editany_lora.py:395-405)."""
+        again - the reference's tile pipeline runs the same base model as the main one (editany_lora.py:395-405).
+        controlnets_packed: already packed ControlNets (another engine's `.cns`) used instead of `controlnet_sds`,
+        for an engine that re-packs only its UNet (a LoRA merged after loading)."""
         if cfg.in_channels not in (4, 9):
             raise ValueError(f"the UNet takes 4 latent channels, or 9 (latents, mask, masked-image latents) for an "
                              f"inpainting base model; got in_channels={cfg.in_channels}")
         self.cfg, self.dev = cfg, device
         self.ops = backend or default_ops()
         self.unet = unet_packed if unet_packed is not None else PackedNet(cfg, "unet", unet_sd, device, backend)
-        self.cns = [PackedNet(controlnet_config(cfg), "controlnet", sd, device, backend) for sd in controlnet_sds]
+        self.cns = list(controlnets_packed) if controlnets_packed is not None else \
+            [PackedNet(controlnet_config(cfg), "controlnet", sd, device, backend) for sd in controlnet_sds]
         self.runner = UNetRunner(self.unet, self.cns, device)
         self.hdt = self.unet.hdt
         self._graph = None

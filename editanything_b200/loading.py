@@ -116,9 +116,13 @@ def vae_config_from_diffusers(c):
 
 
 def load_pipeline_parts(base_model_path, device, *, text_encoder=None, tokenizer=None, vae=None, scheduler=None,
-                        unet_packed=None):
+                        unet_packed=None, lora=(), merge_text_encoder=True):
     """Everything `StableDiffusionControlNetInpaintPipeline.from_pretrained` needs from the base checkpoint:
-    (cfg, unet ldm state dict or None when `unet_packed` is shared, vae engine, text_encoder, tokenizer, scheduler)."""
+    (cfg, unet ldm state dict or None when `unet_packed` is shared, vae engine, text_encoder, tokenizer, scheduler).
+    lora: [(path, multiplier), ...] merged (editanything_b200.lora) into the diffusers UNet state dict it loads,
+    before the ldm re-keying and any packing, and with `merge_text_encoder` into the text encoder in place
+    (editany_lora.py:378-381).  Every entry is checked before any weight changes."""
+    from . import lora as L
     from .pipeline import DDIMScheduler
     from .vae import VaeEngine
     from .weights import diffusers_to_ldm, vae_diffusers_to_ldm
@@ -126,7 +130,7 @@ def load_pipeline_parts(base_model_path, device, *, text_encoder=None, tokenizer
     ucfg = unet_config_from_diffusers(_read_json(os.path.join(root, "unet", "config.json")))
     usd = None
     if unet_packed is None:
-        usd = diffusers_to_ldm(load_weights(os.path.join(root, "unet")), "unet", ucfg)
+        usd = load_weights(os.path.join(root, "unet"))
     if vae is None:
         vcfg = vae_config_from_diffusers(_read_json(os.path.join(root, "vae", "config.json")))
         vsd = vae_diffusers_to_ldm(load_weights(os.path.join(root, "vae")), vcfg, parts=("decoder", "encoder"))
@@ -138,6 +142,9 @@ def load_pipeline_parts(base_model_path, device, *, text_encoder=None, tokenizer
         if text_encoder is None:
             text_encoder = CLIPTextModel.from_pretrained(os.path.join(root, "text_encoder"), torch_dtype=torch.float16)
             text_encoder = text_encoder.to(device).eval()
+    L.merge(lora, unet_sd=usd, text_encoder=text_encoder if merge_text_encoder else None)
+    if usd is not None:
+        usd = diffusers_to_ldm(usd, "unet", ucfg)
     if scheduler is None:
         sp = os.path.join(root, "scheduler", "scheduler_config.json")
         sc = _read_json(sp) if os.path.exists(sp) else {}

@@ -171,6 +171,8 @@ class StableDiffusionControlNetInpaintPipeline:
         self.vae, self.text_encoder, self.tokenizer = vae, text_encoder, tokenizer
         self.scheduler = scheduler if scheduler is not None else DDIMScheduler()
         self.safety_checker, self.feature_extractor = safety_checker, feature_extractor
+        self.lora = []                     # [(path, multiplier), ...] merged into the UNet and text encoder
+        self.text_encoder_shared = False   # another pipeline holds the same text encoder module (share_with)
         dt = engine.hdt
         self.unet = _NetStub(engine.cfg.in_channels, dt)
         self.controlnet = _NetStub(4, dt, nets=[_NetStub(4, dt) for _ in engine.cns])
@@ -179,29 +181,38 @@ class StableDiffusionControlNetInpaintPipeline:
     @classmethod
     def from_pretrained(cls, pretrained_model_name_or_path, controlnet=None, torch_dtype=None, safety_checker=None,
                         feature_extractor=None, device=None, share_with=None, text_encoder=None, tokenizer=None,
-                        vae=None, scheduler=None, **_unused):
+                        vae=None, scheduler=None, lora=None, **_unused):
         """editany_lora.py:372-377: `from_pretrained(base_model_path, controlnet=[...], torch_dtype=torch.float16,
         safety_checker=None)`.  `controlnet`: one `ControlNetModel(2)` or a list (editanything_b200.loading);
         components may be passed in like diffusers allows (text_encoder=, tokenizer=, vae=, scheduler=).
-        `share_with`: another pipeline of the same base model whose packed UNet, VAE, text encoder and tokenizer
-        are reused (the tile-refinement pipeline, editany_lora.py:391-423)."""
+        `lora`: kohya LoRA files [(path, multiplier), ...] merged into the UNet and the text encoder before packing,
+        in order, like the reference's `load_lora_weights(pipe, [path], multiplier, "cpu", torch.float32)` right
+        after loading (editany_lora.py:378-381, editanything_b200.lora); the ControlNets are not touched.  Recorded
+        as `pipe.lora` with real paths.
+        `share_with`: another pipeline of the same base model whose VAE and tokenizer are reused, and whose packed
+        UNet and text encoder are reused too when it carries the same LoRA list (the tile-refinement pipeline,
+        editany_lora.py:391-423); with a different list both are loaded and merged afresh."""
+        from .lora import normalize
         from .loading import load_pipeline_parts, resolve_model_path, unet_config_from_diffusers, _read_json
         from .unet_spec import controlnet_config
         dev = torch.device(device) if device is not None else torch.device("cuda:0" if torch.cuda.is_available() else "cpu")
         cns = [] if controlnet is None else (list(controlnet) if isinstance(controlnet, (list, tuple)) else [controlnet])
+        lora = normalize(lora)
         base_dir = os.path.realpath(resolve_model_path(pretrained_model_name_or_path))
-        shared = share_with.engine.unet if share_with is not None else None
+        shared, shared_te = None, None
         if share_with is not None:
             ucfg = unet_config_from_diffusers(_read_json(os.path.join(base_dir, "unet", "config.json")))
             if share_with.engine.cfg != ucfg:
                 raise ValueError(f"share_with runs a UNet {share_with.engine.cfg}, the base model "
                                  f"'{pretrained_model_name_or_path}' has {ucfg}: nothing can be shared")
-            text_encoder = text_encoder or share_with.text_encoder
+            if getattr(share_with, "lora", []) == lora:
+                shared, shared_te = share_with.engine.unet, share_with.text_encoder
+                text_encoder = text_encoder or shared_te
             tokenizer = tokenizer or share_with.tokenizer
             vae = vae or share_with.vae
         ucfg, usd, vae, text_encoder, tokenizer, sched = load_pipeline_parts(
             base_dir, dev, text_encoder=text_encoder, tokenizer=tokenizer, vae=vae, scheduler=scheduler,
-            unet_packed=shared)
+            unet_packed=shared, lora=lora, merge_text_encoder=text_encoder is None or text_encoder is not shared_te)
         for c in cns:
             # the ControlNets of a 9-channel inpainting UNet are 4-channel nets (models/cldm_v21.yaml:44)
             if c.cfg != controlnet_config(ucfg):
@@ -210,6 +221,9 @@ class StableDiffusionControlNetInpaintPipeline:
         pipe = cls(eng, vae=vae, text_encoder=text_encoder, tokenizer=tokenizer, scheduler=sched,
                    safety_checker=safety_checker, feature_extractor=feature_extractor)
         pipe.base_model_dir = base_dir
+        pipe.lora = lora
+        if shared_te is not None and text_encoder is shared_te:
+            share_with.text_encoder_shared = pipe.text_encoder_shared = True
         for stub, c in zip(pipe.controlnet.nets, cns):
             stub.config = c.config
         return pipe
