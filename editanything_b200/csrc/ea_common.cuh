@@ -167,6 +167,12 @@ __device__ __forceinline__ void wgmma_fence_regs(float (&d)[R]) {
 #pragma unroll
   for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
+// Warp-specialised register budgets: every warp of a warp-group executes the same setmaxnreg; .dec hands registers
+// back to the SM's pool, .inc waits until the pool can grant the larger budget.
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
 
 // --------------------------- wgmma descriptors -------------------------------
 // Shared-memory matrix descriptor (64-bit), sm_90 layout:

@@ -7,21 +7,28 @@
 //     ResBlock's 1x1 skip convolution folded in as extra K-blocks (openaimodel.py:233-240,274)
 //   * 3x3 stride-2 pad-1 convolutions (Downsample, openaimodel.py:133-159) (mode CONV_S2)
 //
-// ea_gemm_kernel<BN, NG>: a CTA computes 128 x BN output tiles, one per CTA, or walking a tile list (persistent
-// launches: one CTA per SM).  Roles (288 threads, one CTA per SM):
-//   TMA producer (warp 8, one thread): A tile (128 rows x 64 halves, SWIZZLE_128B) and B tile (BN x 64) into
-//                  a `stages`-deep shared-memory ring, mbarrier-signalled.  For convolutions the A tile of filter tap
-//                  (kh,kw) is a 4-D box {64ch, bw, bh, bn} of the NHWC tensor shifted by (kh-1, kw-1); the zero padding
-//                  is TMA out-of-bounds fill, no im2col buffer exists.  W-operand loads carry an L2 evict-first hint
-//                  (see gemm_fill_group).
-//   consumers    (warp-groups 0-1): warp-group g issues wgmma.mma_async m64nBNk16 x4 per stage for tile rows
-//                  64g .. 64g+63, accumulating fp32 in registers, and releases each stage as soon as the next one's
-//                  MMAs are in flight.  The finished accumulator is staged row-major in shared memory (over the
-//                  drained ring) and the same 256 threads run the fused epilogue with one thread per tile row and the
-//                  two warp-groups on alternating 64-column groups: bias / time-embedding row vector / LayerNorm fold
-//                  / SiLU|GELU|GEGLU / scale / residual add / accumulate-into-destination (ControlNet zero-conv
-//                  residual, cldm/cldm.py:34-41) / dual store, rows written as coalesced 128-byte pieces through
-//                  shared memory.
+// ea_gemm_kernel<BN, NG, RP>: a CTA computes RP vertically adjacent 128 x BN output tiles (row tiles RP t ..
+// RP t + RP - 1, "sub-tiles") that share every W stage, one work item per CTA, or walking a list of items
+// (persistent launches: one CTA per SM).  RP = 2 loads 2 x 16 KB of A and one W box per 64-deep K-block for twice the
+// MMA work of RP = 1 (85 instead of 64 FLOP per byte of L2 traffic at BN = 128) and pays the per-item fixed costs once
+// per two tiles.  Roles (384 threads = three warp-groups, one CTA per SM, launched at 168 registers per thread;
+// setmaxnreg moves registers from the producer warp-group, 56 per thread, to the consumers, 224 per thread):
+//   TMA producer (warp-group 2; warp 8 lane 0 issues TMA, lanes 2-31 of warp 8 walk the L2 prefetch hint, warps
+//                  9-11 exit): the A box of every valid sub-tile (128 rows x 64 halves, SWIZZLE_128B) and the W box
+//                  (BN x 64) into a `stages`-deep shared-memory ring, mbarrier-signalled.  For convolutions the A box
+//                  of filter tap (kh,kw) is a 4-D box {64ch, bw, bh, bn} of the NHWC tensor shifted by (kh-1, kw-1);
+//                  the zero padding is TMA out-of-bounds fill, no im2col buffer exists.  W-operand loads carry an L2
+//                  evict-first hint (see gemm_fill_group).
+//   consumers    (warp-groups 0-1): per stage, RP = 1: warp-group g issues wgmma m64nBNk16 x4 for tile rows
+//                  64g .. 64g+63; RP = 2: warp-group g owns sub-tile g and issues two m64nBNk16 x4 (its rows 0-63 and
+//                  64-127), BN accumulator registers per thread at most (BN <= 128).  Stages are released as soon as
+//                  the next one's MMAs are in flight.  The finished accumulators are staged row-major in shared memory
+//                  (over the drained ring) and the same 256 threads run the fused epilogue with one thread per
+//                  sub-tile row: RP = 1 with the two warp-groups on alternating 64-column groups of the one tile,
+//                  RP = 2 with warp-group g over all BN columns of sub-tile g.  Epilogue: bias / time-embedding row
+//                  vector / LayerNorm fold / SiLU|GELU|GEGLU / scale / residual add / accumulate-into-destination
+//                  (ControlNet zero-conv residual, cldm/cldm.py:34-41) / dual store, rows written as coalesced
+//                  128-byte pieces through shared memory.
 #include "ea_common.cuh"
 #include "ea_internal.h"
 
@@ -29,22 +36,35 @@ namespace ea {
 
 static constexpr int BM = 128;
 static constexpr int BK = 64;
-// Warp roles: consumer warps 0-7 (two warp-groups), producer warp 8 (lane 0 issues TMA, lanes 2-31 walk the L2
-// prefetch hint).  Nine warps put three on one SM sub-partition, which caps every thread at 168 registers: the
-// 128-column accumulator (64 of them) fits, the 256-column one (128) spills inside the main loop, so the planner
-// never picks BN = 256 (it remains available as a forced width, ea_gemm_args.force_bn).
-static constexpr int GEMM_THREADS = 288;
+// Warp roles: consumer warps 0-7 (warp-groups 0-1), producer warp-group 2 (warps 8-11).  A CTA is launched with
+// 384 x 168 registers (__launch_bounds__(384, 1)); setmaxnreg then re-divides exactly that pool: 224 per consumer
+// thread, which holds the RP = 2 accumulator at BN = 128 (2 x 64 per thread) and the RP = 1 one at BN = 256 (128)
+// without spills, and 56 per producer thread (the grouped two-sub-tile convolution producer spills at 40).  The
+// planner never picks BN = 256 (a forced width only, ea_gemm_args.force_bn): the GEGLU weight interleave and the
+// planner's contract keep BN <= 128.
+static constexpr int GEMM_THREADS = 384;
 static constexpr int W_TMA = 8;
 static constexpr int EPI_WARPS = 8, EPI_THREADS = 256;
-// Shared memory: the stage ring, which after a tile's last MMA also holds the staged fp32 accumulator
-// ([BM][BN + 4]: the pad keeps the row-per-thread reads conflict-free) and 2 x 4 KB of store / residual staging per
-// consumer warp; then the barriers and the per-column vectors.
+static constexpr int PRODUCER_REGS = 56, CONSUMER_REGS = 224;
+static_assert(128 * PRODUCER_REGS + 256 * CONSUMER_REGS <= GEMM_THREADS * 168,
+              "setmaxnreg.inc can only take what .dec released from the CTA's launch allocation");
+// Shared memory: the stage ring (RP A boxes + one W box per stage), which after an item's last MMA also holds the
+// staged fp32 accumulators ([RP * BM][BN + 4]: the pad keeps the row-per-thread reads conflict-free) and 2 x 4 KB of
+// store / residual staging per consumer warp; then the barriers and the per-column vectors.
 static constexpr int GEMM_SMEM_RING = 216 * 1024;
-__host__ __device__ constexpr int gemm_epi_bytes(int bn) { return BM * (bn + 4) * 4 + 2 * 4096 * EPI_WARPS; }
-__host__ __device__ constexpr int gemm_region_bytes(int bn, int stages) {
-  return stages * (BM * BK * 2 + bn * BK * 2) > gemm_epi_bytes(bn) ? stages * (BM * BK * 2 + bn * BK * 2)
-                                                                    : gemm_epi_bytes(bn);
+__host__ __device__ constexpr int gemm_stage_bytes(int bn, int rp) { return rp * BM * BK * 2 + bn * BK * 2; }
+__host__ __device__ constexpr int gemm_epi_bytes(int bn, int rp) {
+  return rp * BM * (bn + 4) * 4 + 2 * 4096 * EPI_WARPS;
 }
+__host__ __device__ constexpr int gemm_region_bytes(int bn, int stages, int rp) {
+  return stages * gemm_stage_bytes(bn, rp) > gemm_epi_bytes(bn, rp) ? stages * gemm_stage_bytes(bn, rp)
+                                                                    : gemm_epi_bytes(bn, rp);
+}
+static_assert(4 * gemm_stage_bytes(128, 2) <= GEMM_SMEM_RING, "RP = 2, BN = 128: four 48 KB stages fill the ring");
+static_assert(gemm_epi_bytes(128, 2) <= GEMM_SMEM_RING && gemm_epi_bytes(256, 1) <= GEMM_SMEM_RING,
+              "the staged accumulators and the store staging fit the ring");
+// per-column epilogue vectors: [2 item parities][RP sub-tiles][2][256] fp32
+__host__ __device__ constexpr int gemm_cb_bytes(int rp) { return 2 * rp * 2 * 256 * 4; }
 
 struct GemmKParams {
   int M, N;
@@ -76,8 +96,8 @@ struct GemmKParams {
   int splits;
   int kb_per_split;
   int no_spin;       // split-K without the sibling wait (concurrent streams)
-  float* ws;   // [tiles][splits][128][BN] fp32
-  int* cnt;    // [tiles][2]: arrived, done (zero between launches)
+  float* ws;   // [items][splits][RP * 128][BN] fp32
+  int* cnt;    // [items][2]: arrived, done (zero between launches)
   // LayerNorm fold (see ea_gemm_args): producer side / consumer side
   float2* rowstats_out;     // [N/32][M] (sum, sumsq) of the stored values per 32-column chunk
   const float2* ln_stats;   // [ln_parts][M] partials of this GEMM's A rows
@@ -116,6 +136,13 @@ __device__ __forceinline__ void tile_origin(const GemmKParams& p, int tm, int& n
   n0 = nb * p.bn;
   h0 = th * p.bh;
   w0 = (r - th * p.tiles_w) * p.bw;
+}
+
+// Whether row tile tm holds any output row: the second sub-tile of the last RP = 2 item lies past the problem when the
+// number of row tiles is odd (its loads and stores are skipped).
+__device__ __forceinline__ bool tile_valid(const GemmKParams& p, int tm) {
+  if (p.mode == EA_GEMM_LINEAR) return (long long)tm * BM < p.M;
+  return tm / (p.tiles_w * p.tiles_h) * p.bn < p.Bsz;
 }
 
 struct RowInfo {
@@ -497,41 +524,43 @@ __device__ __forceinline__ void acc_ld32(const float* accs, int ld, int r, int c
   }
 }
 
-// The tile list runs over (group, split, tn, tm) with tm fastest, so CTAs working side by side share their weight
-// tile in L2; every group has the same shape and plan.  `p` below = the shared fields (group 0), each tile re-binds
-// `p` / the tensor maps to its own group.
+// The work list runs over (group, split, tn, item) with the item (RP row tiles) fastest, so CTAs working side by side
+// share their weight tile in L2; every group has the same shape and plan.  `p` below = the shared fields (group 0),
+// each item re-binds `p` / the tensor maps to its own group.  tm0 = the item's first row tile.
 #define EA_GEMM_TILE()                                                             \
   const int gi = NG == 1 ? 0 : tile / tiles_per_group;                             \
   const int gtile = NG == 1 ? tile : tile - gi * tiles_per_group;                  \
-  const int zsplit = gtile / mn_tiles;                                             \
-  const int mn = gtile - zsplit * mn_tiles;                                        \
+  const int zsplit = gtile / mn_items;                                             \
+  const int mn = gtile - zsplit * mn_items;                                        \
   const GemmGroup& GG = L.g[gi];                                                   \
   const GemmKParams& p = GG.p;                                                     \
-  const int tm = mn % m_tiles, tn = mn / m_tiles;                                  \
+  const int tp = mn % m_items, tn = mn / m_items;                                  \
+  const int tm0 = tp * RP;                                                         \
   const int kb0 = zsplit * p.kb_per_split;                                         \
   const int kb1 = min(nkb, kb0 + p.kb_per_split);
 
-template <int BN, int NG>
+template <int BN, int NG, int RP>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
-ea_gemm_kernel(const __grid_constant__ GemmLaunch<NG> L, const int tiles_per_group, const int m_tiles,
+ea_gemm_kernel(const __grid_constant__ GemmLaunch<NG> L, const int tiles_per_group, const int m_items,
                const int n_groups) {
+  static_assert(RP == 1 || (RP == 2 && BN <= 128), "two row tiles per CTA need BN <= 128 (registers)");
   const GemmKParams& p0 = L.g[0].p;
   const int n_tiles = (p0.N + BN - 1) / BN;
-  const int mn_tiles = m_tiles * n_tiles;
+  const int mn_items = m_items * n_tiles;
   const int num_tiles = tiles_per_group * (NG == 1 ? 1 : n_groups);
   const int nkb = p0.nkb_main + p0.nkb_extra;
   constexpr int a_bytes = BM * BK * 2;
-  constexpr int stage_bytes = a_bytes + BN * BK * 2;
+  constexpr int stage_bytes = gemm_stage_bytes(BN, RP);
   constexpr int ACC_LD = BN + 4;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                              ~uintptr_t(1023));
   float* accs = reinterpret_cast<float*>(smem);
-  uint8_t* stg_base = smem + BM * ACC_LD * 4;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + gemm_region_bytes(BN, p0.stages));
+  uint8_t* stg_base = smem + RP * BM * ACC_LD * 4;
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + gemm_region_bytes(BN, p0.stages, RP));
   uint64_t* empty_bar = full_bar + p0.stages;
   uint64_t* epi_done = empty_bar + p0.stages;       // the staged accumulator has been consumed: the ring is free
-  float* cb = reinterpret_cast<float*>(epi_done + 2);   // [2 tile parities][2][256] per-column vectors
+  float* cb = reinterpret_cast<float*>(epi_done + 2);   // [2 item parities][RP][2][256] per-column vectors
 
   pdl_launch_dependents();
   const int warp = threadIdx.x >> 5;
@@ -562,8 +591,9 @@ ea_gemm_kernel(const __grid_constant__ GemmLaunch<NG> L, const int tiles_per_gro
   __syncthreads();
 
   if (warp >= EPI_WARPS) {
+    setmaxnreg_dec<PRODUCER_REGS>();
+    if (warp != W_TMA || lane != 0) return;
     pdl_wait();
-    if (lane != 0) return;
     // ============================ TMA producer ============================
     // One thread; the loop body is kept to a handful of scalar instructions (no divisions: the filter-tap /
     // channel-block position advances incrementally).
@@ -574,26 +604,28 @@ ea_gemm_kernel(const __grid_constant__ GemmLaunch<NG> L, const int tiles_per_gro
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
       EA_GEMM_TILE()
       const CUtensorMap& tmA0 = GG.tmA0;
-      const CUtensorMap& tmA1 = GG.tmA1;
-      const CUtensorMap& tmA2 = GG.tmA2;
-      const CUtensorMap& tmA3 = GG.tmA3;
       const CUtensorMap& tmAx = GG.tmAx;
       const CUtensorMap& tmB = GG.tmB;
-      if (it > 0) mbar_wait(epi_done, (uint32_t)((it - 1) & 1));   // the previous tile's accumulator is read
+      if (it > 0) mbar_wait(epi_done, (uint32_t)((it - 1) & 1));   // the previous item's accumulator is read
       const int bcol = tn * BN;
+      // sub-tile 0 always holds rows; sub-tile 1 (RP = 2) not in the last item of an odd number of row tiles
+      const bool second = RP == 2 && tile_valid(p, tm0 + 1);
+      const uint32_t tx_bytes = (uint32_t)((second ? 2 : 1) * a_bytes + BN * BK * 2);
       if (p.mode == EA_GEMM_LINEAR) {
-        const int arow = tm * BM;
+        const int arow = tm0 * BM;
         for (int kb = kb0; kb < kb1; ++kb) {
           mbar_wait(&empty_bar[stage], phase ^ 1u);
-          mbar_expect_tx(&full_bar[stage], (uint32_t)stage_bytes);
+          mbar_expect_tx(&full_bar[stage], tx_bytes);
           tma_load_2d(sa, &tmA0, &full_bar[stage], kb * BK, arow);
-          tma_load_2d_hint(sa + a_bytes, &tmB, &full_bar[stage], kb * BK, bcol, p.b_policy);
+          if (second) tma_load_2d(sa + a_bytes, &tmA0, &full_bar[stage], kb * BK, arow + BM);
+          tma_load_2d_hint(sa + RP * a_bytes, &tmB, &full_bar[stage], kb * BK, bcol, p.b_policy);
           sa += stage_bytes;
           if (++stage == p.stages) { stage = 0; phase ^= 1u; sa = smem; }
         }
       } else {
-        int n0, h0, w0;
-        tile_origin(p, tm, n0, h0, w0);
+        int n0, h0, w0, n1 = 0, h1 = 0, w1 = 0;
+        tile_origin(p, tm0, n0, h0, w0);
+        if (second) tile_origin(p, tm0 + 1, n1, h1, w1);
         // position of kb0: tap (kh, kw) and channel block c0 of the main source
         int tap = kb0 / p.cin_blocks;
         int c0 = (kb0 - tap * p.cin_blocks) * BK;
@@ -601,12 +633,14 @@ ea_gemm_kernel(const __grid_constant__ GemmLaunch<NG> L, const int tiles_per_gro
         const int cin = p.cin_blocks * BK;
         for (int kb = kb0; kb < kb1; ++kb) {
           mbar_wait(&empty_bar[stage], phase ^ 1u);
-          mbar_expect_tx(&full_bar[stage], (uint32_t)stage_bytes);
+          mbar_expect_tx(&full_bar[stage], tx_bytes);
           if (kb >= p.nkb_main) {
             // fused 1x1 skip convolution: centre tap of the raw block input
             tma_load_4d(sa, &tmAx, &full_bar[stage], (kb - p.nkb_main) * BK, w0, h0, n0);
+            if (second) tma_load_4d(sa + a_bytes, &tmAx, &full_bar[stage], (kb - p.nkb_main) * BK, w1, h1, n1);
           } else if (p.mode == EA_GEMM_CONV_S1) {
             tma_load_4d(sa, &tmA0, &full_bar[stage], c0, w0 + kw - 1, h0 + kh - 1, n0);
+            if (second) tma_load_4d(sa + a_bytes, &tmA0, &full_bar[stage], c0, w1 + kw - 1, h1 + kh - 1, n1);
           } else {
             // stride 2, pad 1: input row 2*oh + kh - 1 lives in phase ph = (kh != 1) at index oh + dh.
             // stride 2, pad (0,1,0,1) (CONV_S2A, the VAE encoder's Downsample): input row 2*oh + kh lives in
@@ -617,10 +651,11 @@ ea_gemm_kernel(const __grid_constant__ GemmLaunch<NG> L, const int tiles_per_gro
             const int pw = asym ? (kw == 1 ? 1 : 0) : (kw == 1 ? 0 : 1);
             const int dw = asym ? (kw == 2 ? 1 : 0) : (kw == 0 ? -1 : 0);
             const int sel = ph * 2 + pw;
-            const CUtensorMap* m = sel == 0 ? &tmA0 : sel == 1 ? &tmA1 : sel == 2 ? &tmA2 : &tmA3;
+            const CUtensorMap* m = &tmA0 + sel;   // tmA0 .. tmA3 are consecutive members of GemmGroup
             tma_load_4d(sa, m, &full_bar[stage], c0, w0 + dw, h0 + dh, n0);
+            if (second) tma_load_4d(sa + a_bytes, m, &full_bar[stage], c0, w1 + dw, h1 + dh, n1);
           }
-          tma_load_2d_hint(sa + a_bytes, &tmB, &full_bar[stage], kb * BK, bcol, p.b_policy);
+          tma_load_2d_hint(sa + RP * a_bytes, &tmB, &full_bar[stage], kb * BK, bcol, p.b_policy);
           c0 += BK;
           if (c0 == cin) { c0 = 0; if (++kw == 3) { kw = 0; ++kh; } }
           sa += stage_bytes;
@@ -632,12 +667,22 @@ ea_gemm_kernel(const __grid_constant__ GemmLaunch<NG> L, const int tiles_per_gro
   }
 
   // ================================ consumers =================================
+  setmaxnreg_inc<CONSUMER_REGS>();
   pdl_wait();
-  const int wg = warp >> 2;            // MMA: tile rows 64 wg ..; epilogue: the 64-column groups gi with gi % 2 == wg
+  const int wg = warp >> 2;
   const int wq = warp & 3;
-  const int r = wq * 32 + lane;        // epilogue: tile row owned by this thread
+  const int r = wq * 32 + lane;        // epilogue: sub-tile row owned by this thread
   const int et = threadIdx.x;          // 0 .. EPI_THREADS-1
-  constexpr int GSTEP = 128;           // column distance between two 64-column groups of one warp-group
+  // RP = 1: both warp-groups share the tile's rows (MMA: rows 64 wg ..) and take alternating 64-column groups of the
+  // epilogue.  RP = 2: warp-group wg owns sub-tile wg, all of its rows and columns.
+  const int sub = RP == 2 ? wg : 0;
+  const int ar = sub * BM + r;                       // row of the staged accumulators
+  constexpr int SUB_THREADS = EPI_THREADS / RP;      // epilogue threads of one sub-tile
+  const int st_i = RP == 2 ? et & (SUB_THREADS - 1) : et;
+  const int c64 = RP == 2 ? 0 : wg * 64;             // first 64-column group of this warp-group
+  constexpr int GSTEP = RP == 2 ? 64 : 128;          // distance between two 64-column groups of one warp-group
+  const int c32 = RP == 2 ? 0 : wg * 32;             // first 32-column chunk (general / split-K epilogues)
+  constexpr int CSTEP = RP == 2 ? 32 : 64;
   uint4* stg = reinterpret_cast<uint4*>(stg_base + warp * 4096);
   uint4* stg2 = reinterpret_cast<uint4*>(stg_base + 4096 * EPI_WARPS + warp * 4096);
   const uint32_t smem0 = smem_u32(smem);
@@ -646,18 +691,21 @@ ea_gemm_kernel(const __grid_constant__ GemmLaunch<NG> L, const int tiles_per_gro
   int it = 0;
   for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
     EA_GEMM_TILE()
+    const int tm = tm0 + sub;                        // this thread's row tile
+    const bool sub_ok = RP == 1 || tile_valid(p, tm);
     const bool geglu = p.act == EA_ACT_GEGLU;
     const int half_bn = BN >> 1;
     const bool has_res = p.residual != nullptr;
     const RowInfo ri = row_info(p, tm, r);
     const int ncol0 = tn * BN;
-    float* cbt = cb + (it & 1) * 512;
+    float* cbt = cb + ((it & 1) * RP + sub) * 512;
     const long long lin_m0 = p.mode == EA_GEMM_LINEAR ? (long long)tm * BM + wq * 32 : -1;
     const int b_first = row_info(p, tm, 0).batch, b_last = row_info(p, tm, BM - 1).batch;
     // Fast path (the common case): before the main loop, bias (+ the per-image time-embedding row vector) for the
     // tile's columns is staged in shared memory and the first residual chunk is pulled into registers, so that the
     // per-chunk work after the main loop is load -> FMA -> 16-byte stores with the NEXT chunk's residual in flight.
-    const bool fast = p.splits == 1 && !geglu && !p.out_f32 && !p.accumulate && !p.row_scale && (b_last - b_first) <= 1;
+    const bool fast = sub_ok && p.splits == 1 && !geglu && !p.out_f32 && !p.accumulate && !p.row_scale &&
+                      (b_last - b_first) <= 1;
     uint4 rres[8];   // next 64-column group of the residual (coalesced layout)
     // LayerNorm fold, consumer side: this row's mean / rstd from the producer's per-chunk partials (fixed
     // summation order: deterministic).  out = acc * ln_r + ln_nm * g[n] + c[n].
@@ -665,7 +713,7 @@ ea_gemm_kernel(const __grid_constant__ GemmLaunch<NG> L, const int tiles_per_gro
     float ln_r = 1.f, ln_nm = 0.f;
     if (ln && ri.ok) ln_row_stats(p, ri.m, ln_r, ln_nm);
     if (fast) {
-      for (int i = et; i < BN; i += EPI_THREADS) {
+      for (int i = st_i; i < BN; i += SUB_THREADS) {
         const int col = ncol0 + i;
         float v0 = 0.f, v1 = 0.f;
         if (col < p.N) {
@@ -677,10 +725,10 @@ ea_gemm_kernel(const __grid_constant__ GemmLaunch<NG> L, const int tiles_per_gro
         cbt[i] = v0;
         cbt[256 + i] = v1;
       }
-      if (has_res && wg * 64 < BN)
-        residual_load64(rres, p.residual, p.ldr, lane, ri.m, ri.ok, ncol0 + wg * 64, BN - wg * 64, p.N, lin_m0, p.M);
+      if (has_res && c64 < BN)
+        residual_load64(rres, p.residual, p.ldr, lane, ri.m, ri.ok, ncol0 + c64, BN - c64, p.N, lin_m0, p.M);
     } else if (geglu && p.splits == 1) {
-      for (int i = et; i < BN; i += EPI_THREADS) {
+      for (int i = st_i; i < BN; i += SUB_THREADS) {
         const bool in = ncol0 + i < p.N;
         cbt[i] = (p.bias && in) ? __ldg(p.bias + ncol0 + i) : 0.f;
         if (ln) cbt[256 + i] = in ? __ldg(p.ln_g + ncol0 + i) : 0.f;
@@ -688,19 +736,28 @@ ea_gemm_kernel(const __grid_constant__ GemmLaunch<NG> L, const int tiles_per_gro
     }
 
     // ---- main loop: the stage of K-block kb is released once the MMAs of kb + 1 are in flight
+    //      (a warp-group whose sub-tile lies past the problem multiplies whatever its A slot holds; nothing of it is
+    //      stored)
     {
-      float acc[BN / 2];
+      float acc[RP][BN / 2];
 #pragma unroll
-      for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+      for (int h = 0; h < RP; ++h)
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) acc[h][i] = 0.f;
+      // A rows of this warp-group's 64-row MMA block h: RP = 1 -> tile rows 64 wg ..; RP = 2 -> sub-tile wg, rows 64 h ..
+      const uint32_t a_off = RP == 2 ? (uint32_t)(wg * a_bytes) : (uint32_t)(wg * 64 * 128);
       int prev = -1;
       for (int kb = kb0; kb < kb1; ++kb) {
         mbar_wait(&full_bar[stage], phase);
         const uint32_t sa = smem0 + (uint32_t)(stage * stage_bytes);
-        const uint64_t da = gmma_desc_k_sw128(sa + (uint32_t)(wg * 64 * 128), 1024);
-        const uint64_t db = gmma_desc_k_sw128(sa + (uint32_t)a_bytes, 1024);
+        const uint64_t db = gmma_desc_k_sw128(sa + (uint32_t)(RP * a_bytes), 1024);
         wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < 4; ++k) Wgmma<BN>::ss(acc, da + 2 * k, db + 2 * k, 1u);
+        for (int h = 0; h < RP; ++h) {
+          const uint64_t da = gmma_desc_k_sw128(sa + a_off + (uint32_t)(h * 64 * 128), 1024);
+#pragma unroll
+          for (int k = 0; k < 4; ++k) Wgmma<BN>::ss(acc[h], da + 2 * k, db + 2 * k, 1u);
+        }
         wgmma_commit();
         wgmma_wait<1>();
         if (prev >= 0) {
@@ -711,31 +768,35 @@ ea_gemm_kernel(const __grid_constant__ GemmLaunch<NG> L, const int tiles_per_gro
         if (++stage == p.stages) { stage = 0; phase ^= 1u; }
       }
       wgmma_wait<0>();
-      wgmma_fence_regs(acc);
+#pragma unroll
+      for (int h = 0; h < RP; ++h) wgmma_fence_regs(acc[h]);
       if (prev >= 0) {
         __syncwarp();
         if (lane == 0) mbar_arrive(&empty_bar[prev]);
       }
-      // every TMA load of this tile has landed and, once both warp-groups are here, every MMA has retired: the ring
-      // is free for the accumulator
+      // every TMA load of this item has landed and, once both warp-groups are here, every MMA has retired: the ring
+      // is free for the accumulators
       epi_bar_sync();
-      const int r0 = wg * 64 + wq * 16 + (lane >> 2);
-      float* d0 = accs + (size_t)r0 * ACC_LD + 2 * (lane & 3);
 #pragma unroll
-      for (int j = 0; j < BN / 8; ++j) {
-        *reinterpret_cast<float2*>(d0 + 8 * j) = make_float2(acc[4 * j], acc[4 * j + 1]);
-        *reinterpret_cast<float2*>(d0 + 8 * ACC_LD + 8 * j) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+      for (int h = 0; h < RP; ++h) {
+        const int r0 = (RP == 2 ? wg * BM + h * 64 : wg * 64) + wq * 16 + (lane >> 2);
+        float* d0 = accs + (size_t)r0 * ACC_LD + 2 * (lane & 3);
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+          *reinterpret_cast<float2*>(d0 + 8 * j) = make_float2(acc[h][4 * j], acc[h][4 * j + 1]);
+          *reinterpret_cast<float2*>(d0 + 8 * ACC_LD + 8 * j) = make_float2(acc[h][4 * j + 2], acc[h][4 * j + 3]);
+        }
       }
     }
     epi_bar_sync();
 
     if (fast) {
       const float* cbr = cbt + ((!ln && ri.batch != b_first) ? 256 : 0);
-      // this warp-group's chunks: both halves of the 64-column groups wg, wg + 2, ...
+      // this warp-group's chunks: both halves of the 64-column groups c64, c64 + GSTEP, ...
       auto next_chunk = [&](int c) { return ((c & 32) == 0 && c + 32 < BN) ? c + 32 : (c & ~63) + GSTEP; };
-      for (int c = wg * 64; c < BN; c = next_chunk(c)) {
+      for (int c = c64; c < BN; c = next_chunk(c)) {
         uint32_t v[32];
-        acc_ld32(accs, ACC_LD, r, c, v);
+        acc_ld32(accs, ACC_LD, ar, c, v);
         const int n_first = ncol0 + c;
         const int half = (c >> 5) & 1;
         if (has_res && half == 0) {
@@ -811,12 +872,12 @@ ea_gemm_kernel(const __grid_constant__ GemmLaunch<NG> L, const int tiles_per_gro
       }
     } else if (p.splits == 1) {
       if (geglu) {
-        // tile columns: [0, BN/2) = value half, [BN/2, BN) = gate half (weights pre-interleaved); the 32-column
-        // output chunks alternate between the two warp-groups, each flushed on its own
-        for (int c = wg * 32; c < half_bn; c += 64) {
+        // tile columns: [0, BN/2) = value half, [BN/2, BN) = gate half (weights pre-interleaved); RP = 1: the
+        // 32-column output chunks alternate between the two warp-groups, each flushed on its own
+        for (int c = c32; c < half_bn; c += CSTEP) {
           uint32_t xv[32], gv[32];
-          acc_ld32(accs, ACC_LD, r, c, xv);
-          acc_ld32(accs, ACC_LD, r, half_bn + c, gv);
+          acc_ld32(accs, ACC_LD, ar, c, xv);
+          acc_ld32(accs, ACC_LD, ar, half_bn + c, gv);
           float fx[32], fg[32];
 #pragma unroll
           for (int j = 0; j < 32; ++j) { fx[j] = __uint_as_float(xv[j]); fg[j] = __uint_as_float(gv[j]); }
@@ -829,9 +890,9 @@ ea_gemm_kernel(const __grid_constant__ GemmLaunch<NG> L, const int tiles_per_gro
             stage_flush(stg, lane, p.out, p.ldo, nullptr, 0, ri.m, ri.ok, (ncol0 >> 1) + c, 4, p.N >> 1, lin_m0, p.M);
         }
       } else {
-        for (int c = wg * 32; c < BN; c += 64) {
+        for (int c = c32; c < BN; c += CSTEP) {
           uint32_t v[32];
-          acc_ld32(accs, ACC_LD, r, c, v);
+          acc_ld32(accs, ACC_LD, ar, c, v);
           float f[32];
 #pragma unroll
           for (int j = 0; j < 32; ++j) f[j] = __uint_as_float(v[j]);
@@ -840,15 +901,16 @@ ea_gemm_kernel(const __grid_constant__ GemmLaunch<NG> L, const int tiles_per_gro
         }
       }
     } else {
-      // ---- split-K: publish the fp32 partial tile, wait for the sibling splits, then every
-      //      split CTA reduces and finishes a 1/splits share of the tile's (row, 32-col) units.
-      const int tile_id = tn * m_tiles + tm;
-      float* wtile = p.ws + (size_t)tile_id * p.splits * (BM * BN);
-      float* mine = wtile + (size_t)zsplit * (BM * BN);
-      for (int c = wg * 32; c < BN; c += 64) {
+      // ---- split-K: publish the fp32 partial item (RP sub-tiles), wait for the sibling splits, then every
+      //      split CTA reduces and finishes a 1/splits share of the item's (row, 32-col) units.
+      constexpr int RB = RP * BM;                    // rows of one item
+      const int tile_id = tn * m_items + tp;
+      float* wtile = p.ws + (size_t)tile_id * p.splits * (RB * BN);
+      float* mine = wtile + (size_t)zsplit * (RB * BN);
+      for (int c = c32; c < BN; c += CSTEP) {
         uint32_t v[32];
-        acc_ld32(accs, ACC_LD, r, c, v);
-        float4* dst = reinterpret_cast<float4*>(mine + (size_t)r * BN + c);
+        acc_ld32(accs, ACC_LD, ar, c, v);
+        float4* dst = reinterpret_cast<float4*>(mine + (size_t)ar * BN + c);
 #pragma unroll
         for (int j = 0; j < 8; ++j)
           __stcg(dst + j, make_float4(__uint_as_float(v[4 * j]), __uint_as_float(v[4 * j + 1]),
@@ -858,7 +920,7 @@ ea_gemm_kernel(const __grid_constant__ GemmLaunch<NG> L, const int tiles_per_gro
       epi_bar_sync();
       int* cnt = p.cnt + 2 * tile_id;
       bool take_all = false;   // no_spin: the LAST split CTA to arrive finishes the whole tile
-      volatile int* flag = reinterpret_cast<volatile int*>(cbt);
+      volatile int* flag = reinterpret_cast<volatile int*>(cb + (it & 1) * RP * 512);   // one slot for the CTA
       if (p.no_spin) {
         if (et == 0) *flag = atomicAdd(cnt, 1);
         epi_bar_sync();
@@ -878,7 +940,7 @@ ea_gemm_kernel(const __grid_constant__ GemmLaunch<NG> L, const int tiles_per_gro
       __threadfence();
       if (!p.no_spin || take_all) {
         const int chunks = geglu ? (half_bn >> 5) : (BN >> 5);
-        const int units = BM * chunks;
+        const int units = RB * chunks;
         const int u0 = take_all ? 0 : (int)(((long long)units * zsplit) / p.splits);
         const int u1 = take_all ? units : (int)(((long long)units * (zsplit + 1)) / p.splits);
         // Stage 1 (all consumer threads, float4 granularity, loads of the sibling partials unrolled for
@@ -887,7 +949,7 @@ ea_gemm_kernel(const __grid_constant__ GemmLaunch<NG> L, const int tiles_per_gro
         const int segs = geglu ? 2 : 1;                 // 32-float segments per unit (value | gate)
         const int ustride = segs * 32 + 4;              // padded floats per unit in smem
         float* stage_f = accs;
-        const size_t split_stride = (size_t)BM * BN;
+        const size_t split_stride = (size_t)RB * BN;
         for (int ub = u0; ub < u1; ub += EPI_THREADS) {
           const int nu = min(EPI_THREADS, u1 - ub);
           const int nvec4 = nu * segs * 8;
@@ -896,8 +958,8 @@ ea_gemm_kernel(const __grid_constant__ GemmLaunch<NG> L, const int tiles_per_gro
             const int rem = idx - ul * (segs * 8);
             const int seg = rem >> 3, q = rem & 7;
             const int u = ub + ul;
-            const int rr = u & (BM - 1);
-            const int c = ((u >> 7) << 5) + seg * half_bn * (geglu ? 1 : 0);
+            const int rr = u & (RB - 1);
+            const int c = ((u / RB) << 5) + seg * half_bn * (geglu ? 1 : 0);
             const float4* src = reinterpret_cast<const float4*>(wtile + (size_t)rr * BN + c) + q;
             float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
             int sidx = 0;
@@ -920,9 +982,9 @@ ea_gemm_kernel(const __grid_constant__ GemmLaunch<NG> L, const int tiles_per_gro
           epi_bar_sync();
           if (et < nu) {
             const int u = ub + et;
-            const int rr = u & (BM - 1);
-            const int c = (u >> 7) << 5;
-            RowInfo r2 = row_info(p, tm, rr);
+            const int rr = u & (RB - 1);
+            const int c = (u / RB) << 5;
+            RowInfo r2 = row_info(p, tm0 + rr / BM, rr & (BM - 1));
             const float4* sp = reinterpret_cast<const float4*>(stage_f + et * ustride);
             float f[32];
 #pragma unroll
@@ -968,72 +1030,85 @@ ea_gemm_kernel(const __grid_constant__ GemmLaunch<NG> L, const int tiles_per_gro
 #undef EA_GEMM_TILE
 
 // ---- launch planner -------------------------------------------------------------------
-// Picks (BN, stages, split-K) for one problem from a small cycle model: per K-block a CTA needs max(MMA time,
-// its share of chip bandwidth, TMA latency / stages in flight); small-M layers (8x8 / 16x16 latents: M = 128 / 512)
-// are weight-streaming bound, so K is split across CTAs until every SM has one deep pipeline, and the partial
-// tiles are combined in-kernel (see the epilogue).
-struct GemmPlan { int BN, stages, splits, kbps, occ; double cost; };
+// Picks (BN, row tiles per CTA, stages, split-K) for one problem from a small cycle model: per K-block a CTA needs
+// max(MMA time, its share of chip bandwidth, TMA latency / stages in flight); small-M layers (8x8 / 16x16 latents:
+// M = 128 / 512) are weight-streaming bound, so K is split across CTAs until every SM has one deep pipeline, and the
+// partial tiles are combined in-kernel (see the epilogue).  Two row tiles per CTA (rp = 2) share each W box: per
+// K-block the A bytes and the MMA time double, the W bytes do not, and the fixed costs are paid once per pair.  They
+// are never combined with split-K, which exists because there are fewer tiles than SMs.
+struct GemmPlan { int BN, stages, splits, kbps, occ, rp; double cost; };
 
 // Per-SM and chip rates in bytes per SM clock, from the H100 SXM data sheet (3.35 TB/s HBM3; fp16 wgmma at
 // 989 TFLOP/s over 132 SMs = 2048 MAC / clk / SM, so a 128 x BN x 64 K-block takes 4 BN clk) and L2 at about 1.6x
 // HBM; the fixed costs (pipeline start ~3800 clk, ~50 clk per accumulator column of epilogue) are not measured
-// per shape on H100.
+// per shape.  tools/gemm_rowpair_ab.py times every GEMM shape of the bench step both ways; on an H100 SXM at a
+// 400 W power limit no single-wave shape reached the MMA rate (120 CTAs of 512 x 1280 x 5120: ~1190 clk per
+// 512-clk K-block), so these constants rank layouts rather than predict times.
 static constexpr double PL_LAT = 2100.0, PL_SM_CAP = 57.0, PL_L2 = 3000.0, PL_HBM = 1900.0;
 static constexpr double PL_SPLIT_COL = 8.0, PL_SPLIT_FIX = 7000.0;
 static constexpr double PL_START = 3800.0, PL_EPI = 50.0, PL_EPI_RES = 21.0;
 static constexpr int GEMM_BN[3] = {128, 64, 32};   // the tile widths the planner picks from (see GEMM_THREADS)
 
 // groups: identical problems run by the same launch - they multiply the CTAs (waves, what is left to split K
-// over) but not the reuse of one weight tile across its M-tiles.
+// over) but not the reuse of one weight tile across its M-tiles.  force_rp: 0 = either, 1 / 2 = only that.
 static GemmPlan plan_gemm(int mt, int N, int nkb, int act, long long ws_floats, int n_sm, bool has_res = false,
-                          int groups = 1) {
+                          int groups = 1, int force_rp = 0) {
   const double epi_col = (PL_EPI + (has_res ? PL_EPI_RES : 0.0)) * (act == EA_ACT_GEGLU ? 0.84 : 1.0);
-  GemmPlan best = {0, 0, 1, nkb, 1, 1e30};
-  for (int BN : GEMM_BN) {
-    if (act == EA_ACT_GEGLU && BN != 128) continue;  // weights are interleaved per 128-row block
-    if (BN > 32 && N <= BN - 32) continue;            // a narrower tile covers N just as well
-    const int nt = (N + BN - 1) / BN;
-    const long long tiles = (long long)mt * nt * groups;
-    const int stage_bytes = BM * BK * 2 + BN * BK * 2;
-    int st = GEMM_SMEM_RING / stage_bytes;
-    if (st > 8) st = 8;
-    if (st > nkb) st = nkb < 2 ? 2 : nkb;
-    const long long slots = n_sm;                   // one CTA per SM
-    for (int pass = 0; pass < 2; ++pass) {
-      int splits = 1, kbps = nkb;
-      if (pass == 1) {
-        if (tiles >= slots || nkb < 8) break;
-        int s_max = (int)(slots / tiles);
-        if (s_max > nkb / 4) s_max = nkb / 4;
-        if (s_max < 2) break;
-        kbps = (nkb + s_max - 1) / s_max;
-        splits = (nkb + kbps - 1) / kbps;  // every split owns at least one K-block
-        if (splits < 2) break;
-        if (tiles > 2048 || tiles * splits * (long long)(BM * BN) > ws_floats) break;
+  GemmPlan best = {0, 0, 1, nkb, 1, 1, 1e30};
+  for (int rp = 1; rp <= 2; ++rp) {
+    if (force_rp > 0 && rp != force_rp) continue;
+    if (force_rp == 0 && rp == 2 && mt < 2) continue;
+    const int mi = (mt + rp - 1) / rp;              // row items (CTAs along M)
+    for (int BN : GEMM_BN) {
+      if (act == EA_ACT_GEGLU && BN != 128) continue;  // weights are interleaved per 128-row block
+      if (BN > 32 && N <= BN - 32) continue;            // a narrower tile covers N just as well
+      const int nt = (N + BN - 1) / BN;
+      const long long tiles = (long long)mi * nt * groups;
+      const int stage_bytes = gemm_stage_bytes(BN, rp);
+      int st = GEMM_SMEM_RING / stage_bytes;
+      if (st > 8) st = 8;
+      if (st > nkb) st = nkb < 2 ? 2 : nkb;
+      const long long slots = n_sm;                   // one CTA per SM
+      // Pairs only pay once one tile per CTA needs more than one wave: below that they halve the SMs at work, and
+      // on H100 (tools/gemm_rowpair_ab.py) every such step shape ran slower paired, e.g. 120 tiles of 512 x 1280 x
+      // 5120: 54 us single, 74 us paired.
+      if (force_rp == 0 && rp == 2 && (long long)mt * nt * groups <= slots) continue;
+      for (int pass = 0; pass < (rp == 1 ? 2 : 1); ++pass) {
+        int splits = 1, kbps = nkb;
+        if (pass == 1) {
+          if (tiles >= slots || nkb < 8) break;
+          int s_max = (int)(slots / tiles);
+          if (s_max > nkb / 4) s_max = nkb / 4;
+          if (s_max < 2) break;
+          kbps = (nkb + s_max - 1) / s_max;
+          splits = (nkb + kbps - 1) / kbps;  // every split owns at least one K-block
+          if (splits < 2) break;
+          if (tiles > 2048 || tiles * splits * (long long)(BM * BN) > ws_floats) break;
+        }
+        const long long ctas = tiles * splits;
+        const long long waves = (ctas + slots - 1) / slots;
+        const long long conc = ctas < slots ? ctas : slots;
+        const double t_mma = 4.0 * BN * rp;
+        const double t_sm = (double)stage_bytes / PL_SM_CAP;               // per-SM TMA fill cap
+        const double a_bytes = rp * BM * BK * 2.0, b_bytes = BN * BK * 2.0;
+        const double hbm_frac = 1.0 / (double)mi;                         // weights: HBM once, then L2
+        const double t_chip = (double)conc * (a_bytes / PL_L2 + b_bytes * hbm_frac / PL_HBM +
+                                              b_bytes * (1.0 - hbm_frac) / PL_L2);
+        const double t_lat = PL_LAT / st;
+        double t_kb = t_mma;
+        if (t_sm > t_kb) t_kb = t_sm;
+        if (t_chip > t_kb) t_kb = t_chip;
+        if (t_lat > t_kb) t_kb = t_lat;
+        double cost;
+        if (splits == 1) {
+          cost = (double)waves * (PL_START + kbps * t_kb + epi_col * BN * rp);
+        } else {
+          // fp32 partial store, arrival counter, distributed reduce + fused epilogue
+          cost = (double)waves * (PL_START + kbps * t_kb + PL_SPLIT_COL * BN) + PL_SPLIT_FIX +
+                 3.0 * (BM * BN * 4.0) / 25.0 + 150.0 * splits;
+        }
+        if (cost < best.cost) best = {BN, st, splits, kbps, 1, rp, cost};
       }
-      const long long ctas = tiles * splits;
-      const long long waves = (ctas + slots - 1) / slots;
-      const long long conc = ctas < slots ? ctas : slots;
-      const double t_mma = 4.0 * BN;
-      const double t_sm = (double)stage_bytes / PL_SM_CAP;               // per-SM TMA fill cap
-      const double a_bytes = BM * BK * 2.0, b_bytes = BN * BK * 2.0;
-      const double hbm_frac = 1.0 / (double)mt;                         // weights: HBM once, then L2
-      const double t_chip = (double)conc * (a_bytes / PL_L2 + b_bytes * hbm_frac / PL_HBM +
-                                            b_bytes * (1.0 - hbm_frac) / PL_L2);
-      const double t_lat = PL_LAT / st;
-      double t_kb = t_mma;
-      if (t_sm > t_kb) t_kb = t_sm;
-      if (t_chip > t_kb) t_kb = t_chip;
-      if (t_lat > t_kb) t_kb = t_lat;
-      double cost;
-      if (splits == 1) {
-        cost = (double)waves * (PL_START + kbps * t_kb + epi_col * BN);
-      } else {
-        // fp32 partial store, arrival counter, distributed reduce + fused epilogue
-        cost = (double)waves * (PL_START + kbps * t_kb + PL_SPLIT_COL * BN) + PL_SPLIT_FIX +
-               3.0 * (BM * BN * 4.0) / 25.0 + 150.0 * splits;
-      }
-      if (cost < best.cost) best = {BN, st, splits, kbps, 1, cost};
     }
   }
   return best;
@@ -1193,23 +1268,30 @@ static int set_max_smem(K kernel, int bytes, int& cached) {
   return EA_OK;
 }
 
-template <int BN, int NG>
-static cudaError_t launch_gemm(const GemmLaunch<NG>& L, int grid, int smem_bytes, int tiles_per_group, int m_tiles,
+template <int BN, int NG, int RP>
+static cudaError_t launch_gemm(const GemmLaunch<NG>& L, int grid, int smem_bytes, int tiles_per_group, int m_items,
                                int n_groups, cudaStream_t stream, int& rc) {
   static int cache[EA_MAX_DEV];   // zero-initialised; per device (see ea_internal.h)
-  if ((rc = set_max_smem(ea_gemm_kernel<BN, NG>, smem_bytes, cache[ea_dev()]))) return cudaSuccess;
-  return ea_launch(ea_gemm_kernel<BN, NG>, dim3((unsigned)grid), dim3(GEMM_THREADS), (size_t)smem_bytes, stream, L,
-                   tiles_per_group, m_tiles, n_groups);
+  if ((rc = set_max_smem(ea_gemm_kernel<BN, NG, RP>, smem_bytes, cache[ea_dev()]))) return cudaSuccess;
+  return ea_launch(ea_gemm_kernel<BN, NG, RP>, dim3((unsigned)grid), dim3(GEMM_THREADS), (size_t)smem_bytes, stream,
+                   L, tiles_per_group, m_items, n_groups);
 }
 
 template <int NG>
-static cudaError_t launch_gemm_bn(int BN, const GemmLaunch<NG>& L, int grid, int smem_bytes, int tiles_per_group,
-                                  int m_tiles, int n_groups, cudaStream_t stream, int& rc) {
+static cudaError_t launch_gemm_bn(int BN, int rp, const GemmLaunch<NG>& L, int grid, int smem_bytes,
+                                  int tiles_per_group, int m_items, int n_groups, cudaStream_t stream, int& rc) {
+  if (rp == 2) {
+    switch (BN) {
+      case 32: return launch_gemm<32, NG, 2>(L, grid, smem_bytes, tiles_per_group, m_items, n_groups, stream, rc);
+      case 64: return launch_gemm<64, NG, 2>(L, grid, smem_bytes, tiles_per_group, m_items, n_groups, stream, rc);
+      default: return launch_gemm<128, NG, 2>(L, grid, smem_bytes, tiles_per_group, m_items, n_groups, stream, rc);
+    }
+  }
   switch (BN) {
-    case 32: return launch_gemm<32, NG>(L, grid, smem_bytes, tiles_per_group, m_tiles, n_groups, stream, rc);
-    case 64: return launch_gemm<64, NG>(L, grid, smem_bytes, tiles_per_group, m_tiles, n_groups, stream, rc);
-    case 128: return launch_gemm<128, NG>(L, grid, smem_bytes, tiles_per_group, m_tiles, n_groups, stream, rc);
-    default: return launch_gemm<256, NG>(L, grid, smem_bytes, tiles_per_group, m_tiles, n_groups, stream, rc);
+    case 32: return launch_gemm<32, NG, 1>(L, grid, smem_bytes, tiles_per_group, m_items, n_groups, stream, rc);
+    case 64: return launch_gemm<64, NG, 1>(L, grid, smem_bytes, tiles_per_group, m_items, n_groups, stream, rc);
+    case 128: return launch_gemm<128, NG, 1>(L, grid, smem_bytes, tiles_per_group, m_items, n_groups, stream, rc);
+    default: return launch_gemm<256, NG, 1>(L, grid, smem_bytes, tiles_per_group, m_items, n_groups, stream, rc);
   }
 }
 
@@ -1235,10 +1317,17 @@ extern "C" int ea_gemm_grouped(const ea_gemm_args* args, int n_groups, void* str
   // force_persistent > 0: one CTA per SM walking the tile list (no split-K); otherwise one tile per CTA
   const bool persist = a->force_persistent > 0;
   const bool has_res = a->residual != nullptr;
-  GemmPlan plan = plan_gemm(m_tiles, a->N, nkb, a->act, persist ? 0 : ws_floats, sm_count(), has_res, G);
+  // force_2cta: 1 = two row tiles per CTA, -1 = one, 0 = the planner's choice
+  const int force_rp = a->force_2cta > 0 ? 2 : a->force_2cta < 0 ? 1 : 0;
+  GemmPlan plan =
+      plan_gemm(m_tiles, a->N, nkb, a->act, persist ? 0 : ws_floats, sm_count(), has_res, G, force_rp);
+  if (a->force_bn > 256 - 128 * (plan.rp - 1)) {   // BN = 256 has one row tile per CTA (registers)
+    if (force_rp == 2) return EA_ERR_SHAPE;
+    plan.rp = 1;
+  }
   if (a->force_bn > 0 || a->force_stages > 0 || a->force_splits > 0) {
     if (a->force_bn > 0) plan.BN = a->force_bn;
-    const int sb = BM * BK * 2 + plan.BN * BK * 2;
+    const int sb = gemm_stage_bytes(plan.BN, plan.rp);
     if (a->force_bn > 0) plan.stages = plan.BN <= 128 ? 3 : 4;
     if (a->force_stages > 0) plan.stages = a->force_stages;
     if (plan.stages * sb > GEMM_SMEM_RING) plan.stages = GEMM_SMEM_RING / sb;
@@ -1250,13 +1339,14 @@ extern "C" int ea_gemm_grouped(const ea_gemm_args* args, int n_groups, void* str
     }
   }
   if (ln_any && plan.splits > 1) return EA_ERR_ARG;
-  const int BN = plan.BN;
+  const int BN = plan.BN, RP = plan.rp;
   if (BN != 32 && BN != 64 && BN != 128 && BN != 256) return EA_ERR_SHAPE;
   if (a->act == EA_ACT_GEGLU && (a->N % 128 != 0 || BN != 128)) return EA_ERR_SHAPE;
   const int n_tiles = (a->N + BN - 1) / BN;
-  const long long tiles = (long long)m_tiles * n_tiles;      // per group
+  const int m_items = (m_tiles + RP - 1) / RP;
+  const long long tiles = (long long)m_items * n_tiles;      // work items (CTAs without split-K) per group
   if (plan.splits > 1 &&
-      (!ws_floats || tiles * G > 8192 || tiles * G * plan.splits * (long long)(BM * BN) > ws_floats))
+      (!ws_floats || tiles * G > 8192 || tiles * G * plan.splits * (long long)(RP * BM * BN) > ws_floats))
     return EA_ERR_SHAPE;
   // the spinning split-K fix-up makes split CTAs wait for their siblings: every CTA of the grid must be resident at
   // once (one per SM; the planner guarantees it, forced test configurations are checked here instead of deadlocking)
@@ -1265,7 +1355,7 @@ extern "C" int ea_gemm_grouped(const ea_gemm_args* args, int n_groups, void* str
   int stages = plan.stages;
   if (stages > 8) stages = 8;
   if (stages < 2) stages = 2;
-  const int smem_bytes = gemm_region_bytes(BN, stages) + (2 * stages + 2) * 8 + 2 * 2 * 256 * 4 + 1024;
+  const int smem_bytes = gemm_region_bytes(BN, stages, RP) + (2 * stages + 2) * 8 + gemm_cb_bytes(RP) + 1024;
   const long long tiles_per_group = tiles * plan.splits;
   for (int g = 0; g < G; ++g) {
     GemmKParams& p = L.g[g].p;
@@ -1278,7 +1368,7 @@ extern "C" int ea_gemm_grouped(const ea_gemm_args* args, int n_groups, void* str
     if (p.splits > 1) {   // every group has its own counters and partial tiles in the (shared) workspace
       p.cnt = reinterpret_cast<int*>(a->workspace) + 2 * g * tiles;
       p.ws = reinterpret_cast<float*>(reinterpret_cast<char*>(a->workspace) + 65536) +
-             (size_t)g * tiles * p.splits * (BM * BN);
+             (size_t)g * tiles * p.splits * (RP * BM * BN);
     }
     const long long ldw = ag->ldw > 0 ? ag->ldw : sh0.Ktot;
     if (ldw % 8 != 0) return EA_ERR_SHAPE;
@@ -1300,9 +1390,9 @@ extern "C" int ea_gemm_grouped(const ea_gemm_args* args, int n_groups, void* str
   if (G == 1) {
     GemmLaunch<1> L1;
     L1.g[0] = L.g[0];
-    le = launch_gemm_bn<1>(BN, L1, grid, smem_bytes, (int)tiles_per_group, m_tiles, G, stream, rc);
+    le = launch_gemm_bn<1>(BN, RP, L1, grid, smem_bytes, (int)tiles_per_group, m_items, G, stream, rc);
   } else {
-    le = launch_gemm_bn<GEMM_MAX_GROUPS>(BN, L, grid, smem_bytes, (int)tiles_per_group, m_tiles, G, stream, rc);
+    le = launch_gemm_bn<GEMM_MAX_GROUPS>(BN, RP, L, grid, smem_bytes, (int)tiles_per_group, m_items, G, stream, rc);
   }
   if (rc) return rc;
   ea_count_launch();

@@ -108,7 +108,8 @@ typedef struct ea_gemm_args {
   int force_bn;              /* 0 = auto; else 32/64/128/256 (testing) */
   int force_stages;          /* 0 = auto */
   int force_splits;          /* 0 = auto; 1 = never split K; n = split K n ways (testing) */
-  int force_2cta;            /* ignored (kept for ABI compatibility) */
+  int force_2cta;            /* row tiles per CTA: 1 = two vertically adjacent 128-row tiles sharing each W stage,
+                                -1 = one, 0 = the planner's choice (testing) */
   int no_spin;               /* 1: split-K without the sibling wait - the last split CTA to arrive reduces
                                 the whole tile (required when other streams run kernels concurrently) */
   int force_persistent;      /* > 0: one CTA per SM walks the tile list (no split-K); 0 / -1 = one tile per CTA */
