@@ -5,18 +5,26 @@
 // _ATTN_PRECISION="fp32" path) and SAM's windowed / global attention with decomposed relative
 // position bias (SURVEY.md App. C).  The N x N logits never touch HBM.
 //
-// One CTA = one (batch, head) and a tile of 128 query rows; two warp-groups, warp-group g owns query rows
-// 64g .. 64g+63.  Per 128-key tile:
-//              S = Q K^T with wgmma (A = Q, B = K, both K-major from shared memory) into 64 fp32 registers per
-//              thread; scale (+ the SAM rel-pos bias in the BIAS kernels), mask of missing keys, online softmax
-//              with the running max / sum per row (a row's 128 logits sit on the 4 lanes of a quad); P packed to
-//              16 bit straight from the accumulator layout into the A-operand fragments of the second wgmma,
-//              O += P V (B = V, MN-major from its row-major tile) into DO / 2 registers per thread.  Final 1 / l
-//              normalisation and stores.
-// Thread 0 also drives TMA: the Q tile once, then K/V tiles into a `stages`-deep ring, refilling a stage with the
-// tile `stages` ahead as soon as every warp has released it (a separate producer warp would put three warps on one
-// SM sub-partition and cap every thread at 168 registers: the 192-wide P V accumulator alone is 96).  Head dims that are not a multiple of 64 (40, 80, 160) are zero-padded for free by TMA
-// out-of-bounds fill (tensor-map inner extent d, box 64 wide).
+// One CTA = one (batch, head) and a tile of 128 query rows; 384 threads = three warp-groups, one CTA per SM, launched
+// at 168 registers per thread and re-divided by setmaxnreg (24 per producer thread, 240 per consumer thread):
+//   producer (warp-group 2; one thread, the other producer warps exit): TMA of the Q tile once, then K/V tiles into a
+//            `stages`-deep shared-memory ring with full / empty mbarriers.  Q and K are K-major SWIZZLE_128B boxes of
+//            64 columns; V is ceil(d / 16) SWIZZLE_32B boxes of 16 columns, so the P V accumulator is DO = d rounded
+//            up to an instantiated multiple of 16 (48, 64, 80, 160, 192) rather than to 64.  Columns past d (and keys
+//            past Nkv) are TMA out-of-bounds zero fill: the tensor maps' inner extent is d.
+//   consumers (warp-groups 0-1): warp-group g owns query rows 64g .. 64g+63.  Per 128-key tile j: S = Q K^T (64 fp32
+//            registers per thread), [+ the SAM rel-pos bias in the BIAS kernels], missing keys -> -inf on a ragged last
+//            tile only, online softmax with the running max / sum per row (a row's 128 logits sit on the 4 lanes of
+//            a quad), P packed to 16 bit straight from the accumulator layout into the A fragments of O += P V
+//            (DO / 2 registers per thread).  Final 1 / l normalisation and stores.
+// ptxas still compiles every thread for the 168-register launch ceiling, so S over 128 keys fits next to O only up to
+// DO = 80; the DO >= 160 kernels take each stage as two 64-key sub-tiles.
+// Two overlaps keep the tensor cores busy while the softmax runs (FlashAttention-3, Shah et al. 2024, §3.1-3.2):
+//   * within a warp-group (DO <= 80 without the bias, two or more stages), S_j = Q K_j^T and O += P_{j-1} V_{j-1} are
+//     issued together and the softmax of S_j runs while P_{j-1} V_{j-1} is still in flight; the other kernels, and a
+//     one-stage ring, run one MMA at a time per warp-group;
+//   * between the warp-groups, named barriers 2 and 3 hand the right to issue wgmmas back and forth, so one
+//     warp-group's MMAs run while the other one computes exponentials.
 #include <stdlib.h>
 #include "ea_common.cuh"
 #include "ea_internal.h"
@@ -25,14 +33,18 @@ namespace ea {
 
 static constexpr int AT_BQ = 128;
 static constexpr int AT_BKV = 128;
-static constexpr int AT_ATOM = 128 * 128;  // bytes of one 128-row x 64-half swizzled atom
+static constexpr int AT_ATOM = 128 * 128;    // bytes of one 128-row x 64-half SWIZZLE_128B box (Q, K)
+static constexpr int AT_VBOX = AT_BKV * 32;  // bytes of one 128-key x 16-half SWIZZLE_32B box (V)
 static constexpr int AT_MAX_STAGES = 4;
-static constexpr int AT_THREADS = 256;   // no separate producer warp: 8 warps may use up to 255 registers a thread
-static constexpr int AT_WARPS = 8;
+static constexpr int AT_THREADS = 384;
+static constexpr int AT_CONSUMER_WARPS = 8;
+static constexpr int AT_PRODUCER_REGS = 24, AT_CONSUMER_REGS = 240;
+static_assert(128 * AT_PRODUCER_REGS + 256 * AT_CONSUMER_REGS <= AT_THREADS * 168,
+              "setmaxnreg.inc can only take what .dec released from the CTA's launch allocation");
 
 struct AttnKParams {
   int Nq, Nkv, d, heads;
-  int nd;      // ceil(d / 64) atoms along the head dim
+  int nd;      // ceil(d / 64) Q / K boxes along the head dim
   int ksteps;  // ceil(d / 16) MMA K-steps for Q K^T
   int stages;
   float scale_log2;
@@ -43,12 +55,6 @@ struct AttnKParams {
   int rel_s;
 };
 
-__device__ __forceinline__ float ex2_approx(float x) {
-  float y;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
-}
-
 template <int R>
 __device__ __forceinline__ void wgmma_fence_regs_u32(uint32_t (&a)[R][4]) {
 #pragma unroll
@@ -57,18 +63,24 @@ __device__ __forceinline__ void wgmma_fence_regs_u32(uint32_t (&a)[R][4]) {
     for (int k = 0; k < 4; ++k) asm volatile("" : "+r"(a[i][k])::"memory");
 }
 
-// DO: width of the P V accumulator (64 / 128 / 192, >= d; the columns past d are TMA zero fill)
+// Named barriers over the 256 consumer threads: 1 = both warp-groups, 2 + g = warp-group g may issue its wgmmas.
+__device__ __forceinline__ void consumer_bar_sync(int id) { asm volatile("bar.sync %0, 256;" ::"r"(id) : "memory"); }
+__device__ __forceinline__ void consumer_bar_arrive(int id) { asm volatile("bar.arrive %0, 256;" ::"r"(id) : "memory"); }
+
+// DO: width of the P V accumulator (a multiple of 16, >= d; the columns past d are TMA zero fill)
 template <int DO, bool BIAS>
 __global__ void __launch_bounds__(AT_THREADS, 1)
 ea_attn_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                const __grid_constant__ CUtensorMap tmV, const AttnKParams p) {
+  constexpr int NV = DO / 16;   // V boxes per stage
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                              ~uintptr_t(1023));
-  // layout: Q[nd] | KV[stages][K nd | V nd] | rel_w rows (BIAS) | barriers
+  // layout: Q[nd] | KV[stages][K nd | V NV] | rel_w rows (BIAS) | barriers
+  const int k_bytes = p.nd * AT_ATOM;
+  const int kv_stage_bytes = k_bytes + NV * AT_VBOX;
   uint8_t* sQ = smem;
-  uint8_t* sKV = sQ + p.nd * AT_ATOM;
-  const int kv_stage_bytes = 2 * p.nd * AT_ATOM;
+  uint8_t* sKV = sQ + k_bytes;
   float* rw_s = reinterpret_cast<float*>(sKV + p.stages * kv_stage_bytes);   // [128][rel_s + 1]
   const int bias_floats = BIAS ? ((AT_BQ * (p.rel_s + 1) + 3) & ~3) : 0;
   uint64_t* bars = reinterpret_cast<uint64_t*>(rw_s + bias_floats);
@@ -81,38 +93,45 @@ ea_attn_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ 
   const int lane = threadIdx.x & 31;
   const int qb = blockIdx.x, head = blockIdx.y, b = blockIdx.z;
   const int n_tiles = (p.Nkv + AT_BKV - 1) / AT_BKV;
-  const bool producer = threadIdx.x == 0;
 
-  if (producer) {
-    tma_prefetch_desc(&tmQ);
-    tma_prefetch_desc(&tmK);
-    tma_prefetch_desc(&tmV);
+  if (threadIdx.x == 0) {
     mbar_init(q_full, 1);
     for (int s = 0; s < AT_MAX_STAGES; ++s) {
       mbar_init(&kv_full[s], 1);
-      mbar_init(&kv_empty[s], AT_WARPS);
+      mbar_init(&kv_empty[s], AT_CONSUMER_WARPS);
     }
     fence_mbar_init();
   }
   __syncthreads();
-  pdl_wait();
-  // K/V tile jj into its stage of the ring (thread 0; the stage's previous tile has been released)
-  auto load_kv = [&](int jj) {
-    const int st = jj % p.stages;
-    uint8_t* sK = sKV + st * kv_stage_bytes;
-    uint8_t* sV = sK + p.nd * AT_ATOM;
-    mbar_expect_tx(&kv_full[st], (uint32_t)kv_stage_bytes);
-    for (int a = 0; a < p.nd; ++a) {
-      tma_load_4d(sK + a * AT_ATOM, &tmK, &kv_full[st], a * 64, head, jj * AT_BKV, b);
-      tma_load_4d(sV + a * AT_ATOM, &tmV, &kv_full[st], a * 64, head, jj * AT_BKV, b);
-    }
-  };
-  if (producer) {
-    mbar_expect_tx(q_full, (uint32_t)(p.nd * AT_ATOM));
+
+  if (warp >= AT_CONSUMER_WARPS) {
+    setmaxnreg_dec<AT_PRODUCER_REGS>();
+    if (threadIdx.x != AT_CONSUMER_WARPS * 32) return;
+    // ============================ TMA producer ============================
+    tma_prefetch_desc(&tmQ);
+    tma_prefetch_desc(&tmK);
+    tma_prefetch_desc(&tmV);
+    pdl_wait();
+    mbar_expect_tx(q_full, (uint32_t)k_bytes);
     for (int a = 0; a < p.nd; ++a) tma_load_4d(sQ + a * AT_ATOM, &tmQ, q_full, a * 64, head, qb * AT_BQ, b);
-    for (int jj = 0; jj < p.stages && jj < n_tiles; ++jj) load_kv(jj);
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int j = 0; j < n_tiles; ++j) {
+      mbar_wait(&kv_empty[stage], phase ^ 1u);
+      uint8_t* sK = sKV + stage * kv_stage_bytes;
+      uint8_t* sV = sK + k_bytes;
+      mbar_expect_tx(&kv_full[stage], (uint32_t)kv_stage_bytes);
+      for (int a = 0; a < p.nd; ++a) tma_load_4d(sK + a * AT_ATOM, &tmK, &kv_full[stage], a * 64, head, j * AT_BKV, b);
+#pragma unroll
+      for (int c = 0; c < NV; ++c) tma_load_4d(sV + c * AT_VBOX, &tmV, &kv_full[stage], c * 16, head, j * AT_BKV, b);
+      if (++stage == p.stages) { stage = 0; phase ^= 1u; }
+    }
+    return;
   }
 
+  // ================================ consumers =================================
+  setmaxnreg_inc<AT_CONSUMER_REGS>();
+  pdl_wait();
   const int wg = warp >> 2, wq = warp & 3;
   const int g = lane >> 2, t4 = lane & 3;
   // accumulator layout (ea_wgmma.cuh): this thread holds rows rl (i % 4 < 2) and rl + 8 (i % 4 >= 2) of the tile,
@@ -125,112 +144,191 @@ ea_attn_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ 
   if (BIAS) {
     // rel_w rows of the CTA's queries (pre-multiplied by log2e) in shared memory; rel_h comes through L1
     const long long bh = (long long)b * p.heads + head;
-    for (int idx = threadIdx.x; idx < AT_BQ * p.rel_s; idx += AT_THREADS) {
+    for (int idx = threadIdx.x; idx < AT_BQ * p.rel_s; idx += AT_CONSUMER_WARPS * 32) {
       const int row = idx / p.rel_s, i = idx - row * p.rel_s;
       const int q = qb * AT_BQ + row;
       rw_s[row * (p.rel_s + 1) + i] = q < p.Nq ? __ldg(p.rel_w + (bh * p.Nq + q) * p.rel_s + i) * LOG2E : 0.f;
     }
     rh_lo = p.rel_h + (bh * p.Nq + (q_lo < p.Nq ? q_lo : 0)) * p.rel_s;
     rh_hi = p.rel_h + (bh * p.Nq + (q_hi < p.Nq ? q_hi : 0)) * p.rel_s;
-    asm volatile("bar.sync 1, 256;" ::: "memory");
+    consumer_bar_sync(1);
   }
   const uint64_t dQ0 = gmma_desc_k_sw128(smem_u32(sQ) + (uint32_t)(wg * 64 * 128), 1024);
   const uint64_t dK0 = gmma_desc_k_sw128(smem_u32(sKV), 1024);
-  const uint64_t dV0 = gmma_desc_mn_sw128(smem_u32(sKV) + (uint32_t)(p.nd * AT_ATOM), AT_ATOM, 1024);
+  const uint64_t dV0 = gmma_desc_mn_sw32(smem_u32(sKV) + (uint32_t)k_bytes, AT_VBOX, 256);
   const uint32_t kv_stage16 = (uint32_t)kv_stage_bytes >> 4;
+  // BIAS: the logits are scaled when the bias is added, so the softmax below sees scale 1
+  const float sc = BIAS ? 1.f : p.scale_log2;
+  const int my_bar = 2 + wg, other_bar = 2 + (wg ^ 1);
+
+  // Keys per S sub-tile: the whole 128-key stage up to DO = 80; 64 at DO >= 160, where S over 128 keys next to O does
+  // not fit: ptxas allocates every thread of a 384-thread CTA at most 168 registers, setmaxnreg.inc notwithstanding.
+  constexpr int SN = DO <= 80 ? AT_BKV : 64;
+  constexpr int SUB = AT_BKV / SN;   // sub-tiles per stage
+  // S_j in flight next to P_{j-1} V_{j-1} needs both in registers: only without the bias terms does that fit
+  constexpr bool PIPELINE = SN == AT_BKV && !BIAS;
+  const int n_sub = (p.Nkv + SN - 1) / SN;
+  const bool ragged = p.Nkv % SN != 0;
 
   float o[DO / 2];
 #pragma unroll
   for (int i = 0; i < DO / 2; ++i) o[i] = 0.f;
+  float s[SN / 2];
+  uint32_t pa[SN / 16][4];                    // P as the A fragments of the K-steps (16 keys each) of P V
   float m_lo = -INFINITY, m_hi = -INFINITY;   // running max in the scaled log2 domain
   float l_lo = 0.f, l_hi = 0.f;               // this thread's share of the running sum
-  mbar_wait(q_full, 0);
-  int stage = 0;
-  uint32_t phase = 0;
-  for (int j = 0; j < n_tiles; ++j) {
-    mbar_wait(&kv_full[stage], phase);
-    // ---- S = Q K^T.  K-step ks sits at atom (ks >> 2), +32 B * (ks & 3)
-    float s[64];
-    {
-      uint64_t dq = dQ0, dk = dK0 + (uint64_t)(stage * kv_stage16);
-      wgmma_fence();
-      Wgmma<128>::ss(s, dq, dk, 0u);
-      for (int ks = 1; ks < p.ksteps; ++ks) {
-        const uint32_t step = (ks & 3) ? 2u : (uint32_t)((AT_ATOM >> 4) - 6);
-        dq += step;
-        dk += step;
-        Wgmma<128>::ss(s, dq, dk, 1u);
-      }
-      wgmma_commit();
-      wgmma_wait<0>();
-      wgmma_fence_regs(s);
+  float a_lo = 0.f, a_hi = 0.f;               // rescale factor of O for the latest sub-tile
+
+  // Every wgmma issue is bracketed by mma_begin() ... mma_end(): warp-group 1 opens the sequence for warp-group 0 and
+  // skips the arrive after its last issue, so the arrivals match the syncs.
+  auto mma_begin = [&]() {
+    consumer_bar_sync(my_bar);
+    wgmma_fence();
+  };
+  auto mma_end = [&](bool last) {
+    if (!(last && wg == 1)) consumer_bar_arrive(other_bar);
+  };
+  // S = Q K^T over keys SN h .. of stage st.  K-step ks sits at box (ks >> 2), +32 B * (ks & 3)
+  auto issue_s = [&](int st, int h) {
+    uint64_t dq = dQ0, dk = dK0 + (uint64_t)(st * kv_stage16 + h * ((SN * 128) >> 4));
+    Wgmma<SN>::ss(s, dq, dk, 0u);
+    for (int ks = 1; ks < p.ksteps; ++ks) {
+      const uint32_t step = (ks & 3) ? 2u : (uint32_t)((AT_ATOM >> 4) - 6);
+      dq += step;
+      dk += step;
+      Wgmma<SN>::ss(s, dq, dk, 1u);
     }
-    // ---- scaled logits (+ bias), missing keys of the last tile -> -inf, row max
-    const int valid = min(AT_BKV, p.Nkv - j * AT_BKV);  // keys of this tile that exist (>= 1)
+    wgmma_commit();
+  };
+  // O += P V ; V K-step kk = 16 key rows = +512 B of every 16-column box
+  auto issue_pv = [&](int st, int h) {
+    const uint64_t dv = dV0 + (uint64_t)(st * kv_stage16 + h * ((SN * 32) >> 4));
+#pragma unroll
+    for (int kk = 0; kk < SN / 16; ++kk) Wgmma<DO>::rs(o, pa[kk], dv + (uint64_t)(kk * ((16 * 32) >> 4)), 1u);
+    wgmma_commit();
+  };
+  auto wait_pv = [&]() {
+    wgmma_wait<0>();
+    wgmma_fence_regs(o);
+    wgmma_fence_regs_u32(pa);
+  };
+  auto release = [&](int st) {
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&kv_empty[st]);
+  };
+  // S of sub-tile t -> exponentials in place; updates m, l and sets the O rescale factors a_lo / a_hi
+  auto softmax = [&](int t) {
+    if (BIAS) {
+#pragma unroll
+      for (int i = 0; i < SN / 2; ++i) {
+        const int key = t * SN + 8 * (i >> 2) + 2 * t4 + (i & 1);
+        const bool hi = (i >> 1) & 1;
+        const int kh = key / p.rel_s, kw = key - kh * p.rel_s;
+        s[i] = fmaf(s[i], p.scale_log2,
+                    rw_s[(rl + (hi ? 8 : 0)) * (p.rel_s + 1) + kw] + __ldg((hi ? rh_hi : rh_lo) + min(kh, p.rel_s - 1)) * LOG2E);
+      }
+    }
+    if (ragged && t == n_sub - 1) {
+      const int valid = p.Nkv - t * SN;   // keys of this sub-tile that exist (>= 1)
+#pragma unroll
+      for (int i = 0; i < SN / 2; ++i)
+        if (8 * (i >> 2) + 2 * t4 + (i & 1) >= valid) s[i] = -INFINITY;
+    }
     float mx_lo = -INFINITY, mx_hi = -INFINITY;
 #pragma unroll
-    for (int i = 0; i < 64; i += 2) {
-      const int col = 8 * (i >> 2) + 2 * t4;
-      const bool hi = (i >> 1) & 1;
-#pragma unroll
-      for (int e = 0; e < 2; ++e) {
-        float x = s[i + e] * p.scale_log2;
-        if (BIAS) {
-          const int key = j * AT_BKV + col + e;
-          const int kh = key / p.rel_s, kw = key - kh * p.rel_s;
-          x += rw_s[(rl + (hi ? 8 : 0)) * (p.rel_s + 1) + kw] + __ldg((hi ? rh_hi : rh_lo) + min(kh, p.rel_s - 1)) * LOG2E;
-        }
-        if (col + e >= valid) x = -INFINITY;
-        s[i + e] = x;
-        if (hi) mx_hi = fmaxf(mx_hi, x);
-        else mx_lo = fmaxf(mx_lo, x);
-      }
+    for (int i = 0; i < SN / 2; i += 4) {
+      mx_lo = fmaxf(mx_lo, fmaxf(s[i], s[i + 1]));
+      mx_hi = fmaxf(mx_hi, fmaxf(s[i + 2], s[i + 3]));
     }
     mx_lo = fmaxf(mx_lo, __shfl_xor_sync(0xffffffffu, mx_lo, 1));
     mx_lo = fmaxf(mx_lo, __shfl_xor_sync(0xffffffffu, mx_lo, 2));
     mx_hi = fmaxf(mx_hi, __shfl_xor_sync(0xffffffffu, mx_hi, 1));
     mx_hi = fmaxf(mx_hi, __shfl_xor_sync(0xffffffffu, mx_hi, 2));
-    const float mn_lo = fmaxf(m_lo, mx_lo), mn_hi = fmaxf(m_hi, mx_hi);
-    const float a_lo = ex2_approx(m_lo - mn_lo), a_hi = ex2_approx(m_hi - mn_hi);   // 0 on the first tile
+    // sc > 0, so the max of the scaled logits is the scaled max
+    const float mn_lo = fmaxf(m_lo, mx_lo * sc), mn_hi = fmaxf(m_hi, mx_hi * sc);
+    a_lo = mufu_ex2(m_lo - mn_lo);   // 0 on the first sub-tile
+    a_hi = mufu_ex2(m_hi - mn_hi);
     m_lo = mn_lo;
     m_hi = mn_hi;
-    l_lo *= a_lo;
-    l_hi *= a_hi;
+    float sum_lo = 0.f, sum_hi = 0.f;
+#pragma unroll
+    for (int i = 0; i < SN / 2; i += 4) {
+      s[i] = mufu_ex2(fmaf(s[i], sc, -mn_lo));
+      s[i + 1] = mufu_ex2(fmaf(s[i + 1], sc, -mn_lo));
+      s[i + 2] = mufu_ex2(fmaf(s[i + 2], sc, -mn_hi));
+      s[i + 3] = mufu_ex2(fmaf(s[i + 3], sc, -mn_hi));
+      sum_lo += s[i] + s[i + 1];
+      sum_hi += s[i + 2] + s[i + 3];
+    }
+    l_lo = fmaf(l_lo, a_lo, sum_lo);
+    l_hi = fmaf(l_hi, a_hi, sum_hi);
+  };
+  auto rescale_and_pack = [&]() {
 #pragma unroll
     for (int i = 0; i < DO / 2; ++i) o[i] *= ((i >> 1) & 1) ? a_hi : a_lo;
-    // ---- P = exp2(x - m), packed to 16 bit as the A fragments of the 8 K-steps (16 keys each) of P V
-    uint32_t pa[8][4];
 #pragma unroll
-    for (int kk = 0; kk < 8; ++kk) {
+    for (int kk = 0; kk < SN / 16; ++kk)
 #pragma unroll
-      for (int h = 0; h < 4; ++h) {
-        const int i = 8 * kk + 2 * h;
-        const float m = (h & 1) ? m_hi : m_lo;
-        const float e0 = ex2_approx(s[i] - m), e1 = ex2_approx(s[i + 1] - m);
-        if (h & 1) l_hi += e0 + e1;
-        else l_lo += e0 + e1;
-        pa[kk][h] = ea_pack2(e0, e1);
+      for (int h = 0; h < 4; ++h) pa[kk][h] = ea_pack2(s[8 * kk + 2 * h], s[8 * kk + 2 * h + 1]);
+  };
+
+  if (wg == 1) consumer_bar_arrive(2);
+  mbar_wait(q_full, 0);
+  int stage = 0;
+  uint32_t phase = 0;
+  if (PIPELINE && p.stages > 1) {
+    // S_j and P_{j-1} V_{j-1} in flight together; the softmax of S_j runs while P_{j-1} V_{j-1} does
+    mbar_wait(&kv_full[0], 0);
+    mma_begin();
+    issue_s(0, 0);
+    mma_end(false);
+    wgmma_wait<0>();
+    wgmma_fence_regs(s);
+    softmax(0);
+    rescale_and_pack();
+    for (int j = 1; j < n_sub; ++j) {
+      const int prev = stage;
+      if (++stage == p.stages) { stage = 0; phase ^= 1u; }
+      mbar_wait(&kv_full[stage], phase);
+      mma_begin();
+      issue_s(stage, 0);
+      issue_pv(prev, 0);
+      mma_end(false);
+      wgmma_wait<1>();
+      wgmma_fence_regs(s);
+      softmax(j);
+      wait_pv();
+      release(prev);
+      rescale_and_pack();
+    }
+    mma_begin();
+    issue_pv(stage, 0);
+    mma_end(true);
+    wait_pv();
+  } else {
+    // one MMA at a time per warp-group: the BIAS kernels, 64-key sub-tiles (DO >= 160), or a one-stage ring, where
+    // tile j can only be loaded once P V_{j-1} has released the stage
+    for (int t = 0; t < n_sub; ++t) {
+      const int h = t % SUB;
+      if (h == 0) mbar_wait(&kv_full[stage], phase);
+      mma_begin();
+      issue_s(stage, h);
+      mma_end(false);
+      wgmma_wait<0>();
+      wgmma_fence_regs(s);
+      softmax(t);
+      rescale_and_pack();
+      mma_begin();
+      issue_pv(stage, h);
+      mma_end(t == n_sub - 1);
+      wait_pv();
+      if (h == SUB - 1) {
+        release(stage);
+        if (++stage == p.stages) { stage = 0; phase ^= 1u; }
       }
     }
-    // ---- O += P V ; V K-step kk = 16 key rows = +2048 B
-    {
-      uint64_t dv = dV0 + (uint64_t)(stage * kv_stage16);
-      wgmma_fence();
-#pragma unroll
-      for (int kk = 0; kk < 8; ++kk) Wgmma<DO>::rs(o, pa[kk], dv + (uint64_t)(kk * ((16 * 128) >> 4)), 1u);
-      wgmma_commit();
-      wgmma_wait<0>();
-      wgmma_fence_regs(o);
-      wgmma_fence_regs_u32(pa);
-    }
-    __syncwarp();
-    if (lane == 0) mbar_arrive(&kv_empty[stage]);
-    if (producer && j + p.stages < n_tiles) {   // every warp has released tile j's stage: refill it
-      mbar_wait(&kv_empty[stage], phase);
-      load_kv(j + p.stages);
-    }
-    if (++stage == p.stages) { stage = 0; phase ^= 1u; }
   }
+
   // ---- epilogue: O / l
   l_lo += __shfl_xor_sync(0xffffffffu, l_lo, 1);
   l_lo += __shfl_xor_sync(0xffffffffu, l_lo, 2);
@@ -249,14 +347,15 @@ ea_attn_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ 
   }
 }
 
+// [B, N, heads, d] with strides (bs, ns, d) elements; boxes of `box_cols` head-dim columns x 128 rows
 static int encode_qkv(CUtensorMap* m, const void* base, int d, int heads, int N, int B,
-                      long long ns, long long bs) {
+                      long long ns, long long bs, int box_cols, CUtensorMapSwizzle swizzle) {
   cuuint64_t dims[4] = {(cuuint64_t)d, (cuuint64_t)heads, (cuuint64_t)N, (cuuint64_t)B};
   cuuint64_t strides[3] = {(cuuint64_t)d * 2, (cuuint64_t)ns * 2, (cuuint64_t)bs * 2};
-  cuuint32_t box[4] = {64, 1, 128, 1};
+  cuuint32_t box[4] = {(cuuint32_t)box_cols, 1, 128, 1};
   cuuint32_t estr[4] = {1, 1, 1, 1};
   CUresult r = ea_tmap_encode()(m, EA_TMAP_DTYPE, 4, const_cast<void*>(base), dims, strides, box,
-                                estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                                estr, CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle,
                                 CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                                 CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   return r == CUDA_SUCCESS ? 0 : (int)r;
@@ -278,6 +377,19 @@ static int launch_attn(const CUtensorMap& tq, const CUtensorMap& tk, const CUten
   return e == cudaSuccess ? 0 : ea_cuda_fail(e, "ea_attention: kernel launch");
 }
 
+template <int DO>
+static int launch_attn_width(bool bias, const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv,
+                             const AttnKParams& p, dim3 grid, int smem_bytes, cudaStream_t stream) {
+  return bias ? launch_attn<DO, true>(tq, tk, tv, p, grid, smem_bytes, stream)
+              : launch_attn<DO, false>(tq, tk, tv, p, grid, smem_bytes, stream);
+}
+
+// P V accumulator width for head dim d: the head dims the UNets and SAM run (40, 64, 80, 160) rounded up to 16,
+// and 192 for the rest of the ABI's range
+static int attn_pv_width(int d) {
+  return d <= 48 ? 48 : d <= 64 ? 64 : d <= 80 ? 80 : d <= 160 ? 160 : 192;
+}
+
 }  // namespace ea
 
 using namespace ea;
@@ -290,6 +402,7 @@ extern "C" int ea_attention(const ea_attn_args* a, void* stream_) {
   if (a->q_ns % 8 || a->k_ns % 8 || a->v_ns % 8 || a->q_bs % 8 || a->k_bs % 8 || a->v_bs % 8 ||
       a->o_ns % 8 || a->o_bs % 8)
     return EA_ERR_SHAPE;
+  if (!(a->scale > 0.f) || isinf(a->scale)) return EA_ERR_ARG;   // the kernel scales the row max, not every logit
   if ((a->rel_h != nullptr) != (a->rel_w != nullptr)) return EA_ERR_ARG;
   if (a->rel_h && a->rel_s <= 0) return EA_ERR_ARG;
 
@@ -304,9 +417,11 @@ extern "C" int ea_attention(const ea_attn_args* a, void* stream_) {
   p.rel_h = a->rel_h; p.rel_w = a->rel_w; p.rel_s = a->rel_s;
 
   const bool bias = a->rel_h != nullptr;
+  const int dv = attn_pv_width(a->d);
   const int budget = 227 * 1024 - 1024 - 256;
   const int bias_bytes = bias ? ((AT_BQ * (a->rel_s + 1) + 3) & ~3) * 4 : 0;
-  int stages = (budget - p.nd * AT_ATOM - bias_bytes) / (2 * p.nd * AT_ATOM);
+  const int stage_bytes = p.nd * AT_ATOM + dv / 16 * AT_VBOX;
+  int stages = (budget - p.nd * AT_ATOM - bias_bytes) / stage_bytes;
   if (stages > AT_MAX_STAGES) stages = AT_MAX_STAGES;
   if (stages < 1) return EA_ERR_SHAPE;
   const int n_tiles = (a->Nkv + AT_BKV - 1) / AT_BKV;
@@ -314,19 +429,23 @@ extern "C" int ea_attention(const ea_attn_args* a, void* stream_) {
   p.stages = stages;
 
   CUtensorMap tq, tk, tv;
-  if (encode_qkv(&tq, a->q, a->d, a->heads, a->Nq, a->B, a->q_ns, a->q_bs)) return EA_ERR_TMAP;
-  if (encode_qkv(&tk, a->k, a->d, a->heads, a->Nkv, a->B, a->k_ns, a->k_bs)) return EA_ERR_TMAP;
-  if (encode_qkv(&tv, a->v, a->d, a->heads, a->Nkv, a->B, a->v_ns, a->v_bs)) return EA_ERR_TMAP;
+  if (encode_qkv(&tq, a->q, a->d, a->heads, a->Nq, a->B, a->q_ns, a->q_bs, 64, CU_TENSOR_MAP_SWIZZLE_128B))
+    return EA_ERR_TMAP;
+  if (encode_qkv(&tk, a->k, a->d, a->heads, a->Nkv, a->B, a->k_ns, a->k_bs, 64, CU_TENSOR_MAP_SWIZZLE_128B))
+    return EA_ERR_TMAP;
+  if (encode_qkv(&tv, a->v, a->d, a->heads, a->Nkv, a->B, a->v_ns, a->v_bs, 16, CU_TENSOR_MAP_SWIZZLE_32B))
+    return EA_ERR_TMAP;
 
-  const int smem_bytes = p.nd * AT_ATOM + stages * 2 * p.nd * AT_ATOM + bias_bytes + (1 + 2 * AT_MAX_STAGES) * 8 + 1024;
+  const int smem_bytes = p.nd * AT_ATOM + stages * stage_bytes + bias_bytes + (1 + 2 * AT_MAX_STAGES) * 8 + 1024;
   dim3 grid((unsigned)((a->Nq + AT_BQ - 1) / AT_BQ), (unsigned)a->heads, (unsigned)a->B);
   int st;
-  if (a->d <= 64) st = bias ? launch_attn<64, true>(tq, tk, tv, p, grid, smem_bytes, stream)
-                            : launch_attn<64, false>(tq, tk, tv, p, grid, smem_bytes, stream);
-  else if (a->d <= 128) st = bias ? launch_attn<128, true>(tq, tk, tv, p, grid, smem_bytes, stream)
-                                  : launch_attn<128, false>(tq, tk, tv, p, grid, smem_bytes, stream);
-  else st = bias ? launch_attn<192, true>(tq, tk, tv, p, grid, smem_bytes, stream)
-                 : launch_attn<192, false>(tq, tk, tv, p, grid, smem_bytes, stream);
+  switch (dv) {
+    case 48: st = launch_attn_width<48>(bias, tq, tk, tv, p, grid, smem_bytes, stream); break;
+    case 64: st = launch_attn_width<64>(bias, tq, tk, tv, p, grid, smem_bytes, stream); break;
+    case 80: st = launch_attn_width<80>(bias, tq, tk, tv, p, grid, smem_bytes, stream); break;
+    case 160: st = launch_attn_width<160>(bias, tq, tk, tv, p, grid, smem_bytes, stream); break;
+    default: st = launch_attn_width<192>(bias, tq, tk, tv, p, grid, smem_bytes, stream); break;
+  }
   if (st) return st;
   ea_count_launch();
   const cudaError_t e = cudaGetLastError();

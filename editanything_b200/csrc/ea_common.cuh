@@ -202,6 +202,17 @@ __device__ __forceinline__ uint64_t gmma_desc_mn_sw128(uint32_t saddr, uint32_t 
   d |= (uint64_t)1 << 62;
   return d;
 }
+// MN-major operand, SWIZZLE_32B: the atom is 16 MN-elements (32 B) x 8 K-rows (256 B), so N may be any multiple
+// of 16; 16-wide column blocks are `lbo_bytes` apart, groups of 8 K-rows `sbo_bytes` apart.
+__device__ __forceinline__ uint64_t gmma_desc_mn_sw32(uint32_t saddr, uint32_t lbo_bytes,
+                                                      uint32_t sbo_bytes) {
+  uint64_t d = 0;
+  d |= (uint64_t)((saddr >> 4) & 0x3FFF);
+  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
+  d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
+  d |= (uint64_t)3 << 62;
+  return d;
+}
 
 // ------------------------- programmatic dependent launch -------------------
 // wait: all prerequisite grids have completed and their writes are visible (no-op when the kernel

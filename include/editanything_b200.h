@@ -157,7 +157,7 @@ int ea_gemm_plan(int m_tiles, int N, int k_blocks, int act, long long workspace_
  * Replaces CrossAttention.forward core  ldm/modules/attention.py:170-193 (QK^T in fp32,
  * softmax, PV) and SAM Attention.forward (decomposed rel-pos, SURVEY.md App. C).
  * q: [B, Nq, heads, d] with strides (q_bs, q_ns, d) elements; k, v likewise with Nkv rows;
- * out: [B, Nq, heads*d] contiguous rows of stride o_ns.  d % 8 == 0, d <= 160.
+ * out: [B, Nq, heads*d] contiguous rows of stride o_ns.  d % 8 == 0, d <= 192.  scale > 0 (finite).
  * rel_h / rel_w (optional, fp32 [B*heads, Nq, rel_s]): bias[q, kk] = rel_h[q, kk / rel_s] +
  * rel_w[q, kk % rel_s] added to the scaled logits (SAM add_decomposed_rel_pos).
  */

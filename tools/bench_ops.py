@@ -53,17 +53,29 @@ def timeit(fn, iters=20, warm=3):
 def bench_attn():
     dt = ops.half_dtype()
     out = []
-    # (name, B, heads, Nq, Nkv, d, fused_qkv)
-    for name, B, h, Nq, Nkv, d in [("self64 d40", 2, 8, 4096, 4096, 40), ("cross64 d40", 2, 8, 4096, 77, 40),
-                                   ("self32 d80", 2, 8, 1024, 1024, 80), ("cross32 d80", 2, 8, 1024, 77, 80),
-                                   ("self16 d160", 2, 8, 256, 256, 160), ("cross16 d160", 2, 8, 256, 77, 160),
-                                   ("self8 d160", 2, 8, 64, 64, 160),
-                                   ("sam_global d80", 1, 16, 4096, 4096, 80), ("sam_window d80", 25, 16, 196, 196, 80),
-                                   ("self128 d40 (1024px)", 2, 8, 16384, 16384, 40)]:
+    # (name, B, heads, Nq, Nkv, d, fused_qkv).  fused_qkv: q, k and v are column slices of one [B, N, 3 C] projection
+    # output, the layout of the step's self-attention (nets.py); B = 6 is the lockstep UNet encoder + 2 ControlNets.
+    for name, B, h, Nq, Nkv, d, fused in [("self64 d40", 2, 8, 4096, 4096, 40, False),
+                                          ("self64 d40 fused B6", 6, 8, 4096, 4096, 40, True),
+                                          ("self64 d40 fused B2", 2, 8, 4096, 4096, 40, True),
+                                          ("cross64 d40", 2, 8, 4096, 77, 40, False),
+                                          ("cross64 d40 B6", 6, 8, 4096, 77, 40, False),
+                                          ("self32 d80", 2, 8, 1024, 1024, 80, False), ("cross32 d80", 2, 8, 1024, 77, 80, False),
+                                          ("self16 d160", 2, 8, 256, 256, 160, False), ("cross16 d160", 2, 8, 256, 77, 160, False),
+                                          ("self8 d160", 2, 8, 64, 64, 160, False),
+                                          ("sam_global d80", 1, 16, 4096, 4096, 80, False),
+                                          ("sam_window d80", 25, 16, 196, 196, 80, False),
+                                          ("self128 d40 (1024px)", 2, 8, 16384, 16384, 40, False)]:
         C_ = h * d
-        q = torch.randn(B, Nq, C_, device="cuda").to(dt)
-        k = torch.randn(B, Nkv, C_, device="cuda").to(dt)
-        v = torch.randn(B, Nkv, C_, device="cuda").to(dt)
+        if fused:
+            qkv = torch.randn(B, Nq, 3 * C_, device="cuda").to(dt)
+            q, k, v = qkv[..., :C_], qkv[..., C_:2 * C_], qkv[..., 2 * C_:]
+            qs = ks = vs = (Nq * 3 * C_, 3 * C_)
+        else:
+            q = torch.randn(B, Nq, C_, device="cuda").to(dt)
+            k = torch.randn(B, Nkv, C_, device="cuda").to(dt)
+            v = torch.randn(B, Nkv, C_, device="cuda").to(dt)
+            qs, ks, vs = (Nq * C_, C_), (Nkv * C_, C_), (Nkv * C_, C_)
         o = torch.empty(B, Nq, C_, device="cuda", dtype=dt)
         rel = {}
         if name.startswith("sam"):
@@ -71,8 +83,8 @@ def bench_attn():
             rel = dict(rel_h=torch.randn(B * h, Nq, S, device="cuda"), rel_w=torch.randn(B * h, Nq, S, device="cuda"), rel_s=S)
 
         def fn():
-            ops.attention(q, k, v, o, B=B, heads=h, Nq=Nq, Nkv=Nkv, d=d, q_strides=(Nq * C_, C_),
-                          k_strides=(Nkv * C_, C_), v_strides=(Nkv * C_, C_), o_strides=(Nq * C_, C_), scale=d ** -0.5, **rel)
+            ops.attention(q, k, v, o, B=B, heads=h, Nq=Nq, Nkv=Nkv, d=d, q_strides=qs, k_strides=ks, v_strides=vs,
+                          o_strides=(Nq * C_, C_), scale=d ** -0.5, **rel)
         us = timeit(fn, iters=5 if Nq > 8000 else 20)
         fl = 4.0 * B * h * Nq * Nkv * d
         out.append({"op": "attn", "case": name, "us": round(us, 1), "tflops": round(fl / us / 1e6, 1)})
