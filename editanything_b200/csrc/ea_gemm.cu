@@ -99,7 +99,7 @@ struct GemmKParams {
   float* ws;   // [items][splits][RP * 128][BN] fp32
   int* cnt;    // [items][2]: arrived, done (zero between launches)
   // LayerNorm fold (see ea_gemm_args): producer side / consumer side
-  float2* rowstats_out;     // [N/32][M] (sum, sumsq) of the stored values per 32-column chunk
+  float2* rowstats_out;     // [N/32][M] (sum, M2 about the chunk mean) of the stored values per 32-column chunk
   const float2* ln_stats;   // [ln_parts][M] partials of this GEMM's A rows
   const float* ln_g;        // [N]
   int ln_parts;
@@ -181,10 +181,10 @@ __device__ __forceinline__ int ld_acquire_gpu(const int* p) {
   return v;
 }
 
-// LayerNorm fold, consumer side: one row's mean / rstd from the producer's per-32-column partial (sum, sumsq) pairs.
-// The loads of a batch of 16 partials are all issued before the first add, so they are in flight together instead of
-// one dependent L2 round trip per partial (10 for C = 320, 40 for C = 1280).  The adds keep their fixed order, so the
-// result stays deterministic.
+// LayerNorm fold, consumer side (ln_row_stats below): one row's mean / rstd from the producer's per-32-column partial
+// (sum, M2) pairs.  The loads of a batch of 16 partials are all issued before the first merge, so they are in flight
+// together instead of one dependent L2 round trip per partial (10 for C = 320, 40 for C = 1280).  The merges keep
+// their fixed order, so the result stays deterministic.
 // L2 prefetch of a later launch's weights (ea_gemm_args.prefetch): lanes `lane0 .. 31` of one warp in each of the first
 // pf_ctas CTAs walk the range line by line.  Issued before the dependency wait - weights are never produced by a
 // predecessor kernel - so HBM works on the next layer while this one computes from L2.
@@ -205,22 +205,32 @@ __device__ __forceinline__ void l2_prefetch_hint(const GemmKParams& p, int cta, 
 }
 
 __device__ __forceinline__ void ln_row_stats(const GemmKParams& p, long long m, float& ln_r, float& ln_nm) {
-  float s = 0.f, q = 0.f;
+  // Chunk j has mean m_j = s_j / 32 and M2_j about it, so over the P = ln_parts chunks
+  //   mean = m_0 + sum d_j / P,  M2 = sum M2_j + 32 (sum d_j^2 - (sum d_j)^2 / P),  d_j = m_j - m_0.
+  // Shifting by the first chunk's mean keeps every term on the scale of the spread, whatever |mean| / std, and the
+  // three sums are independent add chains (no divisions in the loop).
+  float m0 = 0.f, d1 = 0.f, d2 = 0.f, s2 = 0.f;
   const float2* base = p.ln_stats + m;
   for (int j0 = 0; j0 < p.ln_parts; j0 += 16) {
     float2 v[16];
 #pragma unroll
     for (int u = 0; u < 16; ++u)
       v[u] = (j0 + u < p.ln_parts) ? __ldcg(base + (size_t)(j0 + u) * p.M) : make_float2(0.f, 0.f);
+    if (j0 == 0) m0 = v[0].x * (1.f / 32.f);
+    // the slots past ln_parts are zeroed by a factor, not skipped by a branch: a branch per slot lets the compiler
+    // move each load next to its use, one dependent L2 round trip per partial again
 #pragma unroll
     for (int u = 0; u < 16; ++u) {
-      s += v[u].x;
-      q += v[u].y;
+      const float d = fmaf(v[u].x, 1.f / 32.f, -m0) * (j0 + u < p.ln_parts ? 1.f : 0.f);
+      d1 += d;
+      d2 = fmaf(d, d, d2);
+      s2 += v[u].y;
     }
   }
-  const float mu = s * p.ln_inv_c;
-  ln_r = rsqrtf(fmaxf(q * p.ln_inv_c - mu * mu, 0.f) + p.ln_eps);
-  ln_nm = -ln_r * mu;
+  const float ip = 32.f * p.ln_inv_c;   // 1 / ln_parts
+  const float m2 = fmaf(32.f, fmaxf(fmaf(-d1 * ip, d1, d2), 0.f), s2);
+  ln_r = rsqrtf(m2 * p.ln_inv_c + p.ln_eps);
+  ln_nm = -ln_r * fmaf(d1, ip, m0);
 }
 
 // Out-of-line activation for the rarely taken paths (general / split-K epilogues, SiLU): one copy of
@@ -853,18 +863,30 @@ ea_gemm_kernel(const __grid_constant__ GemmLaunch<NG> L, const int tiles_per_gro
             f[q * 8 + 0] += a.x; f[q * 8 + 1] += a.y; f[q * 8 + 2] += b.x; f[q * 8 + 3] += b.y;
             f[q * 8 + 4] += cc.x; f[q * 8 + 5] += cc.y; f[q * 8 + 6] += d.x; f[q * 8 + 7] += d.y;
           }
-          stg[slot] = make_uint4(ea_pack2(f[q * 8 + 0], f[q * 8 + 1]), ea_pack2(f[q * 8 + 2], f[q * 8 + 3]),
-                                 ea_pack2(f[q * 8 + 4], f[q * 8 + 5]), ea_pack2(f[q * 8 + 6], f[q * 8 + 7]));
+          const uint4 o = make_uint4(ea_pack2(f[q * 8 + 0], f[q * 8 + 1]), ea_pack2(f[q * 8 + 2], f[q * 8 + 3]),
+                                     ea_pack2(f[q * 8 + 4], f[q * 8 + 5]), ea_pack2(f[q * 8 + 6], f[q * 8 + 7]));
+          stg[slot] = o;
+          if (p.rowstats_out) {   // the statistics describe the rounded values the consumer will read
+            const float2 a = ea_unpack2(o.x), b = ea_unpack2(o.y), cc = ea_unpack2(o.z), d = ea_unpack2(o.w);
+            f[q * 8 + 0] = a.x; f[q * 8 + 1] = a.y; f[q * 8 + 2] = b.x; f[q * 8 + 3] = b.y;
+            f[q * 8 + 4] = cc.x; f[q * 8 + 5] = cc.y; f[q * 8 + 6] = d.x; f[q * 8 + 7] = d.y;
+          }
         }
         if (p.rowstats_out) {
-          // LayerNorm fold, producer side: this row's (sum, sum of squares) over the chunk's 32 stored values
-          float s0 = 0.f, s1 = 0.f, q0 = 0.f, q1 = 0.f;
+          // LayerNorm fold, producer side: this row's (sum, sum of squared deviations from the chunk mean) over the
+          // chunk's 32 stored values.  Centring on the chunk mean keeps M2 exact to a few ulps whatever |mean| / std.
+          float s0 = 0.f, s1 = 0.f;
+#pragma unroll
+          for (int j = 0; j < 32; j += 2) { s0 += f[j]; s1 += f[j + 1]; }
+          const float s = s0 + s1, mc = s * (1.f / 32.f);
+          float q0 = 0.f, q1 = 0.f;
 #pragma unroll
           for (int j = 0; j < 32; j += 2) {
-            s0 += f[j]; q0 = fmaf(f[j], f[j], q0);
-            s1 += f[j + 1]; q1 = fmaf(f[j + 1], f[j + 1], q1);
+            const float d0 = f[j] - mc, d1 = f[j + 1] - mc;
+            q0 = fmaf(d0, d0, q0);
+            q1 = fmaf(d1, d1, q1);
           }
-          if (ri.ok && n_first < p.N) p.rowstats_out[(size_t)(n_first >> 5) * p.M + ri.m] = make_float2(s0 + s1, q0 + q1);
+          if (ri.ok && n_first < p.N) p.rowstats_out[(size_t)(n_first >> 5) * p.M + ri.m] = make_float2(s, q0 + q1);
         }
         if (half == 1 || c + 32 >= BN)
           stage_flush(stg, lane, p.out, p.ldo, p.out2, p.ldo2, ri.m, ri.ok, n_first - half * 32,
@@ -1171,9 +1193,15 @@ static int gemm_fill_group(const ea_gemm_args* a, GemmGroup& G, GemmShape& sh) {
   // rather than the activations and skip tensors the following launches read.
   p.b_policy = 0x12F0000000000000ull;
   if (a->row_scale && (a->act == EA_ACT_GEGLU || a->rowstats_out || a->ln_stats)) return EA_ERR_ARG;
+  // The GEGLU epilogues apply the bias and the LayerNorm fold only
+  if (a->act == EA_ACT_GEGLU &&
+      (a->rowvec || a->residual || a->out2 || a->out_f32 || a->accumulate || a->out_scale != 1.0f))
+    return EA_ERR_ARG;
   sh.ln_any = a->rowstats_out || a->ln_stats;
   if (sh.ln_any) {
-    if (a->mode != EA_GEMM_LINEAR || a->rowvec || a->out_f32 || a->accumulate) return EA_ERR_ARG;
+    // rows_per_batch could make a tile span more than two batches, whose (general) epilogue has no fold
+    if (a->mode != EA_GEMM_LINEAR || a->rowvec || a->rows_per_batch != 0 || a->out_f32 || a->accumulate)
+      return EA_ERR_ARG;
     if (a->rowstats_out && (a->N % 32 != 0 || a->act == EA_ACT_GEGLU)) return EA_ERR_SHAPE;
     if (a->ln_stats && (!a->ln_g || a->ln_parts <= 0 || a->K != a->ln_parts * 32)) return EA_ERR_ARG;
     p.rowstats_out = reinterpret_cast<float2*>(a->rowstats_out);

@@ -373,7 +373,7 @@ class BlockRunner:
         self.groupnorm(x, p + ".norm", xn, B=B, HW=N, C_=c, eps=1e-6, silu=False, workspace=gn_ws, ldx=x.stride(2))
         fold = self.ln_fold
 
-        def stats():   # per-row partial (sum, sumsq) per 32-column chunk, written by the producing GEMM
+        def stats():   # per-row partial (sum, M2 about the chunk mean) per 32-column chunk, written by the producing GEMM
             return torch.empty(n, inner // 32, M // n, 2, device=self.dev, dtype=torch.float32) if fold else None
 
         def normed(t, st, name, nrm, **kw):   # GEMM on LayerNorm(t): folded, or LayerNorm launch + plain GEMM

@@ -175,7 +175,8 @@ class weight_lookahead:
 
 def gemm(a, w, out=None, **kw):
     """out = epilogue(A @ W^T).  conv = (B, H, W, Cin) output-space geometry for CONV modes.
-    rowstats_out: fp32 [N/32, M, 2] per-row partial (sum, sumsq) of the stored values (LayerNorm fold, producer);
+    rowstats_out: fp32 [N/32, M, 2] per row and 32-column chunk of the stored (half) values: (sum, sum of squared
+    deviations from the chunk mean sum / 32) (LayerNorm fold, producer);
     ln = (stats [K/32, M, 2], g [N], eps): the consumer side - `w` is W*gamma, `bias` is W beta + b."""
     lib = L.lib()
     g = L.GemmArgs()

@@ -71,7 +71,9 @@ void ea_reset_launch_count(void);
  * Epilogue order: +bias[n] -> +rowvec[batch(m), n] -> act -> *out_scale -> +residual[m,n]
  *                 -> (+= out[m,n] if accumulate) -> store out (and out2).
  * act GEGLU: W rows must be pre-interleaved per 128-row block as [64 value rows | 64 gate rows];
- *            output has N/2 columns: value * gelu(gate)   (attention.py:54-56).
+ *            output has N/2 columns: value * gelu(gate)   (attention.py:54-56).  Its epilogue applies the bias
+ *            and the LayerNorm fold only: rowvec, residual, out2, out_f32, accumulate, row_scale and
+ *            out_scale != 1 are rejected (EA_ERR_ARG).
  * Split-K: when the output has fewer tiles than the GPU has SMs, K is split across CTAs; each
  *            split CTA publishes its fp32 partial tile to `workspace`, waits for its siblings
  *            (all resident by construction) and finishes a 1/splits share of the tile with the
@@ -116,11 +118,13 @@ typedef struct ea_gemm_args {
   /* LayerNorm folded into the GEMMs around it (BasicTransformerBlock norm1/2/3, ldm/modules/attention.py:
    * 263-275): LN(x) W^T = rstd[m] * (x (W*gamma)^T - mean[m] * g) + (W beta + b), g[n] = sum_k (W*gamma)[n,k].
    * The GEMM that PRODUCES x (proj_in / to_out + residual) also writes per-row partial statistics of the
-   * values it stores, one (sum, sum of squares) pair per 32-column chunk: rowstats_out fp32 [N/32][M][2]
-   * (deterministic: no atomics).  The GEMM that CONSUMES x (to_q/k/v, GEGLU proj) takes W*gamma as `w`,
-   * W beta + b as `bias`, and ln_stats (= the producer's rowstats_out, ln_parts = K/32 chunks), ln_g, ln_eps:
-   * its epilogue applies rstd / mean per output row.  LINEAR mode, no rowvec / out_f32 / accumulate, N % 32 == 0
-   * for the producer; K is never split for either.  No LayerNorm launch and no normalised tensor exists. */
+   * values it stores (after rounding to the storage type), one pair per 32-column chunk j: (s_j = sum, M2_j = sum of
+   * (x - s_j / 32)^2), rowstats_out fp32 [N/32][M][2] (deterministic: no atomics).  The GEMM that CONSUMES x
+   * (to_q/k/v, GEGLU proj) takes W*gamma as `w`, W beta + b as `bias`, and ln_stats (= the producer's
+   * rowstats_out, ln_parts = K/32 chunks), ln_g, ln_eps: it merges the partials in chunk order, about the first
+   * chunk's mean, and its epilogue applies rstd / mean per output row.  LINEAR mode, no rowvec / rows_per_batch /
+   * out_f32 / accumulate / row_scale, N % 32 == 0 and no GEGLU for the producer; K is never split for either.
+   * No LayerNorm launch and no normalised tensor exists. */
   float* rowstats_out;
   const float* ln_stats;
   const float* ln_g;         /* fp32 [N] */

@@ -35,6 +35,11 @@ def gemm(a, w, out=None, *, mode=0, M=None, N=None, K=None, lda=None, ldw=0, con
          out_scale=1.0, accumulate=False, ldo=None, ldr=None, ldo2=None, ld_extra=0, force_bn=0,
          force_stages=0, force_splits=0, force_2cta=0, force_persistent=0, rowstats_out=None, ln=None,
          row_scale=None):
+    if act == EA_ACT_GEGLU and (rowvec is not None or residual is not None or out2 is not None or out_f32 is not None
+                                or accumulate or out_scale != 1.0 or row_scale is not None):
+        raise RuntimeError("ea_gemm failed (-1): GEGLU applies the bias and the LayerNorm fold only")
+    if (ln is not None or rowstats_out is not None) and rows_per_batch:
+        raise RuntimeError("ea_gemm failed (-1): no rows_per_batch with the LayerNorm fold")
     _bump()
     Nn = w.shape[0]
     if mode == EA_GEMM_LINEAR:
@@ -43,9 +48,10 @@ def gemm(a, w, out=None, *, mode=0, M=None, N=None, K=None, lda=None, ldw=0, con
         batch_rows = rows_per_batch
         if ln is not None:      # LayerNorm fold: rstd * (x W'^T - mean * g) (+ bias below), stats from the producer
             stats, g, eps = ln
-            sq = stats.float().sum(0)                                   # [M, 2]
-            mu = sq[:, 0] / A.shape[1]
-            rstd = torch.rsqrt((sq[:, 1] / A.shape[1] - mu * mu).clamp_min(0) + eps)
+            s, m2 = stats[..., 0].float(), stats[..., 1].float()      # [K/32, M] per chunk: sum, M2 about its mean
+            mu = s.sum(0) / A.shape[1]
+            var = (m2.sum(0) + 32.0 * ((s / 32.0 - mu) ** 2).sum(0)) / A.shape[1]
+            rstd = torch.rsqrt(var + eps)
             y = rstd[:, None] * (y - mu[:, None] * g[None, :])
     else:
         B, H, W_, Cin = conv
@@ -64,7 +70,7 @@ def gemm(a, w, out=None, *, mode=0, M=None, N=None, K=None, lda=None, ldw=0, con
         y = y + bias
     if rowvec is not None:
         nb = y.shape[0] // batch_rows if batch_rows else 1
-        y = y + (rowvec.repeat_interleave(batch_rows, 0) if batch_rows else rowvec[:1])
+        y = y + (rowvec.repeat_interleave(batch_rows, 0)[:y.shape[0]] if batch_rows else rowvec[:1])
     if act == EA_ACT_SILU:
         y = F.silu(y)
     elif act == EA_ACT_GELU:
@@ -85,9 +91,11 @@ def gemm(a, w, out=None, *, mode=0, M=None, N=None, K=None, lda=None, ldw=0, con
     tgt.copy_(y.reshape(tgt.shape))
     if out2 is not None:
         out2.copy_(y.reshape(out2.shape))
-    if rowstats_out is not None:
-        yc = y.reshape(y.shape[0], -1, 32)
-        rowstats_out.copy_(torch.stack([yc.sum(-1), (yc * yc).sum(-1)], -1).permute(1, 0, 2))
+    if rowstats_out is not None:    # statistics of the stored values, each chunk's M2 about its own mean
+        yc = tgt.float().reshape(y.shape[0], -1, 32)
+        s = yc.sum(-1)
+        m2 = ((yc - (s / 32.0)[..., None]) ** 2).sum(-1)
+        rowstats_out.copy_(torch.stack([s, m2], -1).permute(1, 0, 2))
     return tgt
 
 

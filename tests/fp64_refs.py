@@ -1,4 +1,4 @@
-"""Float64 references of the library's non-GEMM operators (and the GEMM epilogue inputs row_scale / out_f32), written
+"""Float64 references of the library's non-GEMM operators (and the GEMM epilogue: activations, row_scale, out_f32), written
 from each operation's definition and independent of tests/cpu_ops.py and tools/gpu_probe_ops.py.
 
 Every function takes the kernel's own inputs upcast to float64 (any device) and returns float64 results in the
@@ -30,6 +30,33 @@ def silu_eval_err(y):
     """Bound on the kernel's fp32 SiLU (ex2.approx + rcp.approx) at y, relative to |silu(y)|: the rounding of
     y * log2(e) is amplified by |y|, the two approximations add a few ulps."""
     return U32 * (8.0 + 2.0 * y.abs()) * silu(y).abs()
+
+
+def gelu(y):
+    """Exact-erf GELU, F.gelu's default: y / 2 (1 + erf(y / sqrt 2)), written as y / 2 erfc(-y / sqrt 2) so that
+    the negative tail (fp16 subnormal outputs) keeps full relative precision."""
+    return 0.5 * y * torch.erfc(-y * math.sqrt(0.5))
+
+
+def gelu_eval_err(y):
+    """Bound on the kernel's fp32 gelu_erf_f at y: erf from Abramowitz & Stegun 7.1.26 (stated |error| < 1.5e-7)
+    scaled by |y| / 2, 32 fp32 ulps of |y| / 2 for evaluating it (ex2.approx, rcp.approx, the polynomial), and 8 ulps
+    of the result."""
+    return 0.5 * y.abs() * (1.5e-7 + 32.0 * U32) + 8.0 * U32 * gelu(y).abs()
+
+
+def geglu_split(y):
+    """[M, N] pre-activations in the weight layout nets packs for GEGLU (per 128 columns: 64 value | 64 gate) ->
+    (value, gate), each [M, N / 2] in output column order."""
+    M, N = y.shape
+    v = y.reshape(M, N // 128, 2, 64)
+    return v[:, :, 0].reshape(M, N // 2), v[:, :, 1].reshape(M, N // 2)
+
+
+def geglu(y):
+    """value * gelu(gate) (ldm/modules/attention.py:54-56) of pre-activations in the packed layout."""
+    x, g = geglu_split(y)
+    return x * gelu(g)
 
 
 # ---- normalisations -------------------------------------------------------------------------------------------

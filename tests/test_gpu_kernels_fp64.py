@@ -1,5 +1,6 @@
-"""-m gpu: the operators of ea_pointwise.cu, and the row_scale / out_f32 inputs of the ea_gemm epilogue, against
-float64 references (tests/fp64_refs.py) at the shapes, strides and value ranges production reaches.
+"""-m gpu: the operators of ea_pointwise.cu, and the ea_gemm epilogue (row_scale / out_f32 inputs, SiLU / GELU /
+GEGLU on every epilogue path, the LayerNorm fold on both of its sides), against float64 references
+(tests/fp64_refs.py) at the shapes, strides and value ranges production reaches.
 
 Every gate is per element:
   * layout / copy operators must match the reference bit for bit;
@@ -7,7 +8,15 @@ Every gate is per element:
     g (x - mu) r + b (an fp32 evaluation cannot do better where those terms cancel);
   * reductions: ulp_out(ref) + K u sum |a_i b_i| (u = 2^-24, K = reduction length, ulp_out = 0 for fp32 outputs),
     propagated through whatever formula is applied to the reduced value;
-  * ea_softmax_rows (uses __expf): 1 ulp of the output plus 1e-5 |ref|.
+  * ea_softmax_rows (uses __expf): 1 ulp of the output plus 1e-5 |ref|;
+  * GEMM activations: the pre-activation's bound e = (K + 2) u (sum |a w| + |bias| + |rowvec|) through the
+    activation's largest slope (SiLU 1.1, GELU 1.13; GEGLU |gelu(g)| e_x + |x| (1.13 e_g + ...)) plus its fp32
+    evaluation error (fp64_refs.silu_eval_err / gelu_eval_err), then scaled by |out_scale|, plus one u per add of
+    the residual / accumulated value and 1 ulp of the output;
+  * the LayerNorm fold with the identity as consumer weights: exactly the LayerNorm gate above, per class of row
+    offset (|mean| / std = 0, 10, 100, 256, variance near eps); a packed consumer: ulp + (K + 2) u rstd
+    (sum |x w'| + |mean| |g|) + 2 u |c|; the producer's rowstats_out per chunk: 32 u sum |x| for the sum,
+    40 u M2 + 32 (u sum |x|)^2 for the squared deviations about the chunk mean.
 A failure names the worst element (index, value, reference, bound)."""
 import math
 
@@ -595,6 +604,233 @@ def test_gemm_out_f32_accumulate_ragged():
     _close("ea_gemm out_f32", "300x72 accumulate", s, ref, (K + 1) * U * mag + 2 * U * (t.abs() + old.abs()))
 
 
+# ================================================ GEMM activations =============================================
+ACTS = {"silu": L.EA_ACT_SILU, "gelu": L.EA_ACT_GELU, "geglu": L.EA_ACT_GEGLU}
+
+
+def _act_ref(act, pre, e):
+    """act(pre) and its error bound, for an fp32 pre-activation `pre` (float64) whose error is bounded by `e`."""
+    if act == "silu":
+        return R.silu(pre), 1.1 * e + R.silu_eval_err(pre)
+    if act == "gelu":
+        return R.gelu(pre), 1.13 * e + R.gelu_eval_err(pre)
+    x, g = R.geglu_split(pre)
+    ex, eg = R.geglu_split(e)
+    gg = R.gelu(g)
+    return x * gg, gg.abs() * ex + x.abs() * (1.13 * eg + R.gelu_eval_err(g))
+
+
+def _act_check(kernel, what, got, act, pre, e, scale=1.0, res=None, old=None):
+    """got = act(pre) * scale (+ res) (+ old) with the rounding of each step, in got's dtype."""
+    y, err = _act_ref(act, pre, e)
+    t = y * scale
+    extra = [v for v in (res, old) if v is not None]
+    ref = t + sum(extra) if extra else t
+    bound = abs(scale) * err + (1 + len(extra)) * U * (t.abs() + sum(v.abs() for v in extra)) + R.ulp(ref, got.dtype)
+    return _close(kernel, what, got, ref, bound)
+
+
+# epilogue paths: the default (fast) one; the general one (a time-embedding row vector whose images change inside a
+# tile); forced split-K with the sibling wait and without it (no_spin); the persistent grid; two row tiles per CTA;
+# an fp32 destination accumulated into
+ACT_PATHS = ["default", "general", "split_k", "split_k_no_spin", "persistent", "row_pair", "f32_accumulate"]
+# GEGLU has neither a row vector nor an fp32 destination; split-K only where every split CTA is resident (M = 300)
+ACT_CASES = [(act, M, K, path) for act in ACTS for path in ACT_PATHS for M in (300, 8192) for K in (320, 200)
+             if not (act == "geglu" and path in ("general", "f32_accumulate"))
+             and not (path.startswith("split_k") and M > 300) and not (path == "f32_accumulate" and K != 320)]
+
+
+@pytest.mark.parametrize("act,M,K,path", ACT_CASES, ids=[f"{a}-M{m}-K{k}-{p}" for a, m, k, p in ACT_CASES])
+def test_gemm_activation(act, M, K, path):
+    """Bias spread over [-12, 12] reaches SiLU's saturation and GELU's negative tail (fp16 subnormal outputs); SiLU and
+    GELU follow the documented order act -> * out_scale -> + residual (zero on every second row, so the tail shows)."""
+    N = 1280
+    geglu = act == "geglu"
+    h = _half()
+    a = _randn((M, K), 111, h)
+    w = _randn((N, K), 112, h, scale=K ** -0.5)
+    bias = torch.rand(N, generator=_gen(113), device=DEV) * 24.0 - 12.0
+    kw = dict(bias=bias, act=ACTS[act])
+    rv = None
+    if path == "general":
+        rv = _randn(((M + 49) // 50, N), 114, scale=2.0)
+        kw.update(rowvec=rv, rows_per_batch=50)            # a 128-row tile spans three images
+    elif path.startswith("split_k"):
+        kw.update(force_splits=4, force_bn=128)            # 30 tiles x <= 4 splits: every CTA resident
+    elif path == "persistent":
+        kw["force_persistent"] = 2
+    elif path == "row_pair":
+        kw["force_2cta"] = 1
+    res = old = None
+    n_out = N // 2 if geglu else N
+    if not geglu:
+        kw["out_scale"] = 0.75
+        res = _randn((M, n_out), 115, h)
+        res[::2] = 0.0
+        kw["residual"] = res
+    if path == "f32_accumulate":
+        old = _randn((M, n_out), 116)
+        out = old.clone()
+        call = lambda: ops.gemm(a, w, out_f32=out, accumulate=True, **kw)
+    else:
+        out = torch.full((M, n_out), 7.0, device=DEV, dtype=h)
+        call = lambda: ops.gemm(a, w, out, **kw)
+    if path == "split_k_no_spin":
+        with _concurrent_lane():
+            call()
+    else:
+        call()
+    torch.cuda.synchronize()
+    pre, _, mag = R.gemm_epilogue(a.double(), w.double(), bias.double())
+    if rv is not None:
+        rvd = rv.double().repeat_interleave(50, dim=0)[:M]
+        pre, mag = pre + rvd, mag + rvd.abs()
+    e = (K + 2) * U * mag
+    _act_check(f"ea_gemm {act}", f"M={M} K={K} {path}", out, act, pre, e, kw.get("out_scale", 1.0),
+               None if res is None else res.double(), None if old is None else old.double())
+
+
+@pytest.mark.parametrize("act", ["silu", "gelu"])
+def test_gemm_activation_conv(act):
+    """CONV_S1 (3x3) with the ResBlock's time-embedding row vector, one per image."""
+    h = _half()
+    B, H, W, cin, cout = 3, 16, 16, 128, 640
+    x = _randn((B, H, W, cin), 121, h)
+    w = _randn((cout, 3, 3, cin), 122, h, scale=(9 * cin) ** -0.5)
+    bias = torch.rand(cout, generator=_gen(123), device=DEV) * 24.0 - 12.0
+    rv = _randn((B, cout), 124, scale=2.0)
+    res = _randn((B * H * W, cout), 125, h)
+    out = torch.full((B * H * W, cout), 7.0, device=DEV, dtype=h)
+    ops.gemm(x, w.reshape(cout, 9 * cin), out, mode=L.EA_GEMM_CONV_S1, conv=(B, H, W, cin), bias=bias, rowvec=rv,
+             act=ACTS[act], out_scale=0.75, residual=res)
+    torch.cuda.synchronize()
+    pre, mag = R.conv_nhwc(x.double(), w.double().permute(1, 2, 3, 0), bias.double())
+    rvd = rv.double()[:, None, None, :]
+    pre, mag = (pre + rvd).reshape(-1, cout), (mag + rvd.abs()).reshape(-1, cout)
+    _act_check(f"ea_gemm {act}", "conv 3x3 + time embedding", out, act, pre, (9 * cin + 2) * U * mag, 0.75,
+               res.double())
+
+
+# ================================================ GEMM LayerNorm fold ==========================================
+# Row classes of the producer's output: (|mean|, spread); |mean| / std = 0, 10, 100, 256, and a variance comparable
+# to eps.  Rows cycle through them.
+LN_ROWS = {"offset0": (0.0, 1.0), "offset10": (2.5, 0.25), "offset100": (25.0, 0.25), "offset256": (64.0, 0.25),
+           "var_near_eps": (0.0, 3.2e-3)}
+
+
+def _ln_producer_inputs(M, C, seed):
+    """Producer operands of x = a w0^T + b0 + residual whose rows fall in the LN_ROWS classes."""
+    h = _half()
+    cls = torch.arange(M, device=DEV) % len(LN_ROWS)
+    sign = torch.where(torch.rand(M, generator=_gen(seed), device=DEV) < 0.5, -1.0, 1.0)
+    off = torch.tensor([v[0] for v in LN_ROWS.values()], device=DEV)[cls] * sign
+    spread = torch.tensor([v[1] for v in LN_ROWS.values()], device=DEV)[cls]
+    a = (_randn((M, C), seed + 1) * spread[:, None] * 0.7).to(h)
+    w0 = _randn((C, C), seed + 2, h, scale=C ** -0.5)
+    b0 = _randn((C,), seed + 3, scale=1e-3)
+    res = (_randn((M, C), seed + 4) * spread[:, None] * 0.7 + off[:, None]).to(h)
+    return a, w0, b0, res, cls
+
+
+def _ln_stats_check(st, x):
+    """rowstats_out [C/32, M, 2] against float64 statistics of the stored x: per 32-column chunk the sum and the sum of
+    squared deviations from the chunk mean.  Bounds: 32 u sum|x| for the sum; for M2 40 u M2 plus what a chunk mean
+    off by up to u sum|x| adds (32 of its square)."""
+    M, C = x.shape
+    xc = x.double().reshape(M, C // 32, 32).permute(1, 0, 2)
+    s = xc.sum(-1)
+    m2 = ((xc - s[..., None] / 32) ** 2).sum(-1)
+    sabs = xc.abs().sum(-1)
+    _close("ea_gemm rowstats_out", "chunk sums", st[..., 0], s, 32 * U * sabs)
+    _close("ea_gemm rowstats_out", "chunk M2", st[..., 1], m2, 40 * U * m2 + 32 * (U * sabs) ** 2)
+
+
+def _ln_fold_check(x, out, beta, cls):
+    """The fold with the identity as consumer weights is a plain LayerNorm: the gate of test_layernorm per row class."""
+    ref, terms = R.layernorm(x.double(), torch.ones_like(beta, dtype=torch.float64), beta.double(), 1e-5)
+    bound = R.ulp(ref, _half()) + NORM_K * U * terms
+    fails = []
+    for i, name in enumerate(LN_ROWS):
+        rows = cls == i
+        try:
+            _close(f"ea_gemm LN fold {name}", "identity consumer", out[rows], ref[rows], bound[rows])
+        except AssertionError as exc:
+            fails.append(str(exc))
+    return fails
+
+
+@pytest.mark.parametrize("variant", ["default", "persistent", "row_pair", "grouped"])
+@pytest.mark.parametrize("M", [301, 4096])
+@pytest.mark.parametrize("C", [320, 640, 1280])
+def test_gemm_layernorm_fold_identity(C, M, variant):
+    """Producer x = a w0^T + b0 + residual with rowstats_out; consumer with w' = I, ln_g = 1, bias = beta computes
+    (x - mean) rstd + beta exactly in its product, so every error beyond the LayerNorm gate comes from the
+    statistics.  Grouped: three networks in one launch on each side, each with its own statistics."""
+    h = _half()
+    force = {"default": {}, "persistent": dict(force_persistent=2), "row_pair": dict(force_2cta=1),
+             "grouped": {}}[variant]
+    n = 3 if variant == "grouped" else 1
+    eye = torch.eye(C, device=DEV, dtype=h)
+    ones = torch.ones(C, device=DEV)
+    prod, cons, checks = [], [], []
+    for g in range(n):
+        a, w0, b0, res, cls = _ln_producer_inputs(M, C, 200 + 10 * g + C + M)
+        x = torch.full((M, C), 7.0, device=DEV, dtype=h)
+        st = torch.full((C // 32, M, 2), float("nan"), device=DEV)
+        beta = _randn((C,), 209 + g, scale=0.3)
+        out = torch.full((M, C), 7.0, device=DEV, dtype=h)
+        prod.append((a, w0, x, dict(bias=b0, residual=res, rowstats_out=st, **force)))
+        cons.append((x, eye, out, dict(bias=beta, ln=(st, ones, 1e-5), **force)))
+        checks.append((x, st, out, beta, cls))
+    if n == 1:
+        ops.gemm(prod[0][0], prod[0][1], prod[0][2], **prod[0][3])
+        ops.gemm(cons[0][0], cons[0][1], cons[0][2], **cons[0][3])
+    else:
+        ops.gemm_grouped(prod)
+        ops.gemm_grouped(cons)
+    torch.cuda.synchronize()
+    fails = []
+    for g, (x, st, out, beta, cls) in enumerate(checks):
+        fails += [f"group {g}: {m}" for m in _ln_fold_check(x, out, beta, cls)]
+        try:
+            _ln_stats_check(st, x)
+        except AssertionError as exc:
+            fails.append(f"group {g}: {exc}")
+    assert not fails, "\n".join(fails)
+
+
+@pytest.mark.parametrize("act", ["none", "geglu"])
+@pytest.mark.parametrize("MC", [(301, 320), (4096, 640)], ids=lambda s: f"M{s[0]}_C{s[1]}")
+def test_gemm_layernorm_fold_consumer(MC, act):
+    """A consumer packed as nets packs it: w' = fp16(W gamma), g = sum_k w' (fp32), bias c = W beta + b; linear with
+    N = 3C (qkv) or GEGLU with N = 8C (ff1).  Reference ((x - mean) rstd) w'^T + c in float64 from the stored x."""
+    M, C = MC
+    h = _half()
+    geglu = act == "geglu"
+    N = 8 * C if geglu else 3 * C
+    a, w0, b0, res, _ = _ln_producer_inputs(M, C, 300 + C)
+    x = torch.full((M, C), 7.0, device=DEV, dtype=h)
+    st = torch.full((C // 32, M, 2), float("nan"), device=DEV)
+    ops.gemm(a, w0, x, bias=b0, residual=res, rowstats_out=st)
+    W = _randn((N, C), 301, scale=C ** -0.5)
+    gam, bet, b1 = _randn((C,), 302, scale=0.2, offset=1.0), _randn((C,), 303, scale=0.3), _randn((N,), 304)
+    wp = (W.double() * gam.double()).to(h)
+    gv = wp.double().sum(1).float()
+    cv = (W.double() @ bet.double() + b1.double()).float()
+    out = torch.full((M, N // 2 if geglu else N), 7.0, device=DEV, dtype=h)
+    ops.gemm(x, wp, out, bias=cv, ln=(st, gv, 1e-5), act=L.EA_ACT_GEGLU if geglu else L.EA_ACT_NONE)
+    torch.cuda.synchronize()
+    xd, wd, cd = x.double(), wp.double(), cv.double()
+    mu = xd.mean(-1, keepdim=True)
+    r = (xd.var(-1, correction=0, keepdim=True) + 1e-5).rsqrt()
+    pre = ((xd - mu) * r) @ wd.T + cd
+    e = (C + 2) * U * r * (xd.abs() @ wd.abs().T + mu.abs() * gv.double().abs()) + 2 * U * cd.abs()
+    if geglu:
+        _act_check("ea_gemm LN fold consumer", f"geglu M={M} C={C}", out, "geglu", pre, e)
+    else:
+        _close("ea_gemm LN fold consumer", f"linear M={M} C={C}", out, pre, R.ulp(pre, h) + e)
+
+
 # ================================================ argument validation ==========================================
 def _rejects(status, fn):
     n0 = ops.launch_count()
@@ -639,3 +875,16 @@ def test_rejected_arguments():
     rs = torch.ones(128, device=DEV)
     _rejects(ARG, lambda: ops.gemm(a, wg, torch.empty(128, 128, device=DEV, dtype=h), act=L.EA_ACT_GEGLU,
                                    row_scale=rs))
+    # gemm: the GEGLU epilogue applies the bias and the LayerNorm fold only
+    o = torch.empty(128, 128, device=DEV, dtype=h)
+    for extra in (dict(rowvec=torch.ones(1, 256, device=DEV)), dict(residual=torch.zeros(128, 128, device=DEV, dtype=h)),
+                  dict(out2=torch.empty(128, 128, device=DEV, dtype=h)), dict(accumulate=True), dict(out_scale=0.5)):
+        _rejects(ARG, lambda: ops.gemm(a, wg, o, act=L.EA_ACT_GEGLU, **extra))
+    _rejects(ARG, lambda: ops.gemm(a, wg, out_f32=torch.empty(128, 128, device=DEV), act=L.EA_ACT_GEGLU))
+    # gemm: rows_per_batch with the LayerNorm fold on either side
+    wl = torch.zeros(64, 64, device=DEV, dtype=h)
+    st = torch.zeros(2, 128, 2, device=DEV)
+    _rejects(ARG, lambda: ops.gemm(a, wl, torch.empty(128, 64, device=DEV, dtype=h), rowstats_out=st,
+                                   rows_per_batch=64))
+    _rejects(ARG, lambda: ops.gemm(a, wl, torch.empty(128, 64, device=DEV, dtype=h),
+                                   ln=(st, torch.ones(64, device=DEV), 1e-5), rows_per_batch=64))

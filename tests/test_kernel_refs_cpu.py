@@ -153,6 +153,64 @@ def test_gemm_epilogue():
     assert torch.allclose(mag, (a.abs() @ w.abs().T + b.abs()) * 0.7 * rs[:, None])
 
 
+def test_gelu_matches_functional():
+    y = torch.cat([torch.linspace(-12, 12, 4001, dtype=torch.float64), _rn(1000, seed=30) * 4])
+    got = R.gelu(y)
+    # F.gelu forms 1 + erf, which cancels in the negative tail: compare it where that costs < 1e-12 relative
+    body = y > -3
+    assert torch.allclose(got[body], F.gelu(y)[body], rtol=1e-12, atol=0)
+    want = torch.tensor([0.5 * v * math.erfc(-v / math.sqrt(2.0)) for v in y.tolist()], dtype=torch.float64)
+    assert torch.allclose(got, want, rtol=1e-13, atol=0)
+
+
+def test_geglu_matches_interleave_loop():
+    M, N = 3, 384
+    y = _rn(M, N, seed=31) * 3
+    want = torch.empty(M, N // 2, dtype=torch.float64)
+    for m in range(M):
+        for blk in range(N // 128):
+            for i in range(64):
+                x, g = float(y[m, blk * 128 + i]), float(y[m, blk * 128 + 64 + i])
+                want[m, blk * 64 + i] = x * 0.5 * g * math.erfc(-g / math.sqrt(2.0))
+    assert torch.allclose(R.geglu(y), want, rtol=1e-13, atol=1e-300)
+
+
+def _gelu_erf_f32(y, pert):
+    """The kernel's gelu_erf_f (ea_common.cuh) in fp32 numpy, with relative error `pert` applied to the results of
+    rcp.approx and ex2.approx (fma as an fp32 multiply-add in float64, rounded once)."""
+    f = np.float32
+
+    def fma(a, b, c):
+        return (a.astype(np.float64) * b + c).astype(np.float32)
+
+    z = (np.abs(y) * f(0.70710678118654752)).astype(np.float32)
+    t = (f(1) / fma(f(0.3275911), z, f(1))).astype(np.float32) * f(pert)
+    poly = fma(f(1.061405429), t, f(-1.453152027))
+    for c in (1.421413741, -0.284496736, 0.254829592):
+        poly = fma(poly, t, f(c))
+    arg = ((z * z).astype(np.float32) * f(-1.4426950408889634)).astype(np.float32)
+    ex = np.exp2(arg.astype(np.float64)).astype(np.float32) * f(pert)
+    e = fma((-poly * t).astype(np.float32), ex, f(1))
+    return (f(0.5) * y * (f(1) + np.copysign(e, y)).astype(np.float32)).astype(np.float32)
+
+
+def test_gelu_eval_err_bounds_fp32_emulation():
+    """gelu_eval_err bounds the kernel's formula evaluated in fp32, with +-2^-22 on the two .approx results, over a
+    dense grid of [-12, 12] and log-spaced points down to 1e-8 on both sides."""
+    y = np.concatenate([np.linspace(-12, 12, 400001), -np.logspace(-8, 1.1, 4001),
+                        np.logspace(-8, 1.1, 4001)]).astype(np.float32)
+    yd = torch.from_numpy(y.astype(np.float64))
+    ref, bound = R.gelu(yd), R.gelu_eval_err(yd)
+    worst = 0.0
+    for pert in (1 - 2.0 ** -22, 1.0, 1 + 2.0 ** -22):
+        got = torch.from_numpy(_gelu_erf_f32(y, pert).astype(np.float64))
+        err = (got - ref).abs()
+        ratio = torch.where(err == 0, torch.zeros_like(err), err / bound)
+        assert bool((err <= bound).all()), float(ratio.max())
+        worst = max(worst, float(ratio.max()))
+    assert worst > 0.05        # the bound is not vacuous
+
+
 def test_ddim_update_matches_ddim_scheduler():
     s = DDIMScheduler()
     s.set_timesteps(20)
