@@ -435,9 +435,11 @@ __global__ void timestep_embedding_kernel(const float* __restrict__ t, float* __
 }
 
 // ---------------- out conv (C -> 4) + CFG + DDIM + inpaint blend -------------
-// One warp per (image, pixel): both CFG halves are reduced by the same warp so the guidance
-// combine and the DDIM update happen in registers.
-__global__ void out_cfg_ddim_kernel(const ea_half* __restrict__ xn, const float* __restrict__ w,
+// One warp per (image, pixel).  kCfg: xn, eps_out and lat_half hold 2*Nimg rows (unconditional first) and both
+// halves are reduced by the same warp, so the guidance combine and the DDIM update happen in registers.  !kCfg:
+// they hold the Nimg rows alone and the update reads their eps directly (sampling without guidance).
+template <bool kCfg>
+__global__ void out_ddim_kernel(const ea_half* __restrict__ xn, const float* __restrict__ w,
                                     const float* __restrict__ bias, float* __restrict__ latents,
                                     float* __restrict__ eps_out, const float* __restrict__ coef,
                                     float guidance, const float* __restrict__ known,
@@ -465,17 +467,21 @@ __global__ void out_cfg_ddim_kernel(const ea_half* __restrict__ xn, const float*
       int wi = wq + kw - 1;
       if (wi < 0 || wi >= W) continue;
       const ea_half* pu = xn + (((long long)img * H + hi) * W + wi) * C;
-      const ea_half* pc = xn + (((long long)(img + Nimg) * H + hi) * W + wi) * C;
+      const ea_half* pc = kCfg ? xn + (((long long)(img + Nimg) * H + hi) * W + wi) * C : nullptr;
       const float* wt = w + (kh * 3 + kw) * C;  // + o*9*C
       for (int c = lane * 8; c < C; c += 256) {
         uint4 uu = __ldg(reinterpret_cast<const uint4*>(pu + c));
-        uint4 uc = __ldg(reinterpret_cast<const uint4*>(pc + c));
         float2 a0 = ea_unpack2(uu.x), a1 = ea_unpack2(uu.y), a2 = ea_unpack2(uu.z),
                a3 = ea_unpack2(uu.w);
-        float2 b0 = ea_unpack2(uc.x), b1 = ea_unpack2(uc.y), b2 = ea_unpack2(uc.z),
-               b3 = ea_unpack2(uc.w);
         float xu[8] = {a0.x, a0.y, a1.x, a1.y, a2.x, a2.y, a3.x, a3.y};
-        float xc[8] = {b0.x, b0.y, b1.x, b1.y, b2.x, b2.y, b3.x, b3.y};
+        float xc[8];
+        if constexpr (kCfg) {
+          uint4 uc = __ldg(reinterpret_cast<const uint4*>(pc + c));
+          float2 b0 = ea_unpack2(uc.x), b1 = ea_unpack2(uc.y), b2 = ea_unpack2(uc.z),
+                 b3 = ea_unpack2(uc.w);
+          xc[0] = b0.x; xc[1] = b0.y; xc[2] = b1.x; xc[3] = b1.y;
+          xc[4] = b2.x; xc[5] = b2.y; xc[6] = b3.x; xc[7] = b3.y;
+        }
 #pragma unroll
         for (int o = 0; o < 4; ++o) {
           const float* wo = wt + (long long)o * 9 * C + c;
@@ -485,7 +491,7 @@ __global__ void out_cfg_ddim_kernel(const ea_half* __restrict__ xn, const float*
 #pragma unroll
           for (int j = 0; j < 8; ++j) {
             au[o] += wv[j] * xu[j];
-            ac[o] += wv[j] * xc[j];
+            if constexpr (kCfg) ac[o] += wv[j] * xc[j];
           }
         }
       }
@@ -494,18 +500,20 @@ __global__ void out_cfg_ddim_kernel(const ea_half* __restrict__ xn, const float*
 #pragma unroll
   for (int o = 0; o < 4; ++o) {
     au[o] = warp_sum(au[o]);
-    ac[o] = warp_sum(ac[o]);
+    if constexpr (kCfg) ac[o] = warp_sum(ac[o]);
   }
   if (lane < 4) {
     const int o = lane;
     float eu = (o == 0 ? au[0] : o == 1 ? au[1] : o == 2 ? au[2] : au[3]) + bias[o];
-    float ec = (o == 0 ? ac[0] : o == 1 ? ac[1] : o == 2 ? ac[2] : ac[3]) + bias[o];
+    float ec = 0.f;
+    if constexpr (kCfg) ec = (o == 0 ? ac[0] : o == 1 ? ac[1] : o == 2 ? ac[2] : ac[3]) + bias[o];
     if (eps_out) {
       eps_out[gw * 4 + o] = eu;
-      eps_out[(gw + npix) * 4 + o] = ec;
+      if constexpr (kCfg) eps_out[(gw + npix) * 4 + o] = ec;
     }
     if (latents) {
-      float e = eu + guidance * (ec - eu);  // cldm/ddim_hacked.py:192
+      // cldm/ddim_hacked.py:192; without guidance the network output itself (:187-188)
+      float e = kCfg ? eu + guidance * (ec - eu) : eu;
       float sa = coef[0], s1a = coef[1], sap = coef[2], s1ap = coef[3];
       float xt = latents[gw * 4 + o];
       float x0 = (xt - s1a * e) / sa;       // :215
@@ -539,7 +547,7 @@ __global__ void out_cfg_ddim_kernel(const ea_half* __restrict__ xn, const float*
       latents[gw * 4 + o] = xp;
       if (lat_half) {
         lat_half[gw * 4 + o] = ea_f2h(xp);
-        lat_half[(gw + npix) * 4 + o] = ea_f2h(xp);
+        if constexpr (kCfg) lat_half[(gw + npix) * 4 + o] = ea_f2h(xp);
       }
     }
   }
@@ -981,19 +989,36 @@ extern "C" int ea_timestep_embedding(const float* t, float* out, int B, int dim,
   return EA_LAUNCH_OK();
 }
 
+template <bool kCfg>
+static int launch_out_ddim(const void* xn, const float* w, const float* bias, float* latents, float* eps_out,
+                           const float* coef, float guidance, const float* known, const float* noise,
+                           const float* mask, void* lat_half_out, int* step_counter, float* hist, int Nimg, int H,
+                           int W, int C, void* stream) {
+  if (!xn || !w || !bias || (!latents && !eps_out)) return EA_ERR_ARG;
+  if (latents && !coef) return EA_ERR_ARG;
+  if ((known && !mask) || (noise && !known)) return EA_ERR_ARG;
+  if (C % 8 != 0 || Nimg < 1 || H < 1 || W < 1) return EA_ERR_SHAPE;
+  long long npix = (long long)Nimg * H * W;
+  const int wpc = 4;
+  ea_launch(out_ddim_kernel<kCfg>, dim3((unsigned)((npix + wpc - 1) / wpc)), dim3(wpc * 32), (size_t)(0), EA_STREAM(stream), reinterpret_cast<const ea_half*>(xn), w, bias, latents, eps_out, coef, guidance, known, noise, mask,
+      reinterpret_cast<ea_half*>(lat_half_out), step_counter, hist, Nimg, H, W, C);
+  return EA_LAUNCH_OK();
+}
+
 extern "C" int ea_out_cfg_ddim(const void* xn, const float* w, const float* bias, float* latents,
                                float* eps_out, const float* coef, float guidance,
                                const float* known, const float* noise, const float* mask, void* lat_half_out,
                                int* step_counter, float* hist, int Nimg, int H, int W, int C, void* stream) {
-  if (!xn || !w || !bias || (!latents && !eps_out)) return EA_ERR_ARG;
-  if (latents && !coef) return EA_ERR_ARG;
-  if ((known && !mask) || (noise && !known)) return EA_ERR_ARG;
-  if (C % 8 != 0) return EA_ERR_SHAPE;
-  long long npix = (long long)Nimg * H * W;
-  const int wpc = 4;
-  ea_launch(out_cfg_ddim_kernel, dim3((unsigned)((npix + wpc - 1) / wpc)), dim3(wpc * 32), (size_t)(0), EA_STREAM(stream), reinterpret_cast<const ea_half*>(xn), w, bias, latents, eps_out, coef, guidance, known, noise, mask,
-      reinterpret_cast<ea_half*>(lat_half_out), step_counter, hist, Nimg, H, W, C);
-  return EA_LAUNCH_OK();
+  return launch_out_ddim<true>(xn, w, bias, latents, eps_out, coef, guidance, known, noise, mask, lat_half_out,
+                               step_counter, hist, Nimg, H, W, C, stream);
+}
+
+extern "C" int ea_out_ddim(const void* xn, const float* w, const float* bias, float* latents, float* eps_out,
+                           const float* coef, const float* known, const float* noise, const float* mask,
+                           void* lat_half_out, int* step_counter, float* hist, int Nimg, int H, int W, int C,
+                           void* stream) {
+  return launch_out_ddim<false>(xn, w, bias, latents, eps_out, coef, 0.f, known, noise, mask, lat_half_out,
+                                step_counter, hist, Nimg, H, W, C, stream);
 }
 
 extern "C" int ea_step_gather(const int* step_counter, int n_rows, int n_tables, const float* const* src,

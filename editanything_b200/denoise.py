@@ -113,11 +113,20 @@ class DenoiseEngine:
         return out
 
     @engine_call
-    def prepare(self, ctx, hints, scales, guess_mode=False, cfg_duplicated=False):
+    def prepare(self, ctx, hints, scales, guess_mode=False, cfg_duplicated=False, guided=True):
         """ctx: [B, L, D] prompt embeddings ([negative; positive] stacked for CFG,
         utils/stable_diffusion_controlnet_inpaint.py:1339-1347); hints: list of NCHW conditioning
-        images [B, 3, 8h, 8w] (un-normalised, editany_lora.py:771-778,814-828); scales: list."""
+        images [B, 3, 8h, 8w] (un-normalised, editany_lora.py:771-778,814-828); scales: list.
+        guided=False: sampling without classifier-free guidance (guidance scale <= 1, :1329): ctx and hints hold
+        the N images once (B = N), every step runs the networks on those rows and feeds their eps to the update."""
+        if not guided and cfg_duplicated:
+            raise ValueError("cfg_duplicated describes [x; x] conditioning images, which only guided sampling has")
         ctx = ctx.to(self.dev)
+        if guided and ctx.shape[0] % 2:
+            raise ValueError(f"guided sampling stacks [negative; positive] prompt embeddings, got {ctx.shape[0]} rows")
+        if guided != getattr(self, "guided", None):
+            self._graph = None        # the step's last launch differs (ea_out_cfg_ddim / ea_out_ddim)
+        self.guided = bool(guided)
         self.B = ctx.shape[0]
         nets = [self.unet] + self.cns
         # lockstep (nets.UNetRunner): the encoder-side K/V of all networks live stacked in ctx_ls; only the UNet
@@ -181,7 +190,8 @@ class DenoiseEngine:
         """The per-request input of a 9-channel (inpainting) UNet: the mask resized to the latents [N, 1, h, w] and
         the VAE latents of the masked image [N, 4, h, w] (utils/...inpaint.py:1448-1468), for the N images.  They
         are the same at every step (:1550-1558), so their part of conv_in, bias included, is computed here once;
-        the CFG duplication is done here too.  Each step's conv_in then reads the 4 latent channels only."""
+        the CFG duplication is done here too (guided requests only).  Each step's conv_in then reads the 4 latent
+        channels only."""
         if self.unet.x_channels == self.cfg.in_channels:
             raise ValueError(f"set_unet_condition needs a 9-channel UNet, this one takes {self.cfg.in_channels}")
         if mask_n1hw.shape[1] != 1 or masked_latents_nchw.shape[1] != 4 or \
@@ -189,7 +199,7 @@ class DenoiseEngine:
             raise ValueError(f"mask {tuple(mask_n1hw.shape)} / masked-image latents {tuple(masked_latents_nchw.shape)}: "
                              "expected [N, 1, h, w] and [N, 4, h, w]")
         g = self._condition(mask_n1hw, masked_latents_nchw)
-        self._keep("cond_in", torch.cat([g, g]))
+        self._keep("cond_in", torch.cat([g, g]) if self.guided else g)
 
     # -- the sampling schedule as device tables -------------------------------------------------
     @engine_call
@@ -248,8 +258,11 @@ class DenoiseEngine:
         xn = self.runner.eps_features(xh, self.t_dev, self.ctx_cache, self.hints, self.scales, self.gn_ws,
                                       embs=self.emb_bufs, ctx_ls=self.ctx_ls, cond_in=cond)
         eps = torch.empty(B, H, W_, 4, device=self.dev, dtype=torch.float32)
-        self.ops.out_cfg_ddim(xn, self.unet.w["out.w"], self.unet.w["out.cb"], eps_out=eps, Nimg=B // 2, H=H,
-                              W=W_, C_=self.cfg.model_channels)
+        w, cb, mc = self.unet.w["out.w"], self.unet.w["out.cb"], self.cfg.model_channels
+        if self.guided and B % 2 == 0:    # the two guidance halves, as the guided step reduces them
+            self.ops.out_cfg_ddim(xn, w, cb, eps_out=eps, Nimg=B // 2, H=H, W=W_, C_=mc)
+        else:
+            self.ops.out_ddim(xn, w, cb, eps_out=eps, Nimg=B, H=H, W=W_, C_=mc)
         return eps.permute(0, 3, 1, 2).contiguous()
 
     # -- production API: one fused denoising step ----------------------------------------------
@@ -259,10 +272,14 @@ class DenoiseEngine:
                              [self.coef_dev] + self.emb_bufs)
         xn = self.runner.eps_features(self.x_half, self.t_dev, self.ctx_cache, self.hints, self.scales, self.gn_ws,
                                       embs=self.emb_bufs, ctx_ls=self.ctx_ls, cond_in=self._step_cond())
-        self.ops.out_cfg_ddim(xn, self.unet.w["out.w"], self.unet.w["out.cb"], latents=self.lat,
-                              coef=self.coef_dev, guidance=self.guidance, known=self.known, noise=self.noise,
-                              mask=self.mask, lat_half_out=self.x_half, step_counter=self.step_ctr, hist=self.hist,
-                              Nimg=self.B // 2, H=H, W=W_, C_=self.cfg.model_channels)
+        kw = dict(latents=self.lat, coef=self.coef_dev, known=self.known, noise=self.noise, mask=self.mask,
+                  lat_half_out=self.x_half, step_counter=self.step_ctr, hist=self.hist, H=H, W=W_,
+                  C_=self.cfg.model_channels)
+        if self.guided:
+            self.ops.out_cfg_ddim(xn, self.unet.w["out.w"], self.unet.w["out.cb"], guidance=self.guidance,
+                                  Nimg=self.B // 2, **kw)
+        else:
+            self.ops.out_ddim(xn, self.unet.w["out.w"], self.unet.w["out.cb"], Nimg=self.B, **kw)
 
     def _step_cond(self):
         if self.unet.x_channels == self.cfg.in_channels:
@@ -273,18 +290,24 @@ class DenoiseEngine:
 
     @engine_call
     def begin(self, latents_nchw, guidance, known_nchw=None, mask_n1hw=None, noise_nchw=None, use_graph=True):
-        """latents: fp32 [N, 4, h, w] initial noise (N = B/2 images).  known/mask: optional inpaint blend
-        tensors (mask == 1 keeps `known`, utils/...inpaint.py:1484-1489,1647-1664); noise: the initial latent
-        noise the kept region is re-noised with (:1446,1650).  The blend buffers always exist (an all-zero mask
-        is an exact no-op), so switching the blend on, off or ending its window never re-captures the graph."""
+        """latents: fp32 [N, 4, h, w] initial noise (N = B/2 images, or B without guidance; `guidance` is then
+        unused).  known/mask: optional inpaint blend tensors (mask == 1 keeps `known`,
+        utils/...inpaint.py:1484-1489,1647-1664); noise: the initial latent noise the kept region is re-noised with
+        (:1446,1650).  The blend buffers always exist (an all-zero mask is an exact no-op), so switching the blend on,
+        off or ending its window never re-captures the graph."""
         def nhwc(t):
             return t.to(self.dev, torch.float32).permute(0, 2, 3, 1).contiguous()
         lat = nhwc(latents_nchw)
+        copies = 2 if self.guided else 1
+        if copies * lat.shape[0] != self.B:
+            raise ValueError(f"{lat.shape[0]} latents for a request prepared with {self.B} network rows "
+                             f"({'guided' if self.guided else 'unguided'})")
         self._keep("lat", lat)
-        self._keep("x_half", torch.cat([lat, lat]).to(self.hdt).contiguous())
-        if getattr(self, "guidance", None) != float(guidance):
+        self._keep("x_half", torch.cat([lat] * copies).to(self.hdt).contiguous())
+        g = float(guidance) if self.guided else None
+        if getattr(self, "guidance", None) != g:
             self._graph = None
-        self.guidance = float(guidance)
+        self.guidance = g
         # (each buffer gets its OWN zeros: _keep adopts the tensor it is given on first use, and known / noise / mask
         # must never alias)
         self._keep("known", nhwc(known_nchw) if known_nchw is not None else torch.zeros_like(lat))
@@ -313,7 +336,7 @@ class DenoiseEngine:
         (utils/...inpaint.py:1647-1656) - for callers that must observe the un-blended latents first."""
         m = self.mask[..., None]
         self.lat.copy_((k_init * self.known + k_noise * self.noise) * m + self.lat * (1 - m))
-        self.x_half.copy_(torch.cat([self.lat, self.lat]).to(self.hdt))
+        self.x_half.copy_(torch.cat([self.lat] * (2 if self.guided else 1)).to(self.hdt))
 
     @engine_call
     def set_known(self, known_nchw):

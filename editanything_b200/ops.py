@@ -293,12 +293,47 @@ def timestep_embedding(t, out, *, B, dim):
     return out
 
 
+def check_out_buffers(what, copies, xn, w, bias, latents, eps_out, coef, known, noise, mask, lat_half_out,
+                      step_counter, hist, Nimg, H, W, C_):
+    """The element count of every buffer of ea_out_cfg_ddim (copies = 2: the network rows are the two guidance
+    halves) or ea_out_ddim (copies = 1), checked before the launch: the kernels index them from (Nimg, H, W, C_)
+    alone, so a buffer sized for the other entry point would be read or written out of bounds."""
+    if min(Nimg, H, W, C_) < 1:
+        raise ValueError(f"{what}: Nimg, H, W, C must be positive, got {(Nimg, H, W, C_)}")
+    px = Nimg * H * W
+    want = {"xn": (xn, copies * px * C_), "w": (w, 36 * C_), "bias": (bias, 4), "latents": (latents, px * 4),
+            "eps_out": (eps_out, copies * px * 4), "known": (known, px * 4),
+            "noise": (noise, px * 4), "mask": (mask, px), "lat_half_out": (lat_half_out, copies * px * 4),
+            "step_counter": (step_counter, 1), "hist": (hist, 3 * px * 4)}
+    for name, (t, n) in want.items():
+        if t is not None and t.numel() != n:
+            raise ValueError(f"{what}: {name} has {t.numel()} elements, Nimg={Nimg}, H={H}, W={W}, C={C_} needs {n}")
+    # coef: the DDIM terms always, the blend terms with noise, the multistep row with hist
+    n_coef = 16 if hist is not None else 7 if noise is not None else 4
+    if latents is not None and (coef is None or coef.numel() < n_coef):
+        raise ValueError(f"{what}: coef needs at least {n_coef} elements, has {None if coef is None else coef.numel()}")
+
+
 def out_cfg_ddim(xn, w, bias, *, latents=None, eps_out=None, coef=None, guidance=1.0, known=None, noise=None,
                  mask=None, lat_half_out=None, step_counter=None, hist=None, Nimg, H, W, C_):
+    check_out_buffers("out_cfg_ddim", 2, xn, w, bias, latents, eps_out, coef, known, noise, mask, lat_half_out,
+                      step_counter, hist, Nimg, H, W, C_)
     lib = L.lib()
     L.check(lib.ea_out_cfg_ddim(_p(xn), _p(w), _p(bias), _p(latents), _p(eps_out), _p(coef),
                                 float(guidance), _p(known), _p(noise), _p(mask), _p(lat_half_out),
                                 _p(step_counter), _p(hist), Nimg, H, W, C_, _stream()), "ea_out_cfg_ddim")
+
+
+def out_ddim(xn, w, bias, *, latents=None, eps_out=None, coef=None, known=None, noise=None, mask=None,
+             lat_half_out=None, step_counter=None, hist=None, Nimg, H, W, C_):
+    """ea_out_ddim: the out conv and update of out_cfg_ddim without guidance; every buffer holds the Nimg images
+    once."""
+    check_out_buffers("out_ddim", 1, xn, w, bias, latents, eps_out, coef, known, noise, mask, lat_half_out,
+                      step_counter, hist, Nimg, H, W, C_)
+    lib = L.lib()
+    L.check(lib.ea_out_ddim(_p(xn), _p(w), _p(bias), _p(latents), _p(eps_out), _p(coef), _p(known), _p(noise),
+                            _p(mask), _p(lat_half_out), _p(step_counter), _p(hist), Nimg, H, W, C_, _stream()),
+            "ea_out_ddim")
 
 
 def step_gather(step_counter, n_rows, tables, dsts):

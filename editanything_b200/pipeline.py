@@ -15,6 +15,11 @@ stabilityai/stable-diffusion-2-inpainting: the UNet also reads the mask and the 
 ControlNets read the 4 latent channels, and there is no blend, so `alignment_ratio` is ignored, :1448-1468,
 :1550-1560, :1647-1664).
 
+Classifier-free guidance follows the reference too (`do_classifier_free_guidance = guidance_scale > 1.0`, :1329): a
+guided request runs the networks on 2N rows ([negative; positive] prompts, doubled conditioning images and latents) and
+combines the two halves in the step's last kernel; with guidance_scale <= 1 only the positive prompt is encoded, the
+networks run on the N images alone and their output drives the scheduler directly, so the scale has no further effect.
+
 Not supported (raises NotImplementedError rather than silently diverging): the reference-only mode
 (`ref_image`, `utils/stable_diffusion_reference.py`), guess_mode.
 """
@@ -456,9 +461,8 @@ class StableDiffusionControlNetInpaintPipeline:
         else:
             batch_size = prompt_embeds.shape[0]
         N = batch_size * num_images_per_prompt
+        # :1329; without guidance the networks run on the N images alone and guidance_scale has no effect
         do_cfg = guidance_scale > 1.0
-        if not do_cfg:
-            raise NotImplementedError("guidance_scale <= 1 (no classifier-free guidance) is not fused")
         n_nets = len(self.controlnet.nets)
         if isinstance(controlnet_conditioning_scale, float):
             controlnet_conditioning_scale = [controlnet_conditioning_scale] * n_nets
@@ -502,7 +506,8 @@ class StableDiffusionControlNetInpaintPipeline:
             if m.shape[0] < N:
                 m = m.repeat(N // m.shape[0], 1, 1, 1)
 
-        eng.prepare(prompt_embeds, conds, controlnet_conditioning_scale, guess_mode=guess_mode, cfg_duplicated=do_cfg)
+        eng.prepare(prompt_embeds, conds, controlnet_conditioning_scale, guess_mode=guess_mode, cfg_duplicated=do_cfg,
+                    guided=do_cfg)
         # fused step: the built-in DDIM, and UniPC (what every reference entry point installs, editany_lora.py:383,418)
         # through its per-step coefficient rows; any other scheduler object runs eng.eps + scheduler.step
         unipc = isinstance(self.scheduler, UniPCMultistepScheduler) and self.scheduler.config.solver_order <= 2
@@ -545,14 +550,15 @@ class StableDiffusionControlNetInpaintPipeline:
                     eng.blend_now(k_next[i][0], k_next[i][1])
             lat = eng.latents()
         else:
+            copies = 2 if do_cfg else 1
             if inpaint_unet:
-                cond = torch.cat([torch.cat([mask_lat] * 2), torch.cat([masked_lat] * 2)], 1)
+                cond = torch.cat([torch.cat([mask_lat] * copies), torch.cat([masked_lat] * copies)], 1)
             for i, t in enumerate(timesteps):
-                x_in = self.scheduler.scale_model_input(torch.cat([lat] * 2), t)
+                x_in = self.scheduler.scale_model_input(torch.cat([lat] * copies), t)
                 if inpaint_unet:
                     x_in = torch.cat([x_in, cond], 1)                                  # :1550-1558
                 eps = eng.eps(x_in, float(t))
-                e = eps[:N] + guidance_scale * (eps[N:] - eps[:N])
+                e = eps[:N] + guidance_scale * (eps[N:] - eps[:N]) if do_cfg else eps   # :1627-1631
                 lat = self.scheduler.step(e, t, lat).prev_sample
                 if callback is not None and i % callback_steps == 0:
                     callback(i, t, lat)

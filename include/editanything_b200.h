@@ -259,6 +259,15 @@ int ea_out_cfg_ddim(const void* xn, const float* w, const float* bias, float* la
                     float* eps_out, const float* coef, float guidance, const float* known,
                     const float* noise, const float* mask, void* lat_half_out, int* step_counter,
                     float* hist, int Nimg, int H, int W, int C, void* stream);
+/* ea_out_ddim: ea_out_cfg_ddim without classifier-free guidance - the sampler's single network evaluation when
+ * the guidance scale is <= 1 (utils/stable_diffusion_controlnet_inpaint.py:1329,1541-1544,1627-1631 skipped;
+ * cldm/ddim_hacked.py:187-188): the update reads eps itself.  Same coef modes, history, blend and step counter as
+ * ea_out_cfg_ddim, but every buffer holds the Nimg images once: xn NHWC half [Nimg, H, W, C], eps_out (optional)
+ * fp32 [Nimg, H, W, 4], lat_half_out (optional) half [Nimg, H, W, 4]; latents / known / noise / mask / hist as above.
+ * Nimg may be any count >= 1 (with latents == NULL: the eps of any batch). */
+int ea_out_ddim(const void* xn, const float* w, const float* bias, float* latents, float* eps_out,
+                const float* coef, const float* known, const float* noise, const float* mask,
+                void* lat_half_out, int* step_counter, float* hist, int Nimg, int H, int W, int C, void* stream);
 
 /* ---- ea_step_gather: first kernel of a captured denoising step ---------------------------------
  * The loop of utils/stable_diffusion_controlnet_inpaint.py:1540-1656 changes only scalars from step to step
