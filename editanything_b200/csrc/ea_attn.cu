@@ -405,6 +405,8 @@ extern "C" int ea_attention(const ea_attn_args* a, void* stream_) {
   if (!(a->scale > 0.f) || isinf(a->scale)) return EA_ERR_ARG;   // the kernel scales the row max, not every logit
   if ((a->rel_h != nullptr) != (a->rel_w != nullptr)) return EA_ERR_ARG;
   if (a->rel_h && a->rel_s <= 0) return EA_ERR_ARG;
+  // bias[q, kk] is defined for kk < rel_s^2 only (the kernel clamps kk / rel_s, which masked keys need)
+  if (a->rel_h && (long long)a->rel_s * a->rel_s < a->Nkv) return EA_ERR_SHAPE;
 
   AttnKParams p;
   memset(&p, 0, sizeof(p));
@@ -419,11 +421,13 @@ extern "C" int ea_attention(const ea_attn_args* a, void* stream_) {
   const bool bias = a->rel_h != nullptr;
   const int dv = attn_pv_width(a->d);
   const int budget = 227 * 1024 - 1024 - 256;
-  const int bias_bytes = bias ? ((AT_BQ * (a->rel_s + 1) + 3) & ~3) * 4 : 0;
+  // 64-bit: rel_w rows of a huge rel_s must not wrap around and pass as a small shared-memory footprint
+  const long long bias_ll = bias ? ((AT_BQ * ((long long)a->rel_s + 1) + 3) & ~3LL) * 4 : 0;
   const int stage_bytes = p.nd * AT_ATOM + dv / 16 * AT_VBOX;
-  int stages = (budget - p.nd * AT_ATOM - bias_bytes) / stage_bytes;
-  if (stages > AT_MAX_STAGES) stages = AT_MAX_STAGES;
-  if (stages < 1) return EA_ERR_SHAPE;
+  const long long stages_ll = (budget - p.nd * AT_ATOM - bias_ll) / stage_bytes;
+  if (stages_ll < 1) return EA_ERR_SHAPE;
+  const int bias_bytes = (int)bias_ll;
+  int stages = stages_ll > AT_MAX_STAGES ? AT_MAX_STAGES : (int)stages_ll;
   const int n_tiles = (a->Nkv + AT_BKV - 1) / AT_BKV;
   if (stages > n_tiles) stages = n_tiles;
   p.stages = stages;

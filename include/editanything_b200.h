@@ -163,7 +163,8 @@ int ea_gemm_plan(int m_tiles, int N, int k_blocks, int act, long long workspace_
  * q: [B, Nq, heads, d] with strides (q_bs, q_ns, d) elements; k, v likewise with Nkv rows;
  * out: [B, Nq, heads*d] contiguous rows of stride o_ns.  d % 8 == 0, d <= 192.  scale > 0 (finite).
  * rel_h / rel_w (optional, fp32 [B*heads, Nq, rel_s]): bias[q, kk] = rel_h[q, kk / rel_s] +
- * rel_w[q, kk % rel_s] added to the scaled logits (SAM add_decomposed_rel_pos).
+ * rel_w[q, kk % rel_s] added to the scaled logits (SAM add_decomposed_rel_pos).  With them, Nkv <= rel_s * rel_s
+ * (else EA_ERR_SHAPE), and 128 rows of rel_w must fit in shared memory next to the K / V tiles.
  */
 typedef struct ea_attn_args {
   const void* q; const void* k; const void* v; void* out;
