@@ -29,7 +29,7 @@ class GemmArgs(C.Structure):
         ("out2", C.c_void_p), ("ldo2", C.c_longlong),
         ("out_f32", C.c_void_p),
         ("act", C.c_int), ("out_scale", C.c_float), ("accumulate", C.c_int),
-        ("force_bn", C.c_int), ("force_stages", C.c_int), ("force_splits", C.c_int), ("force_2cta", C.c_int), ("no_spin", C.c_int),
+        ("force_bn", C.c_int), ("force_splits", C.c_int), ("force_2cta", C.c_int), ("no_spin", C.c_int),
         ("force_persistent", C.c_int),
         ("rowstats_out", C.c_void_p), ("ln_stats", C.c_void_p), ("ln_g", C.c_void_p), ("ln_parts", C.c_int),
         ("ln_eps", C.c_float), ("row_scale", C.c_void_p),

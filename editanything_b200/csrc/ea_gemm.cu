@@ -38,10 +38,8 @@ static constexpr int BM = 128;
 static constexpr int BK = 64;
 // Warp roles: consumer warps 0-7 (warp-groups 0-1), producer warp-group 2 (warps 8-11).  A CTA is launched with
 // 384 x 168 registers (__launch_bounds__(384, 1)); setmaxnreg then re-divides exactly that pool: 224 per consumer
-// thread, which holds the RP = 2 accumulator at BN = 128 (2 x 64 per thread) and the RP = 1 one at BN = 256 (128)
-// without spills, and 56 per producer thread (the grouped two-sub-tile convolution producer spills at 40).  The
-// planner never picks BN = 256 (a forced width only, ea_gemm_args.force_bn): the GEGLU weight interleave and the
-// planner's contract keep BN <= 128.
+// thread, which holds the RP = 2 accumulator at BN = 128 (2 x 64 per thread) without spills, and 56 per producer
+// thread (the grouped two-sub-tile convolution producer spills at 40).
 static constexpr int GEMM_THREADS = 384;
 static constexpr int W_TMA = 8;
 static constexpr int EPI_WARPS = 8, EPI_THREADS = 256;
@@ -61,8 +59,7 @@ __host__ __device__ constexpr int gemm_region_bytes(int bn, int stages, int rp) 
                                                                     : gemm_epi_bytes(bn, rp);
 }
 static_assert(4 * gemm_stage_bytes(128, 2) <= GEMM_SMEM_RING, "RP = 2, BN = 128: four 48 KB stages fill the ring");
-static_assert(gemm_epi_bytes(128, 2) <= GEMM_SMEM_RING && gemm_epi_bytes(256, 1) <= GEMM_SMEM_RING,
-              "the staged accumulators and the store staging fit the ring");
+static_assert(gemm_epi_bytes(128, 2) <= GEMM_SMEM_RING, "the staged accumulators and the store staging fit the ring");
 // per-column epilogue vectors: [2 item parities][RP sub-tiles][2][256] fp32
 __host__ __device__ constexpr int gemm_cb_bytes(int rp) { return 2 * rp * 2 * 256 * 4; }
 
@@ -553,7 +550,6 @@ template <int BN, int NG, int RP>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 ea_gemm_kernel(const __grid_constant__ GemmLaunch<NG> L, const int tiles_per_group, const int m_items,
                const int n_groups) {
-  static_assert(RP == 1 || (RP == 2 && BN <= 128), "two row tiles per CTA need BN <= 128 (registers)");
   const GemmKParams& p0 = L.g[0].p;
   const int n_tiles = (p0.N + BN - 1) / BN;
   const int mn_items = m_items * n_tiles;
@@ -1058,7 +1054,7 @@ ea_gemm_kernel(const __grid_constant__ GemmLaunch<NG> L, const int tiles_per_gro
 // partial tiles are combined in-kernel (see the epilogue).  Two row tiles per CTA (rp = 2) share each W box: per
 // K-block the A bytes and the MMA time double, the W bytes do not, and the fixed costs are paid once per pair.  They
 // are never combined with split-K, which exists because there are fewer tiles than SMs.
-struct GemmPlan { int BN, stages, splits, kbps, occ, rp; double cost; };
+struct GemmPlan { int BN, stages, splits, kbps, rp; double cost; };
 
 // Per-SM and chip rates in bytes per SM clock, from the H100 SXM data sheet (3.35 TB/s HBM3; fp16 wgmma at
 // 989 TFLOP/s over 132 SMs = 2048 MAC / clk / SM, so a 128 x BN x 64 K-block takes 4 BN clk) and L2 at about 1.6x
@@ -1076,7 +1072,7 @@ static constexpr int GEMM_BN[3] = {128, 64, 32};   // the tile widths the planne
 static GemmPlan plan_gemm(int mt, int N, int nkb, int act, long long ws_floats, int n_sm, bool has_res = false,
                           int groups = 1, int force_rp = 0) {
   const double epi_col = (PL_EPI + (has_res ? PL_EPI_RES : 0.0)) * (act == EA_ACT_GEGLU ? 0.84 : 1.0);
-  GemmPlan best = {0, 0, 1, nkb, 1, 1, 1e30};
+  GemmPlan best = {0, 0, 1, nkb, 1, 1e30};
   for (int rp = 1; rp <= 2; ++rp) {
     if (force_rp > 0 && rp != force_rp) continue;
     if (force_rp == 0 && rp == 2 && mt < 2) continue;
@@ -1129,7 +1125,7 @@ static GemmPlan plan_gemm(int mt, int N, int nkb, int act, long long ws_floats, 
           cost = (double)waves * (PL_START + kbps * t_kb + PL_SPLIT_COL * BN) + PL_SPLIT_FIX +
                  3.0 * (BM * BN * 4.0) / 25.0 + 150.0 * splits;
         }
-        if (cost < best.cost) best = {BN, st, splits, kbps, 1, rp, cost};
+        if (cost < best.cost) best = {BN, st, splits, kbps, rp, cost};
       }
     }
   }
@@ -1148,7 +1144,7 @@ extern "C" int ea_gemm_plan(int m_tiles, int N, int k_blocks, int act, long long
   const long long ws_floats = workspace_bytes > 65536 ? (workspace_bytes - 65536) / 4 : 0;
   GemmPlan pl = plan_gemm(m_tiles, N, k_blocks, act, ws_floats, n_sm > 0 ? n_sm : 132);
   out5[0] = pl.BN; out5[1] = pl.stages; out5[2] = pl.splits; out5[3] = pl.kbps;
-  out5[4] = pl.occ;   // tens digit (CTA pairs) is always 0 on this architecture
+  out5[4] = 1;   // CTAs per SM
   return pl.BN ? EA_OK : EA_ERR_SHAPE;
 }
 
@@ -1282,8 +1278,8 @@ static bool gemm_same_problem(const ea_gemm_args* a, const ea_gemm_args* b) {
          (!a->row_scale) == (!b->row_scale) &&
          (!a->rowvec) == (!b->rowvec) && a->rows_per_batch == b->rows_per_batch &&
          (!a->rowstats_out) == (!b->rowstats_out) && (!a->ln_stats) == (!b->ln_stats) && a->ln_parts == b->ln_parts &&
-         a->force_bn == b->force_bn && a->force_stages == b->force_stages && a->force_splits == b->force_splits &&
-         a->force_2cta == b->force_2cta && a->no_spin == b->no_spin && a->force_persistent == b->force_persistent;
+         a->force_bn == b->force_bn && a->force_splits == b->force_splits && a->force_2cta == b->force_2cta &&
+         a->no_spin == b->no_spin && a->force_persistent == b->force_persistent;
 }
 
 template <typename K>
@@ -1312,14 +1308,15 @@ static cudaError_t launch_gemm_bn(int BN, int rp, const GemmLaunch<NG>& L, int g
     switch (BN) {
       case 32: return launch_gemm<32, NG, 2>(L, grid, smem_bytes, tiles_per_group, m_items, n_groups, stream, rc);
       case 64: return launch_gemm<64, NG, 2>(L, grid, smem_bytes, tiles_per_group, m_items, n_groups, stream, rc);
-      default: return launch_gemm<128, NG, 2>(L, grid, smem_bytes, tiles_per_group, m_items, n_groups, stream, rc);
+      case 128: return launch_gemm<128, NG, 2>(L, grid, smem_bytes, tiles_per_group, m_items, n_groups, stream, rc);
+      default: return cudaErrorInvalidValue;   // ea_gemm_grouped admits 32 / 64 / 128 only
     }
   }
   switch (BN) {
     case 32: return launch_gemm<32, NG, 1>(L, grid, smem_bytes, tiles_per_group, m_items, n_groups, stream, rc);
     case 64: return launch_gemm<64, NG, 1>(L, grid, smem_bytes, tiles_per_group, m_items, n_groups, stream, rc);
     case 128: return launch_gemm<128, NG, 1>(L, grid, smem_bytes, tiles_per_group, m_items, n_groups, stream, rc);
-    default: return launch_gemm<256, NG, 1>(L, grid, smem_bytes, tiles_per_group, m_items, n_groups, stream, rc);
+    default: return cudaErrorInvalidValue;
   }
 }
 
@@ -1349,18 +1346,15 @@ extern "C" int ea_gemm_grouped(const ea_gemm_args* args, int n_groups, void* str
   const int force_rp = a->force_2cta > 0 ? 2 : a->force_2cta < 0 ? 1 : 0;
   GemmPlan plan =
       plan_gemm(m_tiles, a->N, nkb, a->act, persist ? 0 : ws_floats, sm_count(), has_res, G, force_rp);
-  if (a->force_bn > 256 - 128 * (plan.rp - 1)) {   // BN = 256 has one row tile per CTA (registers)
-    if (force_rp == 2) return EA_ERR_SHAPE;
-    plan.rp = 1;
-  }
-  if (a->force_bn > 0 || a->force_stages > 0 || a->force_splits > 0) {
-    if (a->force_bn > 0) plan.BN = a->force_bn;
+  if (a->force_bn > 0) plan.BN = a->force_bn;
+  if (plan.BN != 32 && plan.BN != 64 && plan.BN != 128) return EA_ERR_SHAPE;
+  if (a->force_bn > 0 || a->force_splits > 0) {
     const int sb = gemm_stage_bytes(plan.BN, plan.rp);
-    if (a->force_bn > 0) plan.stages = plan.BN <= 128 ? 3 : 4;
-    if (a->force_stages > 0) plan.stages = a->force_stages;
+    if (a->force_bn > 0) plan.stages = 3;
     if (plan.stages * sb > GEMM_SMEM_RING) plan.stages = GEMM_SMEM_RING / sb;
     if (plan.stages > nkb) plan.stages = nkb < 2 ? 2 : nkb;
-    if (a->force_bn > 0 || a->force_splits > 0) { plan.splits = 1; plan.kbps = nkb; }
+    plan.splits = 1;
+    plan.kbps = nkb;
     if (a->force_splits > 1 && !persist) {
       plan.kbps = (nkb + a->force_splits - 1) / a->force_splits;
       plan.splits = (nkb + plan.kbps - 1) / plan.kbps;
@@ -1368,7 +1362,6 @@ extern "C" int ea_gemm_grouped(const ea_gemm_args* args, int n_groups, void* str
   }
   if (ln_any && plan.splits > 1) return EA_ERR_ARG;
   const int BN = plan.BN, RP = plan.rp;
-  if (BN != 32 && BN != 64 && BN != 128 && BN != 256) return EA_ERR_SHAPE;
   if (a->act == EA_ACT_GEGLU && (a->N % 128 != 0 || BN != 128)) return EA_ERR_SHAPE;
   const int n_tiles = (a->N + BN - 1) / BN;
   const int m_items = (m_tiles + RP - 1) / RP;

@@ -32,35 +32,19 @@ int ea_pdl_enabled();
 #ifdef __CUDACC__
 #include <utility>
 template <typename... KArgs, typename... Args>
-static inline cudaError_t ea_launch_cluster(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem,
-                                            cudaStream_t stream, unsigned cluster_x, Args&&... args) {
+static inline cudaError_t ea_launch(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem,
+                                    cudaStream_t stream, Args&&... args) {
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));
   cfg.gridDim = grid;
   cfg.blockDim = block;
   cfg.dynamicSmemBytes = smem;
   cfg.stream = stream;
-  cudaLaunchAttribute at[2];
-  int n = 0;
-  if (ea_pdl_enabled()) {
-    at[n].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    at[n].val.programmaticStreamSerializationAllowed = 1;
-    ++n;
-  }
-  if (cluster_x > 1) {
-    at[n].id = cudaLaunchAttributeClusterDimension;
-    at[n].val.clusterDim.x = cluster_x;
-    at[n].val.clusterDim.y = 1;
-    at[n].val.clusterDim.z = 1;
-    ++n;
-  }
-  cfg.attrs = at;
-  cfg.numAttrs = n;
+  cudaLaunchAttribute at;
+  at.id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  at.val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = &at;
+  cfg.numAttrs = ea_pdl_enabled() ? 1 : 0;
   return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(std::forward<Args>(args))...);
-}
-template <typename... KArgs, typename... Args>
-static inline cudaError_t ea_launch(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem,
-                                    cudaStream_t stream, Args&&... args) {
-  return ea_launch_cluster(kernel, grid, block, smem, stream, 1u, std::forward<Args>(args)...);
 }
 #endif

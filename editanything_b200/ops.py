@@ -60,7 +60,7 @@ def gemm_workspace(device):
 def _fill_gemm(g, a, w, out=None, *, mode=L.EA_GEMM_LINEAR, M=None, N=None, K=None, lda=None, ldw=0,
                conv=None, a_extra=None, bias=None, rowvec=None, rows_per_batch=0, residual=None,
                out2=None, out_f32=None, act=L.EA_ACT_NONE, out_scale=1.0, accumulate=False,
-               ldo=None, ldr=None, ldo2=None, ld_extra=0, force_bn=0, force_stages=0, force_splits=0, force_2cta=0,
+               ldo=None, ldr=None, ldo2=None, ld_extra=0, force_bn=0, force_splits=0, force_2cta=0,
                force_persistent=0, rowstats_out=None, ln=None, row_scale=None):
     """Fills one ea_gemm_args; returns the output tensor (allocated when the caller gave none)."""
     g.mode = mode
@@ -106,7 +106,6 @@ def _fill_gemm(g, a, w, out=None, *, mode=L.EA_GEMM_LINEAR, M=None, N=None, K=No
     g.out_scale = out_scale
     g.accumulate = 1 if accumulate else 0
     g.force_bn = force_bn
-    g.force_stages = force_stages
     g.force_splits = force_splits
     g.force_2cta = force_2cta
     g.force_persistent = force_persistent

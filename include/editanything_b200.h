@@ -107,8 +107,7 @@ typedef struct ea_gemm_args {
   int act;
   float out_scale;           /* set 1.0f when unused */
   int accumulate;
-  int force_bn;              /* 0 = auto; else 32/64/128/256 (testing) */
-  int force_stages;          /* 0 = auto */
+  int force_bn;              /* 0 = auto; else 32/64/128 (testing); any other width is EA_ERR_SHAPE */
   int force_splits;          /* 0 = auto; 1 = never split K; n = split K n ways (testing) */
   int force_2cta;            /* row tiles per CTA: 1 = two vertically adjacent 128-row tiles sharing each W stage,
                                 -1 = one, 0 = the planner's choice (testing) */

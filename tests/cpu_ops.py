@@ -33,8 +33,7 @@ def _bump(n=1):
 def gemm(a, w, out=None, *, mode=0, M=None, N=None, K=None, lda=None, ldw=0, conv=None, a_extra=None,
          bias=None, rowvec=None, rows_per_batch=0, residual=None, out2=None, out_f32=None, act=0,
          out_scale=1.0, accumulate=False, ldo=None, ldr=None, ldo2=None, ld_extra=0, force_bn=0,
-         force_stages=0, force_splits=0, force_2cta=0, force_persistent=0, rowstats_out=None, ln=None,
-         row_scale=None):
+         force_splits=0, force_2cta=0, force_persistent=0, rowstats_out=None, ln=None, row_scale=None):
     if act == EA_ACT_GEGLU and (rowvec is not None or residual is not None or out2 is not None or out_f32 is not None
                                 or accumulate or out_scale != 1.0 or row_scale is not None):
         raise RuntimeError("ea_gemm failed (-1): GEGLU applies the bias and the LayerNorm fold only")

@@ -290,15 +290,18 @@ def test_split_k(M, N, K, splits, epi):
     _check_fp64(got, exp, mag, K, torch.float32 if f32 else dt)
 
 
-def test_bn256_takes_one_row_tile():
-    """BN = 256 keeps one row tile per CTA: forcing two is rejected, the planner's choice falls back to one."""
+def test_bn256_is_rejected():
+    """The tile widths are 32, 64 and 128: a forced width of 256 is refused with either number of row tiles per CTA,
+    and the same call at 128 meets its float64 bound."""
     dt = ops.half_dtype()
     g = torch.Generator(device=DEV).manual_seed(256)
     x = _rand(g, 1024, 256).to(dt)
     w = _rand(g, 512, 256, scale=1 / 16).to(dt)
     with pytest.raises(RuntimeError):
         ops.gemm(x, w, force_bn=256, force_2cta=1)
-    got = ops.gemm(x, w, force_bn=256)
+    with pytest.raises(RuntimeError):
+        ops.gemm(x, w, force_bn=256)
+    got = ops.gemm(x, w, force_bn=128)
     torch.cuda.synchronize()
     exp, _, mag = R.gemm_epilogue(x.double(), w.double())
     _check_fp64(got, exp, mag, 256, dt)

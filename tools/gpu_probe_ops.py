@@ -60,10 +60,6 @@ def case_gemm_bn128():
     return case_gemm_linear(force_bn=128)
 
 
-def case_gemm_bn256():
-    return case_gemm_linear(force_bn=256, M=512, N=512, K=1024)
-
-
 def case_gemm_big():
     return case_gemm_linear(M=8192, N=1280, K=2560)
 
