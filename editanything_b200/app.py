@@ -23,6 +23,17 @@ EditAnything ControlNets (sam2groundingdino_edit.py:36-44), e.g.
 
 whose tile pass loads runwayml/stable-diffusion-v1-5 separately (editany_lora.py:395-405).
 
+v-prediction base models run too: stabilityai/stable-diffusion-2-1 (768x768, the base of the reference's SD2.1
+entry points, sam2image.py:28, sketch2image.py:68) predicts v, which its scheduler_config.json records as
+`"prediction_type": "v_prediction"`; the loader carries that into the scheduler, the UniPC swap keeps it and the fused
+step converts v to x0 and eps.  An SD2.1 base has no tile ControlNet of its own, so pass one, e.g.
+
+    EditAnythingLoraModel(base_model_path="stabilityai/stable-diffusion-2-1",
+                          controlmodel_name="LAION Pretrained(v0-4)-SD21", extra_inpaint=False, use_blip=False,
+                          lora_model_path=None, tile_model=...)
+
+and call `process(..., enable_tile=False)`.
+
 LoRA: `lora_model_path` names a kohya `.safetensors` file merged at `lora_weight` into the UNet and the text
 encoder of the generation and the tile pipeline before their weights are packed (editany_lora.py:378-381, 413-416;
 editanything_b200.lora), e.g. the reference's "Beauty Edit" setup (editany_beauty.py:54-64)

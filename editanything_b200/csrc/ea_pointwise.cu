@@ -438,7 +438,9 @@ __global__ void timestep_embedding_kernel(const float* __restrict__ t, float* __
 // One warp per (image, pixel).  kCfg: xn, eps_out and lat_half hold 2*Nimg rows (unconditional first) and both
 // halves are reduced by the same warp, so the guidance combine and the DDIM update happen in registers.  !kCfg:
 // they hold the Nimg rows alone and the update reads their eps directly (sampling without guidance).
-template <bool kCfg>
+// kV: the network predicts v = sqrt(a) eps - sqrt(1-a) x0 (v-prediction base models such as SD2.1-768); the update
+// converts the (guidance-combined) output to x0 and eps first.  eps_out stays the raw network output either way.
+template <bool kCfg, bool kV>
 __global__ void out_ddim_kernel(const ea_half* __restrict__ xn, const float* __restrict__ w,
                                     const float* __restrict__ bias, float* __restrict__ latents,
                                     float* __restrict__ eps_out, const float* __restrict__ coef,
@@ -512,11 +514,19 @@ __global__ void out_ddim_kernel(const ea_half* __restrict__ xn, const float* __r
       if constexpr (kCfg) eps_out[(gw + npix) * 4 + o] = ec;
     }
     if (latents) {
-      // cldm/ddim_hacked.py:192; without guidance the network output itself (:187-188)
-      float e = kCfg ? eu + guidance * (ec - eu) : eu;
+      // cldm/ddim_hacked.py:192 (applied to v as well, :190-192); without guidance the network output itself
+      // (:187-188)
+      float m = kCfg ? eu + guidance * (ec - eu) : eu;
       float sa = coef[0], s1a = coef[1], sap = coef[2], s1ap = coef[3];
       float xt = latents[gw * 4 + o];
-      float x0 = (xt - s1a * e) / sa;       // :215
+      float x0, e;
+      if constexpr (kV) {
+        x0 = sa * xt - s1a * m;             // :217, ddpm.py:290-296 (predict_start_from_z_and_v)
+        e = sa * m + s1a * xt;              // :195, ddpm.py:298-302 (predict_eps_from_z_and_v)
+      } else {
+        e = m;
+        x0 = (xt - s1a * e) / sa;           // :215
+      }
       float xp = sap * x0 + s1ap * e;       // :226-230 (eta = 0)
       if (hist && coef[7] != 0.f) {
         // Linear multistep predictor-corrector (UniPC, the scheduler every reference entry point installs:
@@ -989,7 +999,7 @@ extern "C" int ea_timestep_embedding(const float* t, float* out, int B, int dim,
   return EA_LAUNCH_OK();
 }
 
-template <bool kCfg>
+template <bool kCfg, bool kV>
 static int launch_out_ddim(const void* xn, const float* w, const float* bias, float* latents, float* eps_out,
                            const float* coef, float guidance, const float* known, const float* noise,
                            const float* mask, void* lat_half_out, int* step_counter, float* hist, int Nimg, int H,
@@ -1000,7 +1010,7 @@ static int launch_out_ddim(const void* xn, const float* w, const float* bias, fl
   if (C % 8 != 0 || Nimg < 1 || H < 1 || W < 1) return EA_ERR_SHAPE;
   long long npix = (long long)Nimg * H * W;
   const int wpc = 4;
-  ea_launch(out_ddim_kernel<kCfg>, dim3((unsigned)((npix + wpc - 1) / wpc)), dim3(wpc * 32), (size_t)(0), EA_STREAM(stream), reinterpret_cast<const ea_half*>(xn), w, bias, latents, eps_out, coef, guidance, known, noise, mask,
+  ea_launch(out_ddim_kernel<kCfg, kV>, dim3((unsigned)((npix + wpc - 1) / wpc)), dim3(wpc * 32), (size_t)(0), EA_STREAM(stream), reinterpret_cast<const ea_half*>(xn), w, bias, latents, eps_out, coef, guidance, known, noise, mask,
       reinterpret_cast<ea_half*>(lat_half_out), step_counter, hist, Nimg, H, W, C);
   return EA_LAUNCH_OK();
 }
@@ -1009,16 +1019,32 @@ extern "C" int ea_out_cfg_ddim(const void* xn, const float* w, const float* bias
                                float* eps_out, const float* coef, float guidance,
                                const float* known, const float* noise, const float* mask, void* lat_half_out,
                                int* step_counter, float* hist, int Nimg, int H, int W, int C, void* stream) {
-  return launch_out_ddim<true>(xn, w, bias, latents, eps_out, coef, guidance, known, noise, mask, lat_half_out,
-                               step_counter, hist, Nimg, H, W, C, stream);
+  return launch_out_ddim<true, false>(xn, w, bias, latents, eps_out, coef, guidance, known, noise, mask,
+                                      lat_half_out, step_counter, hist, Nimg, H, W, C, stream);
 }
 
 extern "C" int ea_out_ddim(const void* xn, const float* w, const float* bias, float* latents, float* eps_out,
                            const float* coef, const float* known, const float* noise, const float* mask,
                            void* lat_half_out, int* step_counter, float* hist, int Nimg, int H, int W, int C,
                            void* stream) {
-  return launch_out_ddim<false>(xn, w, bias, latents, eps_out, coef, 0.f, known, noise, mask, lat_half_out,
-                                step_counter, hist, Nimg, H, W, C, stream);
+  return launch_out_ddim<false, false>(xn, w, bias, latents, eps_out, coef, 0.f, known, noise, mask, lat_half_out,
+                                       step_counter, hist, Nimg, H, W, C, stream);
+}
+
+extern "C" int ea_out_cfg_vpred(const void* xn, const float* w, const float* bias, float* latents,
+                                float* eps_out, const float* coef, float guidance,
+                                const float* known, const float* noise, const float* mask, void* lat_half_out,
+                                int* step_counter, float* hist, int Nimg, int H, int W, int C, void* stream) {
+  return launch_out_ddim<true, true>(xn, w, bias, latents, eps_out, coef, guidance, known, noise, mask,
+                                     lat_half_out, step_counter, hist, Nimg, H, W, C, stream);
+}
+
+extern "C" int ea_out_vpred(const void* xn, const float* w, const float* bias, float* latents, float* eps_out,
+                            const float* coef, const float* known, const float* noise, const float* mask,
+                            void* lat_half_out, int* step_counter, float* hist, int Nimg, int H, int W, int C,
+                            void* stream) {
+  return launch_out_ddim<false, true>(xn, w, bias, latents, eps_out, coef, 0.f, known, noise, mask, lat_half_out,
+                                      step_counter, hist, Nimg, H, W, C, stream);
 }
 
 extern "C" int ea_step_gather(const int* step_counter, int n_rows, int n_tables, const float* const* src,

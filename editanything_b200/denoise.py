@@ -13,6 +13,7 @@ import torch
 
 from ._backend import default_ops, engine_call
 from .nets import PackedNet, UNetRunner
+from .ops import PREDICTION_TYPES
 from .unet_spec import UNetConfig, controlnet_config
 
 
@@ -68,6 +69,7 @@ class DenoiseEngine:
         self.hdt = self.unet.hdt
         self._graph = None
         self.launches_per_step = None
+        self.prediction_type = "epsilon"
 
     def weight_bytes(self):
         return self.unet.weight_bytes() + sum(c.weight_bytes() for c in self.cns)
@@ -203,14 +205,21 @@ class DenoiseEngine:
 
     # -- the sampling schedule as device tables -------------------------------------------------
     @engine_call
-    def set_schedule(self, timesteps, alphas, alphas_prev, blend=None, multistep=None):
+    def set_schedule(self, timesteps, alphas, alphas_prev, blend=None, multistep=None, prediction_type="epsilon"):
         """Everything that changes from step to step of the loop (utils/...inpaint.py:1540-1656), as device
         tables with one row per step: the DDIM coefficients (cldm/ddim_hacked.py:203-231), the per-ResBlock
         time-embedding rows of every net, and the inpaint-blend terms.  `blend` = (k_init[S], k_noise[S],
         on[S]): the kept region of step i is k_init[i] * known + k_noise[i] * noise (add_noise at
         timesteps[i + 1], :1650-1652), applied where on[i] (i < len * alignment_ratio, :1648).  Without `blend`
         the kept region is `known` itself on every step.  The captured step indexes the tables with a device
-        counter (ea_step_gather), so the host issues ONE graph launch per step."""
+        counter (ea_step_gather), so the host issues ONE graph launch per step.
+        prediction_type: what the UNet predicts, "epsilon" or "v_prediction" (SD2.1-768; the update converts v to
+        x0 and eps, cldm/ddim_hacked.py:194-217) - the scheduler's `config.prediction_type`."""
+        if prediction_type not in PREDICTION_TYPES:
+            raise ValueError(f"prediction_type must be one of {PREDICTION_TYPES}, got {prediction_type!r}")
+        if prediction_type != self.prediction_type:
+            self._graph = None        # the step's last launch differs (ea_out_*ddim / ea_out_*vpred)
+        self.prediction_type = prediction_type
         ts = [float(t) for t in timesteps]
         S = len(ts)
         if blend is None:
@@ -243,7 +252,8 @@ class DenoiseEngine:
     @engine_call
     def eps(self, x_nchw, t):
         """eps = unet(x, t, ctx, control=sum_k scale_k * controlnet_k(x, hint_k, t, ctx)) as fp32
-        NCHW - the quantity the reference calls `noise_pred` before guidance.  For a 9-channel UNet x is
+        NCHW - the raw network output, the quantity the reference calls `noise_pred` before guidance: the noise for
+        an epsilon-prediction model, v for a v-prediction one (no conversion here).  For a 9-channel UNet x is
         cat([latents, mask, masked-image latents]) (utils/...inpaint.py:1550-1558) and the ControlNets see
         x[:, :4] (:1607-1615)."""
         B, C, H, W_ = x_nchw.shape
@@ -275,6 +285,8 @@ class DenoiseEngine:
         kw = dict(latents=self.lat, coef=self.coef_dev, known=self.known, noise=self.noise, mask=self.mask,
                   lat_half_out=self.x_half, step_counter=self.step_ctr, hist=self.hist, H=H, W=W_,
                   C_=self.cfg.model_channels)
+        if self.prediction_type != "epsilon":
+            kw["prediction"] = self.prediction_type     # epsilon is the operators' default
         if self.guided:
             self.ops.out_cfg_ddim(xn, self.unet.w["out.w"], self.unet.w["out.cb"], guidance=self.guidance,
                                   Nimg=self.B // 2, **kw)
@@ -346,9 +358,9 @@ class DenoiseEngine:
     def step(self, t=None, a_t=None, a_prev=None):
         """One fused step.  Without arguments: step number *step_ctr of the schedule given to set_schedule()
         (host work: one graph launch).  With (t, a_t, a_prev): a single DDIM (eta=0) step at timestep t
-        (cldm/ddim_hacked.py:181-231) - a one-row schedule."""
+        (cldm/ddim_hacked.py:181-231) - a one-row schedule, with the prediction type of the last set_schedule()."""
         if t is not None:
-            self.set_schedule([t], [a_t], [a_prev])
+            self.set_schedule([t], [a_t], [a_prev], prediction_type=self.prediction_type)
             self.step_ctr.zero_()
         elif self._sched_key is None:
             raise RuntimeError("set_schedule() first, or pass (t, a_t, a_prev)")

@@ -128,6 +128,13 @@ def load_pipeline_parts(base_model_path, device, *, text_encoder=None, tokenizer
     from .weights import diffusers_to_ldm, vae_diffusers_to_ldm
     root = resolve_model_path(base_model_path)
     ucfg = unet_config_from_diffusers(_read_json(os.path.join(root, "unet", "config.json")))
+    if scheduler is None:
+        # read before any weight: a prediction type the sampler cannot run ("sample", or anything unknown) raises
+        # here rather than when sampling.  SD2.1-768 sets "v_prediction".
+        sp = os.path.join(root, "scheduler", "scheduler_config.json")
+        sc = _read_json(sp) if os.path.exists(sp) else {}
+        scheduler = DDIMScheduler(sc.get("beta_start", 0.00085), sc.get("beta_end", 0.012),
+                                  sc.get("num_train_timesteps", 1000), sc.get("prediction_type", "epsilon"))
     usd = None
     if unet_packed is None:
         usd = load_weights(os.path.join(root, "unet"))
@@ -145,9 +152,4 @@ def load_pipeline_parts(base_model_path, device, *, text_encoder=None, tokenizer
     L.merge(lora, unet_sd=usd, text_encoder=text_encoder if merge_text_encoder else None)
     if usd is not None:
         usd = diffusers_to_ldm(usd, "unet", ucfg)
-    if scheduler is None:
-        sp = os.path.join(root, "scheduler", "scheduler_config.json")
-        sc = _read_json(sp) if os.path.exists(sp) else {}
-        scheduler = DDIMScheduler(sc.get("beta_start", 0.00085), sc.get("beta_end", 0.012),
-                                  sc.get("num_train_timesteps", 1000))
     return ucfg, usd, vae, text_encoder, tokenizer, scheduler

@@ -313,26 +313,41 @@ def check_out_buffers(what, copies, xn, w, bias, latents, eps_out, coef, known, 
         raise ValueError(f"{what}: coef needs at least {n_coef} elements, has {None if coef is None else coef.numel()}")
 
 
+PREDICTION_TYPES = ("epsilon", "v_prediction")
+
+
+def check_prediction(what, prediction):
+    """The network-output parameterisations the fused update implements: eps (SD1.5, SD2-inpainting) and v
+    (SD2.1-768, diffusers' "v_prediction")."""
+    if prediction not in PREDICTION_TYPES:
+        raise ValueError(f"{what}: prediction must be one of {PREDICTION_TYPES}, got {prediction!r}")
+
+
 def out_cfg_ddim(xn, w, bias, *, latents=None, eps_out=None, coef=None, guidance=1.0, known=None, noise=None,
-                 mask=None, lat_half_out=None, step_counter=None, hist=None, Nimg, H, W, C_):
+                 mask=None, lat_half_out=None, step_counter=None, hist=None, Nimg, H, W, C_, prediction="epsilon"):
+    """ea_out_cfg_ddim, or ea_out_cfg_vpred with prediction="v_prediction" (the network output is v)."""
+    check_prediction("out_cfg_ddim", prediction)
     check_out_buffers("out_cfg_ddim", 2, xn, w, bias, latents, eps_out, coef, known, noise, mask, lat_half_out,
                       step_counter, hist, Nimg, H, W, C_)
     lib = L.lib()
-    L.check(lib.ea_out_cfg_ddim(_p(xn), _p(w), _p(bias), _p(latents), _p(eps_out), _p(coef),
-                                float(guidance), _p(known), _p(noise), _p(mask), _p(lat_half_out),
-                                _p(step_counter), _p(hist), Nimg, H, W, C_, _stream()), "ea_out_cfg_ddim")
+    name = "ea_out_cfg_ddim" if prediction == "epsilon" else "ea_out_cfg_vpred"
+    L.check(getattr(lib, name)(_p(xn), _p(w), _p(bias), _p(latents), _p(eps_out), _p(coef),
+                               float(guidance), _p(known), _p(noise), _p(mask), _p(lat_half_out),
+                               _p(step_counter), _p(hist), Nimg, H, W, C_, _stream()), name)
 
 
 def out_ddim(xn, w, bias, *, latents=None, eps_out=None, coef=None, known=None, noise=None, mask=None,
-             lat_half_out=None, step_counter=None, hist=None, Nimg, H, W, C_):
+             lat_half_out=None, step_counter=None, hist=None, Nimg, H, W, C_, prediction="epsilon"):
     """ea_out_ddim: the out conv and update of out_cfg_ddim without guidance; every buffer holds the Nimg images
-    once."""
+    once.  prediction="v_prediction": ea_out_vpred."""
+    check_prediction("out_ddim", prediction)
     check_out_buffers("out_ddim", 1, xn, w, bias, latents, eps_out, coef, known, noise, mask, lat_half_out,
                       step_counter, hist, Nimg, H, W, C_)
     lib = L.lib()
-    L.check(lib.ea_out_ddim(_p(xn), _p(w), _p(bias), _p(latents), _p(eps_out), _p(coef), _p(known), _p(noise),
-                            _p(mask), _p(lat_half_out), _p(step_counter), _p(hist), Nimg, H, W, C_, _stream()),
-            "ea_out_ddim")
+    name = "ea_out_ddim" if prediction == "epsilon" else "ea_out_vpred"
+    L.check(getattr(lib, name)(_p(xn), _p(w), _p(bias), _p(latents), _p(eps_out), _p(coef), _p(known), _p(noise),
+                               _p(mask), _p(lat_half_out), _p(step_counter), _p(hist), Nimg, H, W, C_, _stream()),
+            name)
 
 
 def step_gather(step_counter, n_rows, tables, dsts):

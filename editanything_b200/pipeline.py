@@ -20,6 +20,12 @@ guided request runs the networks on 2N rows ([negative; positive] prompts, doubl
 combines the two halves in the step's last kernel; with guidance_scale <= 1 only the positive prompt is encoded, the
 networks run on the N images alone and their output drives the scheduler directly, so the scale has no further effect.
 
+Base models that predict v = sqrt(a) eps - sqrt(1-a) x0 instead of the noise (stabilityai/stable-diffusion-2-1, the
+768x768 SD2.1 model, with the SD2.1 EditAnything ControlNets) run too: the loader reads `prediction_type` from the
+checkpoint's scheduler/scheduler_config.json into `DDIMScheduler`, `UniPCMultistepScheduler.from_config` carries it
+over, and the fused step converts the guidance-combined v to x0 and eps like the reference sampler
+(cldm/ddim_hacked.py:190-217).  Any other scheduler object receives the combined network output in its `step`.
+
 Not supported (raises NotImplementedError rather than silently diverging): the reference-only mode
 (`ref_image`, `utils/stable_diffusion_reference.py`), guess_mode.
 """
@@ -35,6 +41,7 @@ import torch.nn.functional as F
 
 from .denoise import DenoiseEngine, ddim_schedule
 from .loading import ControlNetModel, ControlNetModel2  # noqa: F401  (the names editany_lora.py imports)
+from .ops import PREDICTION_TYPES
 from .schedulers import UniPCMultistepScheduler
 
 try:  # PIL is only needed for PIL inputs / output_type="pil"
@@ -53,13 +60,17 @@ class DDIMScheduler:
     """DDIM (eta = 0) with the reference sampler's 'uniform' timestep table
     (cldm/ddim_hacked.py:23-52, ldm/modules/diffusionmodules/util.py:46-74) behind the scheduler
     surface the pipeline uses (`set_timesteps/timesteps/init_noise_sigma/scale_model_input/step/
-    add_noise/order`, utils/...inpaint.py:1430-1431,1012,1547,1634,1651,1538)."""
+    add_noise/order`, utils/...inpaint.py:1430-1431,1012,1547,1634,1651,1538).
+    prediction_type: what the network predicts - "epsilon" (the noise), or "v_prediction" (v = sqrt(a) eps -
+    sqrt(1-a) x0, the SD2.1-768 base models; cldm/ddim_hacked.py:194-217)."""
     order = 1
     init_noise_sigma = 1.0
 
-    def __init__(self, linear_start=0.00085, linear_end=0.012, num_train_timesteps=1000):
+    def __init__(self, linear_start=0.00085, linear_end=0.012, num_train_timesteps=1000, prediction_type="epsilon"):
+        if prediction_type not in PREDICTION_TYPES:
+            raise NotImplementedError(f"prediction_type {prediction_type!r}: only {PREDICTION_TYPES}")
         self.config = SimpleNamespace(beta_start=linear_start, beta_end=linear_end, beta_schedule="scaled_linear",
-                                      num_train_timesteps=num_train_timesteps, prediction_type="epsilon")
+                                      num_train_timesteps=num_train_timesteps, prediction_type=prediction_type)
         betas = np.linspace(linear_start ** 0.5, linear_end ** 0.5, num_train_timesteps, dtype=np.float64) ** 2
         self.alphas_cumprod = np.cumprod(1.0 - betas, axis=0)
         self.timesteps = None
@@ -79,9 +90,13 @@ class DDIMScheduler:
 
     def step(self, model_output, t, sample, **kw):
         a, ap = self.coefficients(t)
-        x0 = (sample - math.sqrt(1.0 - a) * model_output) / math.sqrt(a)
-        return SimpleNamespace(prev_sample=math.sqrt(ap) * x0 + math.sqrt(1.0 - ap) * model_output,
-                               pred_original_sample=x0)
+        if self.config.prediction_type == "v_prediction":
+            x0 = math.sqrt(a) * sample - math.sqrt(1.0 - a) * model_output     # ddpm.py:290-302
+            e = math.sqrt(a) * model_output + math.sqrt(1.0 - a) * sample
+        else:
+            e = model_output
+            x0 = (sample - math.sqrt(1.0 - a) * e) / math.sqrt(a)
+        return SimpleNamespace(prev_sample=math.sqrt(ap) * x0 + math.sqrt(1.0 - ap) * e, pred_original_sample=x0)
 
     def add_noise(self, original, noise, timesteps):
         t = int(timesteps.reshape(-1)[0]) if torch.is_tensor(timesteps) else int(timesteps)
@@ -537,7 +552,8 @@ class StableDiffusionControlNetInpaintPipeline:
             on = [1.0 if (i < blend_steps and not host_blend) else 0.0 for i in range(n_t)]
             eng.set_schedule([int(t) for t in timesteps], [c[0] for c in coefs], [c[1] for c in coefs],
                              blend=([k[0] for k in k_next], [k[1] for k in k_next], on),
-                             multistep=self.scheduler.coefficient_rows() if unipc else None)
+                             multistep=self.scheduler.coefficient_rows() if unipc else None,
+                             prediction_type=self.scheduler.config.prediction_type)
             if inpaint_unet:
                 eng.set_unet_condition(mask_lat, masked_lat)
             eng.begin(lat, guidance_scale, known_nchw=init_d if blend_steps else None,

@@ -20,6 +20,8 @@ from types import SimpleNamespace
 import numpy as np
 import torch
 
+from .ops import PREDICTION_TYPES
+
 
 def _scaled_linear_alphas_cumprod(beta_start, beta_end, n, schedule="scaled_linear"):
     if schedule == "scaled_linear":
@@ -38,8 +40,8 @@ class UniPCMultistepScheduler:
     def __init__(self, num_train_timesteps=1000, beta_start=0.0001, beta_end=0.02, beta_schedule="linear",
                  solver_order=2, prediction_type="epsilon", thresholding=False, predict_x0=True, solver_type="bh2",
                  lower_order_final=True, disable_corrector=(), **_ignored):
-        if prediction_type != "epsilon" or thresholding or not predict_x0:
-            raise NotImplementedError("only epsilon prediction in data-prediction (x0) form without thresholding")
+        if prediction_type not in PREDICTION_TYPES or thresholding or not predict_x0:
+            raise NotImplementedError("only epsilon or v prediction in data-prediction (x0) form without thresholding")
         if solver_type not in ("bh1", "bh2"):
             raise NotImplementedError(solver_type)
         self.config = SimpleNamespace(num_train_timesteps=num_train_timesteps, beta_start=beta_start, beta_end=beta_end,
@@ -143,7 +145,10 @@ class UniPCMultistepScheduler:
         k = self.config.solver_order
         use_corrector = (step_index > 0 and (step_index - 1) not in self.config.disable_corrector
                          and self.last_sample is not None)
-        x0 = (sample - float(self.sigma_t[t]) * model_output) / float(self.alpha_t[t])        # convert_model_output
+        if self.config.prediction_type == "v_prediction":                                   # convert_model_output
+            x0 = float(self.alpha_t[t]) * sample - float(self.sigma_t[t]) * model_output
+        else:
+            x0 = (sample - float(self.sigma_t[t]) * model_output) / float(self.alpha_t[t])
         if use_corrector:
             s0 = self.timestep_list[-1]
             hist = [ts for ts in self.timestep_list[-2::-1] if ts is not None]
@@ -173,7 +178,7 @@ class UniPCMultistepScheduler:
     # ---- the same loop as a coefficient table (device-side fused update) ----------------------------------------
     def coefficient_rows(self):
         """One row per step for solver_order <= 2, in terms of the tensors a fused update holds:
-            x0  = (x - sigma * eps) / alpha                      (x = latents entering the step)
+            x0  = (x - sigma * eps) / alpha, or alpha * x - sigma * v  (x = latents entering the step)
             xc  = kx * x + kl * last + k1 * m1 + k2 * m2 + k0 * x0     (corrected sample; identity on step 0)
             x'  = px * xc + p0 * x0 + p1 * m1                          (prediction for the next timestep)
             then  m2 <- m1,  m1 <- x0,  last <- xc.

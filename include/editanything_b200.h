@@ -268,6 +268,19 @@ int ea_out_cfg_ddim(const void* xn, const float* w, const float* bias, float* la
 int ea_out_ddim(const void* xn, const float* w, const float* bias, float* latents, float* eps_out,
                 const float* coef, const float* known, const float* noise, const float* mask,
                 void* lat_half_out, int* step_counter, float* hist, int Nimg, int H, int W, int C, void* stream);
+/* ea_out_cfg_vpred / ea_out_vpred: ea_out_cfg_ddim / ea_out_ddim for a v-prediction base model (the network predicts
+ * v = sqrt(a_t) eps - sqrt(1-a_t) x0, e.g. stabilityai/stable-diffusion-2-1 at 768x768; cldm/ddim_hacked.py:194-217,
+ * ldm/models/diffusion/ddpm.py:290-302).  Same arguments and buffers.  m = the network output after the guidance
+ * combine (guided: applied to v, :190-192), then x0 = coef[0] x - coef[1] m and eps = coef[0] m + coef[1] x;
+ * mode 0: x' = coef[2] x0 + coef[3] eps; mode 1: x0 enters the multistep recurrence above unchanged.  Blend,
+ * history, lat_half_out and the step counter are as above; eps_out (optional) is the raw network output (v). */
+int ea_out_cfg_vpred(const void* xn, const float* w, const float* bias, float* latents,
+                     float* eps_out, const float* coef, float guidance, const float* known,
+                     const float* noise, const float* mask, void* lat_half_out, int* step_counter,
+                     float* hist, int Nimg, int H, int W, int C, void* stream);
+int ea_out_vpred(const void* xn, const float* w, const float* bias, float* latents, float* eps_out,
+                 const float* coef, const float* known, const float* noise, const float* mask,
+                 void* lat_half_out, int* step_counter, float* hist, int Nimg, int H, int W, int C, void* stream);
 
 /* ---- ea_step_gather: first kernel of a captured denoising step ---------------------------------
  * The loop of utils/stable_diffusion_controlnet_inpaint.py:1540-1656 changes only scalars from step to step
