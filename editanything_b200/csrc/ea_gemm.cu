@@ -706,12 +706,18 @@ ea_gemm_kernel(const __grid_constant__ GemmLaunch<NG> L, const int tiles_per_gro
     const int ncol0 = tn * BN;
     float* cbt = cb + ((it & 1) * RP + sub) * 512;
     const long long lin_m0 = p.mode == EA_GEMM_LINEAR ? (long long)tm * BM + wq * 32 : -1;
-    const int b_first = row_info(p, tm, 0).batch, b_last = row_info(p, tm, BM - 1).batch;
+    const int b_first = row_info(p, tm, 0).batch, b_end = row_info(p, tm, BM - 1).batch;
+    // rowvec has rows for the problem's batches only; the tile's last row lies past them in a partly empty image
+    // block or in the last partial tile of a LINEAR problem, so the second staged row is that of the last valid row.
+    // The epilogue is still chosen from the tile's full span b_first .. b_end: it decides the rounding order of
+    // bias + rowvec, which must not depend on how many image slots hold data.
+    const int b_last = min(b_end, p.mode != EA_GEMM_LINEAR ? p.Bsz - 1
+                                  : p.rows_per_batch > 0 ? (p.M - 1) / p.rows_per_batch : 0);
     // Fast path (the common case): before the main loop, bias (+ the per-image time-embedding row vector) for the
     // tile's columns is staged in shared memory and the first residual chunk is pulled into registers, so that the
     // per-chunk work after the main loop is load -> FMA -> 16-byte stores with the NEXT chunk's residual in flight.
     const bool fast = sub_ok && p.splits == 1 && !geglu && !p.out_f32 && !p.accumulate && !p.row_scale &&
-                      (b_last - b_first) <= 1;
+                      (b_end - b_first) <= 1;
     uint4 rres[8];   // next 64-column group of the residual (coalesced layout)
     // LayerNorm fold, consumer side: this row's mean / rstd from the producer's per-chunk partials (fixed
     // summation order: deterministic).  out = acc * ln_r + ln_nm * g[n] + c[n].
@@ -1207,12 +1213,15 @@ static int gemm_fill_group(const ea_gemm_args* a, GemmGroup& G, GemmShape& sh) {
     p.ln_inv_c = a->ln_stats ? 1.0f / (float)a->K : 0.f;
     p.ln_eps = a->ln_eps;
   }
-  if (p.ldo % 8 != 0 || (p.residual && p.ldr % 8 != 0) || (p.out2 && p.ldo2 % 8 != 0))
+  // a leading dimension narrower than the row it strides over makes rows overlap (0 writes every row onto row 0)
+  const long long n_out = a->act == EA_ACT_GEGLU ? a->N / 2 : a->N;
+  if (p.ldo % 8 != 0 || p.ldo < n_out || (p.residual && (p.ldr % 8 != 0 || p.ldr < n_out)) ||
+      (p.out2 && (p.ldo2 % 8 != 0 || p.ldo2 < n_out)))
     return EA_ERR_SHAPE;
 
   CUtensorMap* tmA[4] = {&G.tmA0, &G.tmA1, &G.tmA2, &G.tmA3};
   if (a->mode == EA_GEMM_LINEAR) {
-    if (a->K % 8 != 0 || a->lda % 8 != 0) return EA_ERR_SHAPE;
+    if (a->K % 8 != 0 || a->lda % 8 != 0 || a->lda < a->K) return EA_ERR_SHAPE;
     p.nkb_main = (a->K + BK - 1) / BK;
     p.nkb_extra = 0;
     p.cin_blocks = 1;
@@ -1226,6 +1235,7 @@ static int gemm_fill_group(const ea_gemm_args* a, GemmGroup& G, GemmShape& sh) {
     const int H = a->H, W = a->W, B = a->Bsz, C = a->Cin;
     if (C % 64 != 0 || H <= 0 || W <= 0 || B <= 0) return EA_ERR_SHAPE;
     if ((long long)B * H * W != a->M) return EA_ERR_SHAPE;
+    if (a->lda != 0 && (a->lda < C || a->lda % 8 != 0)) return EA_ERR_SHAPE;
     p.H = H; p.W = W; p.Bsz = B;
     conv_geometry(H, W, p.bw, p.bh, p.bn);
     p.tiles_w = W / p.bw;
@@ -1258,6 +1268,7 @@ static int gemm_fill_group(const ea_gemm_args* a, GemmGroup& G, GemmShape& sh) {
     G.tmAx = G.tmA0;
     if (a->a_extra) {
       if (a->mode != EA_GEMM_CONV_S1 || a->Cin_extra % 64 != 0) return EA_ERR_SHAPE;
+      if (a->ld_extra != 0 && (a->ld_extra < a->Cin_extra || a->ld_extra % 8 != 0)) return EA_ERR_SHAPE;
       const long long ldx = a->ld_extra > 0 ? a->ld_extra : a->Cin_extra;
       uint64_t dims[4] = {(uint64_t)a->Cin_extra, (uint64_t)W, (uint64_t)H, (uint64_t)B};
       uint64_t st[3] = {(uint64_t)ldx * 2, (uint64_t)ldx * W * 2, (uint64_t)ldx * W * H * 2};
@@ -1267,6 +1278,7 @@ static int gemm_fill_group(const ea_gemm_args* a, GemmGroup& G, GemmShape& sh) {
     }
   }
   sh.nkb = p.nkb_main + p.nkb_extra;
+  if (a->ldw > 0 && (a->ldw % 8 != 0 || a->ldw < sh.Ktot)) return EA_ERR_SHAPE;
   return EA_OK;
 }
 
@@ -1392,7 +1404,6 @@ extern "C" int ea_gemm_grouped(const ea_gemm_args* args, int n_groups, void* str
              (size_t)g * tiles * p.splits * (RP * BM * BN);
     }
     const long long ldw = ag->ldw > 0 ? ag->ldw : sh0.Ktot;
-    if (ldw % 8 != 0) return EA_ERR_SHAPE;
     if (encode_2d(&L.g[g].tmB, ag->w, (uint64_t)sh0.Ktot, (uint64_t)ag->N, (uint64_t)ldw * 2, BK, (uint32_t)BN))
       return EA_ERR_TMAP;
   }

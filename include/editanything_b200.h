@@ -79,7 +79,9 @@ void ea_reset_launch_count(void);
  *            (all resident by construction) and finishes a 1/splits share of the tile with the
  *            full fused epilogue — deterministic summation order, no extra launch.
  * Constraints: N % 8 == 0, K % 8 == 0, Cin % 64 == 0, all leading dims % 8 == 0,
- *              pointers 16-byte aligned.
+ *              pointers 16-byte aligned.  Leading dims cover a whole row: LINEAR lda >= K; CONV lda (if set)
+ *              >= Cin and ld_extra (if set) >= Cin_extra; ldw (if set) >= total K; ldo, ldo2 and ldr >= the
+ *              output width (N, N/2 for GEGLU).  Anything else is EA_ERR_SHAPE, before any launch.
  */
 #define EA_GEMM_MAX_PREFETCH 3
 typedef struct ea_gemm_args {

@@ -104,6 +104,26 @@ def conv_nhwc(x, w, bias, stride=1):
     return out, mag
 
 
+def conv_gemm(x, w, mode, extra=None):
+    """ea_gemm's implicit-GEMM convolutions.  x: NHWC input [B, Hin, Win, Cin]; w: [Cout, 9 Cin (+ Cin_extra)] with K
+    index (kh * 3 + kw) * Cin + c; mode "s1" (3x3, stride 1, pad 1), "s2" (stride 2, pad 1 on the 2H x 2W input) or
+    "s2a" (F.pad(x, (0, 1, 0, 1)), then stride 2, pad 0); extra: [B, H, W, Cin_extra], the operand of the folded 1x1
+    skip convolution (the last Cin_extra columns of w).  Returns (out [B, H, W, Cout], sum of |a w|), no bias."""
+    cout, cin = w.shape[0], x.shape[-1]
+    wt = w[:, :9 * cin].reshape(cout, 3, 3, cin).permute(0, 3, 1, 2)
+    xc = x.permute(0, 3, 1, 2)
+    if mode == "s2a":
+        xc, kw = F.pad(xc, (0, 1, 0, 1)), dict(stride=2)
+    else:
+        kw = dict(stride=1 if mode == "s1" else 2, padding=1)
+    out = F.conv2d(xc, wt, **kw).permute(0, 2, 3, 1)
+    mag = F.conv2d(xc.abs(), wt.abs(), **kw).permute(0, 2, 3, 1)
+    if extra is not None:
+        we = w[:, 9 * cin:]
+        out, mag = out + extra @ we.T, mag + extra.abs() @ we.abs().T
+    return out, mag
+
+
 def out_conv(xn, w, bias):
     """The out conv of ea_out_cfg_ddim: xn [2N, H, W, C], w [4, 3, 3, C] -> eps [2N, H, W, 4] and its |.| sums."""
     return conv_nhwc(xn, w.permute(1, 2, 3, 0), bias)

@@ -93,6 +93,40 @@ def test_conv_matches_loops():
     assert torch.allclose(eps, want, rtol=1e-12, atol=1e-12)
 
 
+def _im2col(x, mode):
+    """[B, Hin, Win, C] -> [B, H, W, 9 C] in ea_gemm's K order (kh * 3 + kw) * C + c, by index arithmetic: tap (kh, kw)
+    of output pixel (oh, ow) reads input pixel (s oh + kh - p, s ow + kw - p), zero outside the input."""
+    B, Hin, Win, C = x.shape
+    s, p = (1, 1) if mode == "s1" else (2, 1) if mode == "s2" else (2, 0)
+    H, W = Hin // s, Win // s
+    cols = []
+    for kh in range(3):
+        for kw in range(3):
+            ih, iw = s * torch.arange(H) + kh - p, s * torch.arange(W) + kw - p
+            ok = ((ih >= 0) & (ih < Hin))[:, None] & ((iw >= 0) & (iw < Win))[None, :]
+            v = x[:, ih.clamp(0, Hin - 1)][:, :, iw.clamp(0, Win - 1)]
+            cols.append(v * ok[None, :, :, None])
+    return torch.cat(cols, dim=-1)
+
+
+def test_conv_gemm_matches_im2col():
+    """fp64_refs.conv_gemm (F.conv2d / F.pad) against the GEMM view of each mode, with and without the folded skip."""
+    for mode, (Hin, Win), extra in [("s1", (5, 7), 0), ("s1", (4, 6), 3), ("s2", (6, 10), 0), ("s2a", (8, 6), 0),
+                                    ("s2a", (10, 4), 0)]:
+        x = _rn(2, Hin, Win, 4, seed=Hin + Win)
+        s = 1 if mode == "s1" else 2
+        w = _rn(5, 36 + extra, seed=Win)
+        xe = _rn(2, Hin // s, Win // s, extra, seed=3) if extra else None
+        cols = _im2col(x, mode)
+        want, want_mag = cols @ w[:, :36].T, cols.abs() @ w[:, :36].abs().T
+        if extra:
+            want, want_mag = want + xe @ w[:, 36:].T, want_mag + xe.abs() @ w[:, 36:].abs().T
+        out, mag = R.conv_gemm(x, w, mode, xe)
+        assert out.shape == (2, Hin // s, Win // s, 5)
+        assert torch.allclose(out, want, rtol=1e-12, atol=1e-12), mode
+        assert torch.allclose(mag, want_mag, rtol=1e-12, atol=1e-12), mode
+
+
 def test_small_linear_and_timestep_embedding():
     x, w, b = _rn(3, 16, seed=13), _rn(5, 16, seed=14), _rn(5, seed=15)
     y, pre, mag = R.small_linear(x, w, b, True, True)
