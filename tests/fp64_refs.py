@@ -208,7 +208,49 @@ def image_out(x, C, scale, shift, lo, hi):
     return (x[..., :C] * scale + shift).clamp(lo, hi).permute(0, 2, 1)
 
 
+# ---- per-element gate -------------------------------------------------------------------------------------------
+def worst_element(got, ref, bound):
+    """(worst |got - ref| / bound, its flat index, number of elements out of bound) of got against a float64 reference;
+    a NaN difference counts as infinitely far, an exact match as 0 whatever the bound."""
+    err = (got.double() - ref).abs()
+    ratio = torch.where(err == 0, torch.zeros_like(err), err / bound)
+    ratio = torch.where(torch.isnan(err), torch.full_like(err, math.inf), ratio)
+    i = int(torch.argmax(ratio.reshape(-1)))
+    return float(ratio.reshape(-1)[i]), i, int((~(err <= bound)).sum())
+
+
 # ---- GEMM epilogue ---------------------------------------------------------------------------------------------
+def gemm_act(act, pre, e):
+    """act(pre) and its error bound for an fp32 pre-activation `pre` (float64) whose error is bounded by `e`; act is
+    "none", "silu", "gelu" or "geglu" (pre in the packed [value | gate] layout)."""
+    if act == "none":
+        return pre, e
+    if act == "silu":
+        return silu(pre), 1.1 * e + silu_eval_err(pre)
+    if act == "gelu":
+        return gelu(pre), 1.13 * e + gelu_eval_err(pre)
+    x, g = geglu_split(pre)
+    ex, eg = geglu_split(e)
+    gg = gelu(g)
+    return x * gg, gg.abs() * ex + x.abs() * (1.13 * eg + gelu_eval_err(g))
+
+
+def gemm_out(y, err, scale=1.0, extras=(), out_dtype=None, n_scale=0):
+    """(reference, bound) of the stored GEMM output y * scale (+ each of `extras`: residual, accumulated value) for an
+    activation output y with error bound err: the scaled error, one u per add, and 1 ulp of out_dtype (None: an fp32
+    destination, no ulp).  `scale` may be a tensor (out_scale * row_scale[m]).  n_scale: the number of fp32 products
+    the scale takes (out_scale, row_scale), one u of |y * scale| each - the ulp of a half destination covers them,
+    an fp32 destination (the VAE logits, an accumulated zero-conv into fp32) needs them counted."""
+    t = y * scale
+    ref = t + sum(extras) if extras else t
+    bound = abs(scale) * err + (1 + len(extras)) * U32 * (t.abs() + sum(v.abs() for v in extras))
+    if n_scale:
+        bound = bound + n_scale * U32 * t.abs()
+    if out_dtype is not None:
+        bound = bound + ulp(ref, out_dtype)
+    return ref, bound
+
+
 def gemm_epilogue(a, w, bias=None, out_scale=1.0, row_scale=None, old=None):
     """out = (A W^T + bias) * out_scale * row_scale[m] (+ old).  Returns (out, the scaled product term, the scaled
     |.| sums)."""

@@ -132,15 +132,10 @@ def _randn(shape, seed, scale=1.0):
 
 def _close(key, what, got, ref, bound):
     """|got - ref| <= bound per element of [B, H, W, C] (NaN fails); records the worst ratio under `key`."""
-    err = (got.double() - ref).abs()
-    ratio = torch.where(err == 0, torch.zeros_like(err), err / bound)
-    ratio = torch.where(torch.isnan(err), torch.full_like(err, math.inf), ratio)
-    i = int(torch.argmax(ratio.reshape(-1)))
-    worst = float(ratio.reshape(-1)[i])
+    worst, i, n_bad = R.worst_element(got, ref, bound)
     WORST[key] = max(WORST.get(key, 0.0), worst)
     if not worst <= 1.0:
         b, y, x, ch = (int(v) for v in np.unravel_index(i, tuple(ref.shape)))
-        n_bad = int((~(err <= bound)).sum())
         raise AssertionError(f"{what}: {n_bad} of {ref.numel()} elements out of bound; worst at image {b}, y {y}, "
                              f"x {x}, channel {ch}: got {float(got.reshape(-1)[i])!r}, ref {float(ref.reshape(-1)[i])!r}"
                              f", bound {float(bound.reshape(-1)[i]):.3e} (ratio {worst:.3g})")
@@ -232,20 +227,13 @@ class _Case:
         """got: [M, cout] -> per-element gate against the float64 reference."""
         c = self.c
         B, H, W, cout = c["B"], c["H"], c["W"], c["cout"]
-        e = (self.K + 2) * U * self.mag
-        if c.get("silu"):
-            y, err = R.silu(self.pre), 1.1 * e + R.silu_eval_err(self.pre)
-        else:
-            y, err = self.pre, e
+        y, err = R.gemm_act("silu" if c.get("silu") else "none", self.pre, (self.K + 2) * U * self.mag)
         extra = []
         if self.res is not None:
             extra.append(self.res.double().reshape(B, H, W, cout))
         if self.old is not None:
             extra.append(self.old.double().reshape(B, H, W, cout))
-        ref = y + sum(extra) if extra else y
-        bound = err + (1 + len(extra)) * U * (y.abs() + sum(v.abs() for v in extra))
-        if got.dtype != torch.float32:
-            bound = bound + R.ulp(ref, got.dtype)
+        ref, bound = R.gemm_out(y, err, 1.0, extra, None if got.dtype == torch.float32 else got.dtype)
         got = got.reshape(B, H, W, cout)
         _close(key, f"{self.name} {what}", got, ref, bound)
         if "pad" in c:

@@ -61,16 +61,10 @@ def _randn(shape, seed, dtype=torch.float32, scale=1.0, offset=0.0):
 
 def _close(kernel, what, got, ref, bound):
     """|got - ref| <= bound element-wise (NaN fails); records the worst ratio under `kernel`."""
-    got = got.double()
-    err = (got - ref).abs()
-    ratio = torch.where(err == 0, torch.zeros_like(err), err / bound)
-    ratio = torch.where(torch.isnan(err), torch.full_like(err, math.inf), ratio)
-    i = int(torch.argmax(ratio.reshape(-1)))
-    worst = float(ratio.reshape(-1)[i])
+    worst, i, n_bad = R.worst_element(got, ref, bound)
     WORST[kernel] = max(WORST.get(kernel, 0.0), worst)
     if not worst <= 1.0:
         idx = tuple(int(v) for v in np.unravel_index(i, tuple(ref.shape)))
-        n_bad = int((~(err <= bound)).sum())
         raise AssertionError(f"{kernel} {what}: {n_bad} of {ref.numel()} elements out of bound; worst at {idx}: "
                              f"got {float(got.reshape(-1)[i])!r}, ref {float(ref.reshape(-1)[i])!r}, "
                              f"bound {float(bound.reshape(-1)[i]):.3e} (ratio {worst:.3g})")
@@ -608,25 +602,10 @@ def test_gemm_out_f32_accumulate_ragged():
 ACTS = {"silu": L.EA_ACT_SILU, "gelu": L.EA_ACT_GELU, "geglu": L.EA_ACT_GEGLU}
 
 
-def _act_ref(act, pre, e):
-    """act(pre) and its error bound, for an fp32 pre-activation `pre` (float64) whose error is bounded by `e`."""
-    if act == "silu":
-        return R.silu(pre), 1.1 * e + R.silu_eval_err(pre)
-    if act == "gelu":
-        return R.gelu(pre), 1.13 * e + R.gelu_eval_err(pre)
-    x, g = R.geglu_split(pre)
-    ex, eg = R.geglu_split(e)
-    gg = R.gelu(g)
-    return x * gg, gg.abs() * ex + x.abs() * (1.13 * eg + R.gelu_eval_err(g))
-
-
 def _act_check(kernel, what, got, act, pre, e, scale=1.0, res=None, old=None):
     """got = act(pre) * scale (+ res) (+ old) with the rounding of each step, in got's dtype."""
-    y, err = _act_ref(act, pre, e)
-    t = y * scale
-    extra = [v for v in (res, old) if v is not None]
-    ref = t + sum(extra) if extra else t
-    bound = abs(scale) * err + (1 + len(extra)) * U * (t.abs() + sum(v.abs() for v in extra)) + R.ulp(ref, got.dtype)
+    y, err = R.gemm_act(act, pre, e)
+    ref, bound = R.gemm_out(y, err, scale, [v for v in (res, old) if v is not None], got.dtype)
     return _close(kernel, what, got, ref, bound)
 
 
