@@ -1,10 +1,34 @@
-"""The C-ABI library loads and exports every symbol include/editanything_b200.h declares."""
+"""The C-ABI library loads and exports every symbol include/editanything_b200.h declares, and the ctypes argument
+structs have the header's layout."""
 import os
 import re
+
+import pytest
 
 from editanything_b200 import _lib
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+
+
+def _struct_members(name):
+    """(member, array length or None) of `typedef struct <name> {...} <name>;` in the header, in declaration order."""
+    hdr = re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", "editanything_b200.h")).read(), flags=re.S)
+    body = re.search(r"typedef struct %s \{(.*?)\} %s;" % (name, name), hdr, flags=re.S).group(1)
+    members = []
+    for decl in filter(None, (d.strip() for d in body.split(";"))):
+        for declarator in decl.split(","):
+            member, length = re.search(r"(\w+)\s*(?:\[(\w+)\])?\s*$", declarator).groups()
+            members.append((member, int(length) if length else None))
+    return members
+
+
+@pytest.mark.parametrize("struct,cls", [("ea_gemm_args", _lib.GemmArgs), ("ea_attn_args", _lib.AttnArgs),
+                                        ("ea_gn_args", _lib.GnArgs)])
+def test_ctypes_struct_matches_header(struct, cls):
+    """A ctypes field missing, added or out of order shifts every later field: the library would read, say, the
+    workspace pointer from where the caller stored a leading dimension."""
+    fields = [(name, getattr(t, "_length_", None)) for name, t in cls._fields_]
+    assert fields == _struct_members(struct)
 
 
 def test_every_declared_symbol_is_exported_and_bound():
