@@ -34,6 +34,10 @@ step converts v to x0 and eps.  An SD2.1 base has no tile ControlNet of its own,
 
 and call `process(..., enable_tile=False)`.
 
+Tile refinement: `refine_image_resolution` sets the short side of the tile pass's image as in the reference; the
+VAE's attention runs on the fused kernel above 128 x 128 latents, so sizes up to 2048 x 2752 (256 x 344 latents) run
+on one 80 GB H100 and are tested there.  Larger sizes are not verified.
+
 LoRA: `lora_model_path` names a kohya `.safetensors` file merged at `lora_weight` into the UNet and the text
 encoder of the generation and the tile pipeline before their weights are packed (editany_lora.py:378-381, 413-416;
 editanything_b200.lora), e.g. the reference's "Beauty Edit" setup (editany_beauty.py:54-64)

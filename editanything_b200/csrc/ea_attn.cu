@@ -347,12 +347,246 @@ ea_attn_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ 
   }
 }
 
-// [B, N, heads, d] with strides (bs, ns, d) elements; boxes of `box_cols` head-dim columns x 128 rows
+// ---------------------------------------------------------------------------------------------------------------
+// Wide heads, 192 < d <= 512 (the VAE AttnBlock: one head of d = C = 512).  The kernel above cannot take them: a
+// warp-group's O tile of 64 rows x 512 fp32 is 256 registers per thread, and Q for 128 rows x 512 halves plus one
+// 128-key K and V tile is past the 227 KB of shared memory.  So:
+//   * one CTA = one (batch, head) and 64 query rows: Q is 64 KB (nd SWIZZLE_128B boxes of 64 rows x 64 columns);
+//   * 32-key K / V tiles, 32 KB each, in a ring of >= 2 stages (K: nd boxes of 32 rows; V: 32 SWIZZLE_32B boxes of
+//     16 columns, always all of them, so the accumulator is 512 wide and columns past d are TMA zero fill);
+//   * 256 threads = two warp-groups and no producer warp-group: thread 0 issues the TMA loads, refilling a stage
+//     once all 8 warps have released it.  A ninth warp would put three warps on one SM sub-partition's 16K
+//     registers and cap every thread at 168, and setmaxnreg does not lift what ptxas compiles for (see above); at
+//     256 threads each thread may hold 255, enough for O (128), S (16) and P (8) without spills;
+//   * both consumer warp-groups cover the same 64 rows, and warp-group g owns O columns 256 g .. 256 g + 255.  Each
+//     computes S = Q K^T over all d columns itself and runs the online softmax on it, so P stays in registers as the
+//     A operand of its m64n256k16 P V wgmmas, as in the kernel above.
+// That costs 1.5x the minimum MMA work (Q K^T twice).  The alternative, splitting the Q K^T reduction over d between
+// the warp-groups, would need the partial S tiles exchanged through shared memory and a barrier between the two
+// warp-groups on every 32-key tile; duplicating S keeps the warp-groups independent and the kernel the same shape
+// as the one above.  Both warp-groups compute bit-identical S, m and l, so the two halves of a row agree.
+// Per warp-group S_j = Q K_j^T is issued together with O += P_{j-1} V_{j-1}, and the softmax of S_j runs while the
+// P V wgmmas are in flight (the PIPELINE schedule of the kernel above).  No rel-pos bias.
+static constexpr int AW_BQ = 64;
+static constexpr int AW_BKV = 32;
+static constexpr int AW_DO = 512;
+static constexpr int AW_QBOX = AW_BQ * 128;    // bytes of one 64-row x 64-half SWIZZLE_128B box (Q)
+static constexpr int AW_KBOX = AW_BKV * 128;   // bytes of one 32-row x 64-half SWIZZLE_128B box (K)
+static constexpr int AW_VBOX = AW_BKV * 32;    // bytes of one 32-key x 16-half SWIZZLE_32B box (V)
+static constexpr int AW_NV = AW_DO / 16;
+static constexpr int AW_MAX_STAGES = 4;
+static constexpr int AW_WARPS = 8;
+static constexpr int AW_THREADS = AW_WARPS * 32;
+static_assert(8 * AW_QBOX + 2 * (8 * AW_KBOX + AW_NV * AW_VBOX) <= 227 * 1024 - 1024 - 256,
+              "d = 512 must get a ring of two stages: the pipelined loop waits for tile j before it frees tile j - 1");
+
+__global__ void __launch_bounds__(AW_THREADS, 1)
+ea_attn_wide_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
+                    const __grid_constant__ CUtensorMap tmV, const AttnKParams p) {
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
+                                             ~uintptr_t(1023));
+  // layout: Q[nd] | KV[stages][K nd | V AW_NV] | barriers
+  const int q_bytes = p.nd * AW_QBOX;
+  const int k_bytes = p.nd * AW_KBOX;
+  const int kv_stage_bytes = k_bytes + AW_NV * AW_VBOX;
+  uint8_t* sQ = smem;
+  uint8_t* sKV = sQ + q_bytes;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sKV + p.stages * kv_stage_bytes);
+  uint64_t* q_full = bars;                       // [1]
+  uint64_t* kv_full = bars + 1;                  // [AW_MAX_STAGES]
+  uint64_t* kv_empty = kv_full + AW_MAX_STAGES;  // [AW_MAX_STAGES]
+
+  pdl_launch_dependents();
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+  const int qb = blockIdx.x, head = blockIdx.y, b = blockIdx.z;
+  const int n_tiles = (p.Nkv + AW_BKV - 1) / AW_BKV;
+
+  if (threadIdx.x == 0) {
+    mbar_init(q_full, 1);
+    for (int s = 0; s < AW_MAX_STAGES; ++s) {
+      mbar_init(&kv_full[s], 1);
+      mbar_init(&kv_empty[s], AW_WARPS);
+    }
+    fence_mbar_init();
+    tma_prefetch_desc(&tmQ);
+    tma_prefetch_desc(&tmK);
+    tma_prefetch_desc(&tmV);
+  }
+  __syncthreads();
+
+  // K and V of tile t into its stage t % stages (thread 0)
+  auto load_tile = [&](int t) {
+    const int st = t % p.stages;
+    uint8_t* sK = sKV + st * kv_stage_bytes;
+    uint8_t* sV = sK + k_bytes;
+    mbar_expect_tx(&kv_full[st], (uint32_t)kv_stage_bytes);
+    for (int a = 0; a < p.nd; ++a) tma_load_4d(sK + a * AW_KBOX, &tmK, &kv_full[st], a * 64, head, t * AW_BKV, b);
+    for (int c = 0; c < AW_NV; ++c) tma_load_4d(sV + c * AW_VBOX, &tmV, &kv_full[st], c * 16, head, t * AW_BKV, b);
+  };
+  pdl_wait();
+  if (threadIdx.x == 0) {
+    mbar_expect_tx(q_full, (uint32_t)q_bytes);
+    for (int a = 0; a < p.nd; ++a) tma_load_4d(sQ + a * AW_QBOX, &tmQ, q_full, a * 64, head, qb * AW_BQ, b);
+    for (int t = 0; t < p.stages; ++t) load_tile(t);
+  }
+  __syncwarp();
+  const int wg = warp >> 2, wq = warp & 3;
+  const int g = lane >> 2, t4 = lane & 3;
+  // accumulator layout (ea_wgmma.cuh): rows wq * 16 + g (i % 4 < 2) and + 8 (i % 4 >= 2) of the CTA's 64
+  const int q_lo = qb * AW_BQ + wq * 16 + g, q_hi = q_lo + 8;
+  const uint64_t dQ0 = gmma_desc_k_sw128(smem_u32(sQ), 1024);
+  const uint64_t dK0 = gmma_desc_k_sw128(smem_u32(sKV), 1024);
+  // warp-group g multiplies by V columns 256 g .. : its first V box is 16 g
+  const uint64_t dV0 = gmma_desc_mn_sw32(smem_u32(sKV) + (uint32_t)(k_bytes + wg * 16 * AW_VBOX), AW_VBOX, 256);
+  const uint32_t kv_stage16 = (uint32_t)kv_stage_bytes >> 4;
+  const float sc = p.scale_log2;
+  const bool ragged = p.Nkv % AW_BKV != 0;
+
+  float o[AW_DO / 4];
+#pragma unroll
+  for (int i = 0; i < AW_DO / 4; ++i) o[i] = 0.f;
+  float s[AW_BKV / 2];
+  uint32_t pa[AW_BKV / 16][4];
+  float m_lo = -INFINITY, m_hi = -INFINITY;   // running max in the scaled log2 domain
+  float l_lo = 0.f, l_hi = 0.f;               // this thread's share of the running sum
+  float a_lo = 0.f, a_hi = 0.f;               // rescale factor of O for the latest tile
+
+  // S = Q K^T over the keys of stage st.  K-step ks sits at box (ks >> 2), +32 B * (ks & 3)
+  auto issue_s = [&](int st) {
+    uint64_t dq = dQ0, dk = dK0 + (uint64_t)(st * kv_stage16);
+    Wgmma<AW_BKV>::ss(s, dq, dk, 0u);
+    for (int ks = 1; ks < p.ksteps; ++ks) {
+      const bool next_box = (ks & 3) == 0;
+      dq += next_box ? (uint64_t)((AW_QBOX >> 4) - 6) : 2u;
+      dk += next_box ? (uint64_t)((AW_KBOX >> 4) - 6) : 2u;
+      Wgmma<AW_BKV>::ss(s, dq, dk, 1u);
+    }
+    wgmma_commit();
+  };
+  // O += P V ; V K-step kk = 16 key rows = +512 B of every 16-column box
+  auto issue_pv = [&](int st) {
+    const uint64_t dv = dV0 + (uint64_t)(st * kv_stage16);
+#pragma unroll
+    for (int kk = 0; kk < AW_BKV / 16; ++kk)
+      Wgmma<AW_DO / 2>::rs(o, pa[kk], dv + (uint64_t)(kk * ((16 * 32) >> 4)), 1u);
+    wgmma_commit();
+  };
+  auto wait_pv = [&]() {
+    wgmma_wait<0>();
+    wgmma_fence_regs(o);
+    wgmma_fence_regs_u32(pa);
+  };
+  auto release = [&](int st) {
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&kv_empty[st]);
+  };
+  // S of tile t -> exponentials in place; updates m, l and sets the O rescale factors a_lo / a_hi
+  auto softmax = [&](int t) {
+    if (ragged && t == n_tiles - 1) {
+      const int valid = p.Nkv - t * AW_BKV;   // keys of this tile that exist (>= 1)
+#pragma unroll
+      for (int i = 0; i < AW_BKV / 2; ++i)
+        if (8 * (i >> 2) + 2 * t4 + (i & 1) >= valid) s[i] = -INFINITY;
+    }
+    float mx_lo = -INFINITY, mx_hi = -INFINITY;
+#pragma unroll
+    for (int i = 0; i < AW_BKV / 2; i += 4) {
+      mx_lo = fmaxf(mx_lo, fmaxf(s[i], s[i + 1]));
+      mx_hi = fmaxf(mx_hi, fmaxf(s[i + 2], s[i + 3]));
+    }
+    mx_lo = fmaxf(mx_lo, __shfl_xor_sync(0xffffffffu, mx_lo, 1));
+    mx_lo = fmaxf(mx_lo, __shfl_xor_sync(0xffffffffu, mx_lo, 2));
+    mx_hi = fmaxf(mx_hi, __shfl_xor_sync(0xffffffffu, mx_hi, 1));
+    mx_hi = fmaxf(mx_hi, __shfl_xor_sync(0xffffffffu, mx_hi, 2));
+    // sc > 0, so the max of the scaled logits is the scaled max
+    const float mn_lo = fmaxf(m_lo, mx_lo * sc), mn_hi = fmaxf(m_hi, mx_hi * sc);
+    a_lo = mufu_ex2(m_lo - mn_lo);   // 0 on the first tile
+    a_hi = mufu_ex2(m_hi - mn_hi);
+    m_lo = mn_lo;
+    m_hi = mn_hi;
+    float sum_lo = 0.f, sum_hi = 0.f;
+#pragma unroll
+    for (int i = 0; i < AW_BKV / 2; i += 4) {
+      s[i] = mufu_ex2(fmaf(s[i], sc, -mn_lo));
+      s[i + 1] = mufu_ex2(fmaf(s[i + 1], sc, -mn_lo));
+      s[i + 2] = mufu_ex2(fmaf(s[i + 2], sc, -mn_hi));
+      s[i + 3] = mufu_ex2(fmaf(s[i + 3], sc, -mn_hi));
+      sum_lo += s[i] + s[i + 1];
+      sum_hi += s[i + 2] + s[i + 3];
+    }
+    l_lo = fmaf(l_lo, a_lo, sum_lo);
+    l_hi = fmaf(l_hi, a_hi, sum_hi);
+  };
+  auto rescale_and_pack = [&]() {
+#pragma unroll
+    for (int i = 0; i < AW_DO / 4; ++i) o[i] *= ((i >> 1) & 1) ? a_hi : a_lo;
+#pragma unroll
+    for (int kk = 0; kk < AW_BKV / 16; ++kk)
+#pragma unroll
+      for (int h = 0; h < 4; ++h) pa[kk][h] = ea_pack2(s[8 * kk + 2 * h], s[8 * kk + 2 * h + 1]);
+  };
+
+  mbar_wait(q_full, 0);
+  int stage = 0;
+  uint32_t phase = 0;
+  mbar_wait(&kv_full[0], 0);
+  wgmma_fence();
+  issue_s(0);
+  wgmma_wait<0>();
+  wgmma_fence_regs(s);
+  softmax(0);
+  rescale_and_pack();
+  for (int j = 1; j < n_tiles; ++j) {
+    const int prev = stage;
+    if (++stage == p.stages) { stage = 0; phase ^= 1u; }
+    mbar_wait(&kv_full[stage], phase);
+    wgmma_fence();
+    issue_s(stage);
+    issue_pv(prev);
+    wgmma_wait<1>();
+    wgmma_fence_regs(s);
+    softmax(j);
+    wait_pv();
+    release(prev);
+    // tile j - 1 + stages goes where tile j - 1 was, once every warp has released it (the empty barrier's
+    // ((j - 1) / stages)-th phase)
+    if (threadIdx.x == 0 && j - 1 + p.stages < n_tiles) {
+      mbar_wait(&kv_empty[prev], (uint32_t)(((j - 1) / p.stages) & 1));
+      load_tile(j - 1 + p.stages);
+    }
+    __syncwarp();
+    rescale_and_pack();
+  }
+  wgmma_fence();
+  issue_pv(stage);
+  wait_pv();
+
+  // ---- epilogue: O / l
+  l_lo += __shfl_xor_sync(0xffffffffu, l_lo, 1);
+  l_lo += __shfl_xor_sync(0xffffffffu, l_lo, 2);
+  l_hi += __shfl_xor_sync(0xffffffffu, l_hi, 1);
+  l_hi += __shfl_xor_sync(0xffffffffu, l_hi, 2);
+  const float inv_lo = 1.f / l_lo, inv_hi = 1.f / l_hi;
+  ea_half* orow_lo = p.out + (long long)b * p.o_bs + (long long)q_lo * p.o_ns + (long long)head * p.d;
+  ea_half* orow_hi = orow_lo + 8 * p.o_ns;
+#pragma unroll
+  for (int i = 0; i < AW_DO / 4; i += 4) {
+    const int col = wg * (AW_DO / 2) + 8 * (i >> 2) + 2 * t4;
+    if (col < p.d) {
+      if (q_lo < p.Nq) *reinterpret_cast<uint32_t*>(orow_lo + col) = ea_pack2(o[i] * inv_lo, o[i + 1] * inv_lo);
+      if (q_hi < p.Nq) *reinterpret_cast<uint32_t*>(orow_hi + col) = ea_pack2(o[i + 2] * inv_hi, o[i + 3] * inv_hi);
+    }
+  }
+}
+
+// [B, N, heads, d] with strides (bs, ns, d) elements; boxes of `box_cols` head-dim columns x `box_rows` rows
 static int encode_qkv(CUtensorMap* m, const void* base, int d, int heads, int N, int B,
-                      long long ns, long long bs, int box_cols, CUtensorMapSwizzle swizzle) {
+                      long long ns, long long bs, int box_cols, CUtensorMapSwizzle swizzle, int box_rows = 128) {
   cuuint64_t dims[4] = {(cuuint64_t)d, (cuuint64_t)heads, (cuuint64_t)N, (cuuint64_t)B};
   cuuint64_t strides[3] = {(cuuint64_t)d * 2, (cuuint64_t)ns * 2, (cuuint64_t)bs * 2};
-  cuuint32_t box[4] = {(cuuint32_t)box_cols, 1, 128, 1};
+  cuuint32_t box[4] = {(cuuint32_t)box_cols, 1, (cuuint32_t)box_rows, 1};
   cuuint32_t estr[4] = {1, 1, 1, 1};
   CUresult r = ea_tmap_encode()(m, EA_TMAP_DTYPE, 4, const_cast<void*>(base), dims, strides, box,
                                 estr, CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle,
@@ -390,6 +624,40 @@ static int attn_pv_width(int d) {
   return d <= 48 ? 48 : d <= 64 ? 64 : d <= 80 ? 80 : d <= 160 ? 160 : 192;
 }
 
+// 192 < d <= 512, no bias
+static int launch_attn_wide(const ea_attn_args* a, AttnKParams& p, cudaStream_t stream) {
+  const int budget = 227 * 1024 - 1024 - 256;
+  const int q_bytes = p.nd * AW_QBOX;
+  const int stage_bytes = p.nd * AW_KBOX + AW_NV * AW_VBOX;
+  int stages = (budget - q_bytes) / stage_bytes;
+  if (stages > AW_MAX_STAGES) stages = AW_MAX_STAGES;
+  const int n_tiles = (a->Nkv + AW_BKV - 1) / AW_BKV;
+  if (stages > n_tiles) stages = n_tiles;
+  p.stages = stages;
+
+  CUtensorMap tq, tk, tv;
+  if (encode_qkv(&tq, a->q, a->d, a->heads, a->Nq, a->B, a->q_ns, a->q_bs, 64, CU_TENSOR_MAP_SWIZZLE_128B, AW_BQ))
+    return EA_ERR_TMAP;
+  if (encode_qkv(&tk, a->k, a->d, a->heads, a->Nkv, a->B, a->k_ns, a->k_bs, 64, CU_TENSOR_MAP_SWIZZLE_128B, AW_BKV))
+    return EA_ERR_TMAP;
+  if (encode_qkv(&tv, a->v, a->d, a->heads, a->Nkv, a->B, a->v_ns, a->v_bs, 16, CU_TENSOR_MAP_SWIZZLE_32B, AW_BKV))
+    return EA_ERR_TMAP;
+
+  const int smem_bytes = q_bytes + stages * stage_bytes + (1 + 2 * AW_MAX_STAGES) * 8 + 1024;
+  static int max_set_dev[EA_MAX_DEV];
+  int& max_set = max_set_dev[ea_dev()];
+  if (smem_bytes > max_set) {
+    const cudaError_t e = cudaFuncSetAttribute(ea_attn_wide_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                               smem_bytes);
+    if (e != cudaSuccess) return ea_cuda_fail(e, "ea_attention: cudaFuncSetAttribute(MaxDynamicSharedMemorySize)");
+    max_set = smem_bytes;
+  }
+  dim3 grid((unsigned)((a->Nq + AW_BQ - 1) / AW_BQ), (unsigned)a->heads, (unsigned)a->B);
+  const cudaError_t e = ea_launch(ea_attn_wide_kernel, grid, dim3(AW_THREADS), (size_t)smem_bytes, stream,
+                                  tq, tk, tv, p);
+  return e == cudaSuccess ? 0 : ea_cuda_fail(e, "ea_attention: kernel launch");
+}
+
 }  // namespace ea
 
 using namespace ea;
@@ -397,7 +665,7 @@ using namespace ea;
 extern "C" int ea_attention(const ea_attn_args* a, void* stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   if (!a || !a->q || !a->k || !a->v || !a->out) return EA_ERR_ARG;
-  if (a->d % 8 != 0 || a->d < 8 || a->d > 192) return EA_ERR_SHAPE;
+  if (a->d % 8 != 0 || a->d < 8 || a->d > AW_DO) return EA_ERR_SHAPE;
   if (a->Nq <= 0 || a->Nkv <= 0 || a->B <= 0 || a->heads <= 0) return EA_ERR_SHAPE;
   if (a->q_ns % 8 || a->k_ns % 8 || a->v_ns % 8 || a->q_bs % 8 || a->k_bs % 8 || a->v_bs % 8 ||
       a->o_ns % 8 || a->o_bs % 8)
@@ -419,6 +687,14 @@ extern "C" int ea_attention(const ea_attn_args* a, void* stream_) {
   p.rel_h = a->rel_h; p.rel_w = a->rel_w; p.rel_s = a->rel_s;
 
   const bool bias = a->rel_h != nullptr;
+  if (a->d > 192) {
+    if (bias) return EA_ERR_SHAPE;   // the wide kernel has no rel-pos bias terms
+    const int st = launch_attn_wide(a, p, stream);
+    if (st) return st;
+    ea_count_launch();
+    const cudaError_t e = cudaGetLastError();
+    return e == cudaSuccess ? 0 : ea_cuda_fail(e, "ea_attention: after the kernel launch");
+  }
   const int dv = attn_pv_width(a->d);
   const int budget = 227 * 1024 - 1024 - 256;
   // 64-bit: rel_w rows of a huge rel_s must not wrap around and pass as a small shared-memory footprint

@@ -16,9 +16,11 @@ and, for the encode side (`prepare_masked_image_latents`, utils/...inpaint.py:10
     DiagonalGaussianDistribution  ldm/modules/distributions/distributions.py:24-45  mean, logvar.clamp(-30, 20)
 Execution: channels-last half activations, fp32 accumulation; every 3x3 convolution is the wgmma
 implicit GEMM (ea_gemm CONV_S1), the 1x1 shortcut of a channel-changing ResnetBlock rides along as extra
-K columns of conv2, GroupNorm + swish is one fused launch, and the single-head d = 512 attention is two
-plain GEMMs around a row-softmax kernel (fp32 logits).  The last convolution (128 -> 3) is padded to 8
-output channels so it can use the same GEMM; `ea_image_out` drops the padding, applies
+K columns of conv2, GroupNorm + swish is one fused launch, and the single-head attention (d = C, 512 in the
+SD VAE) is, above FUSED_ATTN_MIN_TOKENS tokens, one q|k|v GEMM and one ea_attention launch over all images, so
+the N x N logits are never stored; shorter sequences run two plain GEMMs around a row-softmax kernel (fp32 logits).
+The last convolution (128 -> 3) is padded to 8 output channels so it can use the same GEMM; `ea_image_out`
+drops the padding, applies
 (x / 2 + 0.5).clamp(0, 1) and writes the fp32 NCHW image the pipeline hands to numpy / PIL.
 """
 import types
@@ -31,6 +33,13 @@ from . import _lib as L
 from ._backend import default_ops, engine_call
 from ._graphs import GraphLRU
 from .vae_spec import SD_VAE, VAE_TINY, VaeConfig, decoder_blocks, encoder_blocks, make_vae_state_dict  # noqa: F401
+
+
+# AttnBlock sequence lengths up to this run the logits as GEMMs around a row softmax, longer ones run ea_attention.
+# On an H100 80GB HBM3 (700 W) at C = 512 the fused kernel took 2.1-2.2x the GEMM sequence's time at 64 x 64 latents
+# (N = 4096: 64 CTAs of 64 query rows fill half the SMs), 1.04-1.06x at 128 x 128 and 0.91x at 192 x 256, while the
+# GEMM sequence stores 6 N^2 bytes of logits (1.6 GB at N = 16384, 46.5 GB at 256 x 344).
+FUSED_ATTN_MIN_TOKENS = 128 * 128
 
 
 def _conv3_pack(w):  # [Cout, Cin, 3, 3] -> [Cout, (kh, kw, Cin)]
@@ -65,11 +74,8 @@ class _VaeBase:
             elif kind == "attn":
                 w[p + ".norm.g"], w[p + ".norm.b"] = F(sd[p + ".norm.weight"]), F(sd[p + ".norm.bias"])
                 c = cin
-                qk = torch.cat([sd[p + ".q.weight"].reshape(c, c), sd[p + ".k.weight"].reshape(c, c)], 0)
-                w[p + ".qk.w"], w[p + ".qk.b"] = H(qk), F(torch.cat([sd[p + ".q.bias"], sd[p + ".k.bias"]]))
-                w[p + ".v.w"] = H(sd[p + ".v.weight"].reshape(c, c))
-                # softmax rows sum to 1, so v's bias passes straight through the attention: P (V + 1 b^T) = P V + b^T
-                w[p + ".v.b"] = F(sd[p + ".v.bias"])
+                qkv = torch.cat([sd[f"{p}.{n}.weight"].reshape(c, c) for n in "qkv"], 0)
+                w[p + ".qkv.w"], w[p + ".qkv.b"] = H(qkv), F(torch.cat([sd[f"{p}.{n}.bias"] for n in "qkv"]))
                 w[p + ".proj.w"], w[p + ".proj.b"] = H(sd[p + ".proj_out.weight"].reshape(c, c)), F(sd[p + ".proj_out.bias"])
             else:   # upsample.conv / downsample.conv
                 w[p + ".conv.w"], w[p + ".conv.b"] = H(_conv3_pack(sd[p + ".conv.weight"])), F(sd[p + ".conv.bias"])
@@ -135,20 +141,33 @@ class _VaeBase:
         o, w = self.ops, self.w
         N = H * W_
         hn = self._gn(x, w[p + ".norm.g"], w[p + ".norm.b"], B, N, c, False)
-        qk = self._new(B * N, 2 * c)
-        o.gemm(hn, w[p + ".qk.w"], qk, bias=w[p + ".qk.b"])
+        qkv_w, qkv_b = w[p + ".qkv.w"], w[p + ".qkv.b"]
+        if N <= FUSED_ATTN_MIN_TOKENS:
+            # the logits as plain GEMMs around a row softmax, one image at a time
+            qk = self._new(B * N, 2 * c)
+            o.gemm(hn, qkv_w[:2 * c], qk, bias=qkv_b[:2 * c])
+            out = self._new(B * N, c)
+            s = self._new(N, N, dtype=torch.float32)
+            pr = self._new(N, N)
+            vt = self._new(c, N)
+            ao = self._new(N, c)
+            for b in range(B):
+                rows = slice(b * N, (b + 1) * N)
+                o.gemm(qk[rows, :c], qk[rows, c:], out_f32=s, K=c, lda=2 * c, ldw=2 * c, out_scale=float(c) ** -0.5)
+                o.softmax_rows(s, pr, rows=N, cols=N)
+                o.gemm(qkv_w[2 * c:], hn[rows], vt)                                  # V^T = Wv hn^T   [c, N]
+                # softmax rows sum to 1, so v's bias passes straight through: P (V + 1 b^T) = P V + b^T
+                o.gemm(pr, vt, ao, bias=qkv_b[2 * c:])
+                o.gemm(ao, w[p + ".proj.w"], out[rows], bias=w[p + ".proj.b"], residual=x[rows])
+            return out
+        qkv = self._new(B * N, 3 * c)
+        o.gemm(hn, qkv_w, qkv, bias=qkv_b)
+        ao = self._new(B * N, c)
+        st = (N * 3 * c, 3 * c)                              # one head of d = c per image
+        o.attention(qkv, qkv[:, c:], qkv[:, 2 * c:], ao, B=B, heads=1, Nq=N, Nkv=N, d=c, q_strides=st,
+                    k_strides=st, v_strides=st, o_strides=(N * c, c), scale=float(c) ** -0.5)
         out = self._new(B * N, c)
-        s = self._new(N, N, dtype=torch.float32)
-        pr = self._new(N, N)
-        vt = self._new(c, N)
-        ao = self._new(N, c)
-        for b in range(B):                                   # one head per image: plain GEMMs
-            rows = slice(b * N, (b + 1) * N)
-            o.gemm(qk[rows, :c], qk[rows, c:], out_f32=s, K=c, lda=2 * c, ldw=2 * c, out_scale=float(c) ** -0.5)
-            o.softmax_rows(s, pr, rows=N, cols=N)
-            o.gemm(w[p + ".v.w"], hn[rows], vt)                                  # V^T = Wv hn^T   [c, N]
-            o.gemm(pr, vt, ao, bias=w[p + ".v.b"])                               # P V + b_v
-            o.gemm(ao, w[p + ".proj.w"], out[rows], bias=w[p + ".proj.b"], residual=x[rows])
+        o.gemm(ao, w[p + ".proj.w"], out, bias=w[p + ".proj.b"], residual=x)
         return out
 
 

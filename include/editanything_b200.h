@@ -162,10 +162,13 @@ int ea_gemm_plan(int m_tiles, int N, int k_blocks, int act, long long workspace_
  * Replaces CrossAttention.forward core  ldm/modules/attention.py:170-193 (QK^T in fp32,
  * softmax, PV) and SAM Attention.forward (decomposed rel-pos, SURVEY.md App. C).
  * q: [B, Nq, heads, d] with strides (q_bs, q_ns, d) elements; k, v likewise with Nkv rows;
- * out: [B, Nq, heads*d] contiguous rows of stride o_ns.  d % 8 == 0, d <= 192.  scale > 0 (finite).
+ * out: [B, Nq, heads*d] contiguous rows of stride o_ns.  d % 8 == 0, d <= 512 (EA_ERR_SHAPE above, before any
+ * launch); d <= 192 runs 128-row query tiles, 192 < d <= 512 (the VAE AttnBlock's one head of 512) a kernel of
+ * 64-row query tiles and 32-key K / V tiles.  scale > 0 (finite).
  * rel_h / rel_w (optional, fp32 [B*heads, Nq, rel_s]): bias[q, kk] = rel_h[q, kk / rel_s] +
  * rel_w[q, kk % rel_s] added to the scaled logits (SAM add_decomposed_rel_pos).  With them, Nkv <= rel_s * rel_s
- * (else EA_ERR_SHAPE), and 128 rows of rel_w must fit in shared memory next to the K / V tiles.
+ * (else EA_ERR_SHAPE), and 128 rows of rel_w must fit in shared memory next to the K / V tiles; d > 192 with them
+ * is EA_ERR_SHAPE.
  */
 typedef struct ea_attn_args {
   const void* q; const void* k; const void* v; void* out;
@@ -319,9 +322,7 @@ int ea_nhwc_to_nchw_f32(const void* x, float* out, int B, int HW, int C, void* s
 
 /* ---- VAE decoder helpers (SURVEY.md 8f row N1; reference ldm/modules/diffusionmodules/model.py) ----
  * ea_softmax_rows: p[r, :] = softmax(s[r, :]) for fp32 logits [rows, cols] (row stride lds) -> half
- *   [rows, cols] (row stride ldp); cols % 4 == 0.  The VAE AttnBlock (model.py:181-210) is single-head
- *   with d = C = 512: its logits come from ea_gemm (fp32 output, scale C^-0.5 in the epilogue), this
- *   kernel normalises them, a second ea_gemm applies them to V.
+ *   [rows, cols] (row stride ldp); cols % 4 == 0.  (The VAE AttnBlock now runs on ea_attention.)
  * ea_image_out: half NHWC rows of width ldx (first C channels used) -> fp32 NCHW [B, C, HW],
  *   out = clamp(x * scale + shift, lo, hi): decode_latents' (image / 2 + 0.5).clamp(0, 1)
  *   (utils/stable_diffusion_controlnet_inpaint.py:718-724) fused with the layout change. */
