@@ -50,8 +50,14 @@ Like the reference, a rebuild of the generation pipeline for another ControlNet 
 at weight 1.0: it does not pass `lora_weight` on (editany_lora.py:660-666).  `load_lora_weights(pipe, path,
 multiplier, device, dtype)` merges further files into a built pipeline.
 
+All-region generation (`process(..., enable_all_generate=True)` with no `mask_image`, the demos' third tab) follows
+editany_lora.py:658-676 and :796-812: the generation pipeline is rebuilt for the mode (sharing the packed UNet, VAE
+and text encoder of the current one when the LoRA lists match), the mask is all white, and with `extra_inpaint` the
+text-to-image `StableDiffusionControlNetPipeline` runs with the SAM ControlNet alone; without it the inpaint pipeline
+repaints the whole image.  The tile pass then runs as usual.
+
 Not supported here (raise NotImplementedError instead of diverging silently): reference-only mode (`ref_image`),
-`enable_all_generate` (the text-to-image ControlNet pipeline), the alpha-mixing pipeline.
+the alpha-mixing pipeline.
 """
 import copy
 import os
@@ -142,18 +148,21 @@ def load_lora_weights(pipeline, checkpoint_path, multiplier, device, dtype):
 
 
 def obtain_generation_model(base_model_path, lora_model_path, controlnet_path, generation_only=False,
-                            extra_inpaint=True, lora_weight=1.0):
-    """editany_lora.py:343-388: SAM-ControlNet (+ inpaint-ControlNet) pipeline with the UniPC scheduler."""
-    from .pipeline import ControlNetModel, ControlNetModel2, StableDiffusionControlNetInpaintPipeline
+                            extra_inpaint=True, lora_weight=1.0, share_with=None):
+    """editany_lora.py:343-388: SAM-ControlNet (+ inpaint-ControlNet) pipeline with the UniPC scheduler; for
+    all-region generation with `extra_inpaint` (generation_only=True) the text-to-image pipeline with the SAM
+    ControlNet alone.  `share_with`: a pipeline of the same base model whose packed UNet, VAE and text encoder are
+    reused (StableDiffusionControlNetInpaintPipeline.from_pretrained)."""
+    from .pipeline import (ControlNetModel, ControlNetModel2, StableDiffusionControlNetInpaintPipeline,
+                           StableDiffusionControlNetPipeline)
     from .schedulers import UniPCMultistepScheduler
-    if generation_only and extra_inpaint:
-        raise NotImplementedError("enable_all_generate: the text-to-image ControlNet pipeline is outside the hot path")
     controlnet = [ControlNetModel2.from_pretrained(controlnet_path, torch_dtype=torch.float16)]
     if (not generation_only) and extra_inpaint:
         controlnet.append(ControlNetModel.from_pretrained(INPAINT_CONTROLNET, torch_dtype=torch.float16))
-    pipe = StableDiffusionControlNetInpaintPipeline.from_pretrained(base_model_path, controlnet=controlnet,
-                                                                   torch_dtype=torch.float16, safety_checker=None,
-                                                                   lora=_lora_list(lora_model_path, lora_weight))
+    cls = StableDiffusionControlNetPipeline if generation_only and extra_inpaint else \
+        StableDiffusionControlNetInpaintPipeline
+    pipe = cls.from_pretrained(base_model_path, controlnet=controlnet, torch_dtype=torch.float16, safety_checker=None,
+                               share_with=share_with, lora=_lora_list(lora_model_path, lora_weight))
     pipe.scheduler = UniPCMultistepScheduler.from_config(pipe.scheduler.config)
     pipe.enable_xformers_memory_efficient_attention()
     pipe.enable_model_cpu_offload()
@@ -265,12 +274,17 @@ class EditAnythingLoraModel:
         """editany_lora.py:609-938 -> (results_tile: list[PIL], results: list[PIL], [full_segmask, mask], prompt)."""
         if ref_image is not None:
             raise NotImplementedError("reference-only mode (utils/stable_diffusion_reference.py) is not implemented")
-        if enable_all_generate:
-            raise NotImplementedError("enable_all_generate: the text-to-image ControlNet pipeline is outside the hot path")
         this_controlnet_path = self.default_controlnet_path if condition_model in (None, "EditAnything") else condition_model
         input_image = source_image["image"] if isinstance(source_image, dict) else np.array(source_image, dtype=np.uint8)
         if mask_image is None:
-            mask_image = source_image["mask"]
+            if enable_all_generate != self.defalut_enable_all_generate:     # :658-667 (lora_weight not passed, sic)
+                self.pipe = obtain_generation_model(self.base_model_path, self.lora_model_path, this_controlnet_path,
+                                                    enable_all_generate, self.extra_inpaint, share_with=self.pipe)
+                self.defalut_enable_all_generate = enable_all_generate
+            if enable_all_generate:
+                mask_image = np.ones((input_image.shape[0], input_image.shape[1], 3)) * 255
+            else:
+                mask_image = source_image["mask"]
         else:
             mask_image = np.array(mask_image, dtype=np.uint8)
         if self.default_controlnet_path != this_controlnet_path:          # :679-696
@@ -304,18 +318,25 @@ class EditAnythingLoraModel:
         postive_prompt, negative_prompt = a_prompt, n_prompt            # (sic)
         prompt_embeds, negative_prompt_embeds = get_pipeline_embeds(self.pipe, postive_prompt, negative_prompt, dev)
 
-        multi_condition_image = [control.type(torch.float16)]
-        multi_condition_scale = [float(control_scale)]
-        if self.extra_inpaint:
-            multi_condition_image.append(make_inpaint_condition(img, mask_image_tmp).type(torch.float16))
-            multi_condition_scale.append(1.0)
-        # use_scale_map: the reference builds the map (:838-848) but hands it only to the alpha-mixing pipeline
-        x_samples = self.pipe(image=img, mask_image=mask_image, prompt_embeds=prompt_embeds,
-                              negative_prompt_embeds=negative_prompt_embeds, num_images_per_prompt=num_samples,
-                              num_inference_steps=ddim_steps, generator=generator,
-                              controlnet_conditioning_image=multi_condition_image, height=H, width=W,
-                              controlnet_conditioning_scale=multi_condition_scale, guidance_scale=scale,
-                              guess_mode=guess_mode).images
+        if enable_all_generate and self.extra_inpaint:                    # :796-812, the text-to-image pipeline
+            x_samples = self.pipe(prompt_embeds=prompt_embeds, negative_prompt_embeds=negative_prompt_embeds,
+                                  num_images_per_prompt=num_samples, num_inference_steps=ddim_steps,
+                                  generator=generator, height=H, width=W, image=[control.type(torch.float16)],
+                                  controlnet_conditioning_scale=[float(control_scale)], guidance_scale=scale,
+                                  guess_mode=guess_mode).images
+        else:
+            multi_condition_image = [control.type(torch.float16)]
+            multi_condition_scale = [float(control_scale)]
+            if self.extra_inpaint:
+                multi_condition_image.append(make_inpaint_condition(img, mask_image_tmp).type(torch.float16))
+                multi_condition_scale.append(1.0)
+            # use_scale_map: the reference builds the map (:838-848) but hands it only to the alpha-mixing pipeline
+            x_samples = self.pipe(image=img, mask_image=mask_image, prompt_embeds=prompt_embeds,
+                                  negative_prompt_embeds=negative_prompt_embeds, num_images_per_prompt=num_samples,
+                                  num_inference_steps=ddim_steps, generator=generator,
+                                  controlnet_conditioning_image=multi_condition_image, height=H, width=W,
+                                  controlnet_conditioning_scale=multi_condition_scale, guidance_scale=scale,
+                                  guess_mode=guess_mode).images
         results = [x_samples[i] for i in range(num_samples)]
 
         results_tile = []

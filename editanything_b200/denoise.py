@@ -115,17 +115,32 @@ class DenoiseEngine:
         return out
 
     @engine_call
-    def prepare(self, ctx, hints, scales, guess_mode=False, cfg_duplicated=False, guided=True):
+    def prepare(self, ctx, hints, scales, guess_mode=False, cfg_duplicated=False, guided=True, controlnet_rows="all"):
         """ctx: [B, L, D] prompt embeddings ([negative; positive] stacked for CFG,
         utils/stable_diffusion_controlnet_inpaint.py:1339-1347); hints: list of NCHW conditioning
         images [B, 3, 8h, 8w] (un-normalised, editany_lora.py:771-778,814-828); scales: list.
         guided=False: sampling without classifier-free guidance (guidance scale <= 1, :1329): ctx and hints hold
-        the N images once (B = N), every step runs the networks on those rows and feeds their eps to the update."""
+        the N images once (B = N), every step runs the networks on those rows and feeds their eps to the update.
+        controlnet_rows="conditional" (guided requests only): the ControlNet residuals are added to the N conditional
+        rows and the unconditional rows run the UNet without control - the text-to-image pipeline's guess mode with
+        guidance (utils/stable_diffusion_controlnet.py:579-602).  The hints then hold the N images once.  The
+        ControlNets still run on all B rows; only their zero-convs skip the unconditional half."""
+        if controlnet_rows not in ("all", "conditional"):
+            raise ValueError(f"controlnet_rows must be 'all' or 'conditional', got {controlnet_rows!r}")
+        cond_rows = controlnet_rows == "conditional"
         if not guided and cfg_duplicated:
             raise ValueError("cfg_duplicated describes [x; x] conditioning images, which only guided sampling has")
+        if cond_rows and not guided:
+            raise ValueError("controlnet_rows='conditional' needs guided sampling: without guidance every row is "
+                             "conditional")
+        if cond_rows and any(torch.is_tensor(s) for s in scales):
+            raise NotImplementedError("controlnet_rows='conditional' with a spatial conditioning_scale map")
         ctx = ctx.to(self.dev)
         if guided and ctx.shape[0] % 2:
             raise ValueError(f"guided sampling stacks [negative; positive] prompt embeddings, got {ctx.shape[0]} rows")
+        if cond_rows and any(h.shape[0] * 2 != ctx.shape[0] for h in hints):
+            raise ValueError(f"controlnet_rows='conditional' takes the conditioning images of the "
+                             f"{ctx.shape[0] // 2} images once, got {[h.shape[0] for h in hints]} rows")
         if guided != getattr(self, "guided", None):
             self._graph = None        # the step's last launch differs (ea_out_cfg_ddim / ea_out_ddim)
         self.guided = bool(guided)
@@ -137,20 +152,24 @@ class DenoiseEngine:
         self._keep("ctx_cache", [n.precompute_context(ctx) for n in (nets[:1] if ls else nets)])
         self._keep("ctx_ls", self.runner.precompute_context_lockstep(ctx) if ls else None)
         # cfg_duplicated: the conditioning images are [x; x] (prepare_controlnet_conditioning_image doubles them for
-        # classifier-free guidance, utils/...inpaint.py:380-381) - run the hint stack on one half only
-        if cfg_duplicated and all(h.shape[0] % 2 == 0 for h in hints):
+        # classifier-free guidance, utils/...inpaint.py:380-381) - run the hint stack on one half only; conditional
+        # rows: the N images arrive once and are stacked the same way
+        if cond_rows or cfg_duplicated and all(h.shape[0] % 2 == 0 for h in hints):
             new_hints = []
             for c, h in zip(self.cns, hints):
-                g = c.precompute_hint(h[:h.shape[0] // 2].to(self.dev))
+                g = c.precompute_hint((h if cond_rows else h[:h.shape[0] // 2]).to(self.dev))
                 new_hints.append(torch.cat([g, g]))
         else:
             new_hints = [c.precompute_hint(h.to(self.dev)) for c, h in zip(self.cns, hints)]
         self._keep("hints", new_hints)
         lat_hw = (hints[0].shape[-2] // 8, hints[0].shape[-1] // 8) if len(hints) else (0, 0)
         new_scales = [self._norm_scale(s, guess_mode, self.B, lat_hw) for s in scales]
+        if cond_rows:                 # read by nets.UNetRunner._zero_convs
+            new_scales = [dict(s if isinstance(s, dict) else {"base": s, "per_res": None, "maps": None},
+                               rows="conditional") for s in new_scales]
         plain = all(not isinstance(s, dict) for s in new_scales)
         if not plain or getattr(self, "scales", None) != new_scales:
-            self._graph = None        # scales (and map addresses) are baked into the zero-conv launches
+            self._graph = None        # scales, map addresses and the rows written are baked into the zero-conv launches
         self.scales = new_scales
         if not hasattr(self, "t_dev") or self.t_dev.shape[0] != self.B:
             self._emb_cache = {}

@@ -502,15 +502,21 @@ class UNetRunner:
 
     def _zero_convs(self, R, h, i, slot, scales, deferred):
         """slot += scale * zero_conv_i(h) for every ControlNet of R (i = None: middle_block_out), or the same GEMMs
-        appended to `deferred` as (a, w, out, kwargs)."""
+        appended to `deferred` as (a, w, out, kwargs).  A net whose scale asks for the conditional rows only
+        (DenoiseEngine.prepare(controlnet_rows="conditional")) adds its residual to rows [B/2, B) of the slot and
+        leaves the unconditional rows untouched: cat([zeros_like(d), d]) (utils/stable_diffusion_controlnet.py:
+        579-602)."""
         c = h.shape[-1]
-        M = h.shape[0] // R.n * h.shape[1] * h.shape[2]
         p = "mid_out" if i is None else f"zero_convs.{i}.0"
         for g, nt in enumerate(R.nets):
             if nt.kind == "unet":
                 continue
             f, rs = self.zc_scale(scales[g], i, h.shape)
-            call = (h.chunk(R.n, 0)[g].reshape(M, c), nt.w[p + ".w"], slot,
+            a, out = h.chunk(R.n, 0)[g], slot
+            if self.conditional_rows(scales[g]):
+                a, out = self.conditional_half(a), self.conditional_half(slot)
+            M = a.shape[0] * a.shape[1] * a.shape[2]
+            call = (a.reshape(M, c), nt.w[p + ".w"], out,
                     dict(M=M, bias=nt.w[p + ".b"], out_scale=f, row_scale=rs, accumulate=True, ldo=slot.stride(2)))
             if deferred is not None:
                 deferred.append(call)
@@ -531,6 +537,22 @@ class UNetRunner:
         if scale.get("maps") is not None:
             rs = scale["maps"][(shape[1], shape[2])]
         return f, rs
+
+    @staticmethod
+    def conditional_rows(scale):
+        return isinstance(scale, dict) and scale.get("rows") == "conditional"
+
+    @staticmethod
+    def conditional_half(t):
+        """Rows [B/2, B) of an NHWC tensor or slot view, as a view with the same strides.  The GEMM reads and writes
+        it through TMA, whose base addresses must be 16-byte aligned: checked here, on the host."""
+        if t.shape[0] % 2:
+            raise ValueError(f"conditional rows need an even batch of [unconditional; conditional] rows, got {t.shape[0]}")
+        v = t[t.shape[0] // 2:]
+        if v.data_ptr() % 16:
+            raise ValueError(f"the conditional rows of a {tuple(t.shape)} tensor start at byte offset "
+                             f"{v.data_ptr() - t.data_ptr()}, which is not a multiple of 16")
+        return v
 
     def precompute_context_lockstep(self, ctx):
         """Cross-attention K/V of the encoder + middle attention layers of every network, stacked along the batch
@@ -594,6 +616,14 @@ class UNetRunner:
         if gn_ws is None:
             gn_ws = o.gn_workspace(B, self.dev)
         sinks = self.alloc_sinks(B, H, W_)
+        if any(self.conditional_rows(s) for s in scales):
+            # every offset view the conditional-rows zero-convs will take, checked before the first launch: the
+            # slots, and the ControlNet activations (fresh allocations shaped like the slots' channel part)
+            for s in sinks["skip"] + [sinks["mid"]]:
+                self.conditional_half(s)
+                if (B // 2) * s.shape[1] * s.shape[2] * s.shape[3] * s.element_size() % 16:
+                    raise ValueError(f"the conditional rows of a [{B}, {s.shape[1]}, {s.shape[2]}, {s.shape[3]}] "
+                                     "activation do not start at a 16-byte boundary")
         if embs is None:
             embs = self.compute_embs(t_dev, B)
         n = 1 + len(self.cns)

@@ -26,8 +26,16 @@ checkpoint's scheduler/scheduler_config.json into `DDIMScheduler`, `UniPCMultist
 over, and the fused step converts the guidance-combined v to x0 and eps like the reference sampler
 (cldm/ddim_hacked.py:190-217).  Any other scheduler object receives the combined network output in its `step`.
 
+Guess mode runs as in the reference: the ControlNet residuals are weighted logspace(-1, 0, 13); the inpaint pipeline
+adds them to both guidance halves (:1607-1615).
+
+`StableDiffusionControlNetPipeline` and `StableDiffusionControlNetPipeline2` (bottom of this file) are the
+text-to-image pipelines of all-region generation, sam2image.py and sketch2image.py on the same engine and the same
+sampling loop (`_denoise`): no image, mask or blend, an optional spatial scale map, and in guess mode with guidance the
+residuals on the conditional rows only (utils/stable_diffusion_controlnet.py:579-602).
+
 Not supported (raises NotImplementedError rather than silently diverging): the reference-only mode
-(`ref_image`, `utils/stable_diffusion_reference.py`), guess_mode.
+(`ref_image`, `utils/stable_diffusion_reference.py`).
 """
 import math
 import os
@@ -184,7 +192,10 @@ class _NetStub:
         self.nets = list(nets)
 
 
-class StableDiffusionControlNetInpaintPipeline:
+class _ControlNetPipelineBase:
+    """What the inpaint and the text-to-image pipelines share: construction (`from_pretrained`, `share_with`),
+    prompt encoding, the initial latents, decoding, and the sampling loop on the denoise engine (`_denoise`)."""
+
     def __init__(self, engine: DenoiseEngine, vae=None, text_encoder=None, tokenizer=None, scheduler=None,
                  safety_checker=None, feature_extractor=None):
         self.engine = engine
@@ -246,6 +257,7 @@ class StableDiffusionControlNetInpaintPipeline:
             share_with.text_encoder_shared = pipe.text_encoder_shared = True
         for stub, c in zip(pipe.controlnet.nets, cns):
             stub.config = c.config
+        pipe.controlnet.multi = isinstance(controlnet, (list, tuple))    # diffusers' MultiControlNetModel
         return pipe
 
     def load_textual_inversion(self, *a, **k):
@@ -273,7 +285,161 @@ class StableDiffusionControlNetInpaintPipeline:
     def _execution_device(self):
         return self.engine.dev
 
-    # ---------------------------------------------------------------------------------------
+    def _encode_prompt(self, prompt, num_images_per_prompt, do_cfg, negative_prompt=None, prompt_embeds=None,
+                       negative_prompt_embeds=None):
+        """utils/...inpaint.py:551-703: with embeds given, repeat per image and stack [negative; positive]."""
+        if prompt_embeds is None:
+            if self.tokenizer is None or self.text_encoder is None:
+                raise ValueError("no tokenizer/text_encoder attached: pass `prompt_embeds`")
+            prompt = [prompt] if isinstance(prompt, str) else prompt
+            ids = self.tokenizer(prompt, padding="max_length", max_length=self.tokenizer.model_max_length,
+                                 truncation=True, return_tensors="pt").input_ids
+            prompt_embeds = self.text_encoder(ids.to(self._execution_device))[0]
+        bs, L, D = prompt_embeds.shape
+        prompt_embeds = prompt_embeds.repeat(1, num_images_per_prompt, 1).view(bs * num_images_per_prompt, L, D)
+        if do_cfg:
+            if negative_prompt_embeds is None:
+                if self.tokenizer is None or self.text_encoder is None:
+                    raise ValueError("no tokenizer/text_encoder attached: pass `negative_prompt_embeds`")
+                neg = [""] * bs if negative_prompt is None else (
+                    [negative_prompt] if isinstance(negative_prompt, str) else negative_prompt)
+                ids = self.tokenizer(neg, padding="max_length", max_length=L, truncation=True,
+                                     return_tensors="pt").input_ids
+                negative_prompt_embeds = self.text_encoder(ids.to(self._execution_device))[0]
+            negative_prompt_embeds = negative_prompt_embeds.repeat(1, num_images_per_prompt, 1).view(
+                bs * num_images_per_prompt, L, D)
+            prompt_embeds = torch.cat([negative_prompt_embeds.to(prompt_embeds.device), prompt_embeds])
+        return prompt_embeds
+
+    def prepare_latents(self, batch_size, num_channels_latents, height, width, dtype, generator, latents=None):
+        shape = (batch_size, num_channels_latents, height // self.vae_scale_factor, width // self.vae_scale_factor)
+        if isinstance(generator, list) and len(generator) != batch_size:
+            raise ValueError(f"You have passed a list of generators of length {len(generator)}, but requested an"
+                             f" effective batch size of {batch_size}.")
+        if latents is None:
+            latents = randn_tensor(shape, generator=generator, dtype=dtype)
+        return latents * self.scheduler.init_noise_sigma
+
+    def _vae_device(self):
+        v = self.vae
+        for attr in ("device", "dev"):
+            d = getattr(v, attr, None)
+            if isinstance(d, (torch.device, str)):
+                return torch.device(d)
+        if hasattr(v, "parameters"):
+            try:
+                return next(iter(v.parameters())).device
+            except StopIteration:
+                return None
+        return None
+
+    def run_safety_checker(self, image, device, dtype):
+        """utils/...inpaint.py:705-716."""
+        if self.safety_checker is not None:
+            safety_checker_input = self.feature_extractor(self.numpy_to_pil(image), return_tensors="pt").to(device)
+            image, has_nsfw_concept = self.safety_checker(images=image,
+                                                          clip_input=safety_checker_input.pixel_values.to(dtype))
+        else:
+            has_nsfw_concept = None
+        return image, has_nsfw_concept
+
+    def decode_latents(self, latents):
+        """utils/...inpaint.py:718-724.  A `VaeDecoderEngine` (editanything_b200.vae) does the 1/scaling_factor,
+        the decode and the (x / 2 + 0.5).clamp(0, 1) in its own kernels; any other object with the diffusers
+        AutoencoderKL surface goes through the reference's three lines."""
+        if hasattr(self.vae, "decode_latents"):
+            image = self.vae.decode_latents(latents)
+        else:
+            image = self.vae.decode(latents / self.vae.config.scaling_factor).sample
+            image = (image / 2 + 0.5).clamp(0, 1)
+        return image.cpu().permute(0, 2, 3, 1).float().numpy()
+
+    @staticmethod
+    def numpy_to_pil(images):
+        images = (images * 255).round().astype("uint8")
+        return [PIL.Image.fromarray(i) for i in images]
+
+    def _fused_scheduler(self):
+        """(fused, unipc): the fused step runs the built-in DDIM, and UniPC (what every reference entry point installs,
+        editany_lora.py:383,418) through its per-step coefficient rows; any other scheduler object runs eng.eps +
+        scheduler.step on the host."""
+        unipc = isinstance(self.scheduler, UniPCMultistepScheduler) and self.scheduler.config.solver_order <= 2
+        return isinstance(self.scheduler, DDIMScheduler) or unipc, unipc
+
+    def _denoise(self, lat, timesteps, guidance_scale, do_cfg, callback=None, callback_steps=1, blend=None,
+                 unet_condition=None):
+        """The sampling loop of both pipelines (utils/...inpaint.py:1540-1656, utils/stable_diffusion_controlnet.py:
+        566-627) on the engine `prepare`d for this request: returns the final latents [N, 4, h, w] on the engine's
+        device.  lat: the initial latents [N, 4, h, w].  blend = (blend_steps, init, keep, noise): the inpaint
+        pipeline's kept region, re-noised from `init` while i < blend_steps (keep = 1 keeps it).  unet_condition =
+        (mask, masked-image latents) of a 9-channel UNet."""
+        eng = self.engine
+        N = lat.shape[0]
+        lat = lat.to(eng.dev, torch.float32)
+        blend_steps, init_d, m_d, noise_d = blend if blend is not None else (0, None, None, None)
+        n_t = len(timesteps)
+        fused, unipc = self._fused_scheduler()
+        if fused:
+            acp = self.scheduler.alphas_cumprod
+            coefs = [(float(acp[int(t)]), float(acp[int(t)])) for t in timesteps] if unipc else \
+                [self.scheduler.coefficients(t) for t in timesteps]
+            # the kept region of step i is add_noise(init, noise, timesteps[i + 1]) while i < len * alignment_ratio
+            # (:1647-1656).  With a callback the blend runs on the host side AFTER the callback, like the reference
+            # (:1640-1656 calls back with the un-blended latents); otherwise it is fused into the step's last kernel.
+            host_blend = callback is not None and blend_steps > 0
+            k_next = [(math.sqrt(float(acp[int(timesteps[i + 1])])), math.sqrt(1.0 - float(acp[int(timesteps[i + 1])])))
+                      if i < blend_steps else (1.0, 0.0) for i in range(n_t)]
+            on = [1.0 if (i < blend_steps and not host_blend) else 0.0 for i in range(n_t)]
+            eng.set_schedule([int(t) for t in timesteps], [c[0] for c in coefs], [c[1] for c in coefs],
+                             blend=([k[0] for k in k_next], [k[1] for k in k_next], on),
+                             multistep=self.scheduler.coefficient_rows() if unipc else None,
+                             prediction_type=self.scheduler.config.prediction_type)
+            if unet_condition is not None:
+                eng.set_unet_condition(*unet_condition)
+            eng.begin(lat, guidance_scale, known_nchw=init_d if blend_steps else None,
+                      mask_n1hw=m_d if blend_steps else None, noise_nchw=noise_d if blend_steps else None)
+            for i, t in enumerate(timesteps):
+                eng.step()
+                if callback is not None and i % callback_steps == 0:
+                    callback(i, t, eng.latents())
+                if host_blend and i < blend_steps:
+                    eng.blend_now(k_next[i][0], k_next[i][1])
+            return eng.latents()
+        copies = 2 if do_cfg else 1
+        if unet_condition is not None:
+            mask_lat, masked_lat = unet_condition
+            cond = torch.cat([torch.cat([mask_lat] * copies), torch.cat([masked_lat] * copies)], 1)
+        for i, t in enumerate(timesteps):
+            x_in = self.scheduler.scale_model_input(torch.cat([lat] * copies), t)
+            if unet_condition is not None:
+                x_in = torch.cat([x_in, cond], 1)                                  # :1550-1558
+            eps = eng.eps(x_in, float(t))
+            e = eps[:N] + guidance_scale * (eps[N:] - eps[:N]) if do_cfg else eps   # :1627-1631
+            lat = self.scheduler.step(e, t, lat).prev_sample
+            if callback is not None and i % callback_steps == 0:
+                callback(i, t, lat)
+            if i < blend_steps:
+                lat = self.scheduler.add_noise(init_d, noise_d, timesteps[i + 1]) * m_d + lat * (1 - m_d)
+        return lat
+
+    def _output(self, lat, output_type, return_dict, dtype):
+        """Latents -> the requested output: "latent", "pil" or numpy images (utils/...inpaint.py:1666-1703)."""
+        if output_type == "latent":
+            images, nsfw = lat, None
+        else:
+            if self.vae is None:
+                raise ValueError("a VAE is required unless output_type='latent'")
+            images = self.decode_latents(lat.to(next(iter(self.vae.parameters())).dtype)
+                                         if hasattr(self.vae, "parameters") else lat)
+            images, nsfw = self.run_safety_checker(images, self.engine.dev, dtype)
+            if output_type == "pil":
+                images = self.numpy_to_pil(images)
+        if not return_dict:
+            return images, nsfw
+        return StableDiffusionPipelineOutput(images=images, nsfw_content_detected=nsfw)
+
+
+class StableDiffusionControlNetInpaintPipeline(_ControlNetPipelineBase):
     def check_inputs(self, prompt, image, mask_image, controlnet_conditioning_image, height, width,
                      callback_steps, negative_prompt=None, prompt_embeds=None, negative_prompt_embeds=None,
                      controlnet_conditioning_scale=None):
@@ -358,41 +524,6 @@ class StableDiffusionControlNetInpaintPipeline:
             width = (width // 8) * 8
         return height, width
 
-    def _encode_prompt(self, prompt, num_images_per_prompt, do_cfg, negative_prompt=None, prompt_embeds=None,
-                       negative_prompt_embeds=None):
-        """utils/...inpaint.py:551-703: with embeds given, repeat per image and stack [negative; positive]."""
-        if prompt_embeds is None:
-            if self.tokenizer is None or self.text_encoder is None:
-                raise ValueError("no tokenizer/text_encoder attached: pass `prompt_embeds`")
-            prompt = [prompt] if isinstance(prompt, str) else prompt
-            ids = self.tokenizer(prompt, padding="max_length", max_length=self.tokenizer.model_max_length,
-                                 truncation=True, return_tensors="pt").input_ids
-            prompt_embeds = self.text_encoder(ids.to(self._execution_device))[0]
-        bs, L, D = prompt_embeds.shape
-        prompt_embeds = prompt_embeds.repeat(1, num_images_per_prompt, 1).view(bs * num_images_per_prompt, L, D)
-        if do_cfg:
-            if negative_prompt_embeds is None:
-                if self.tokenizer is None or self.text_encoder is None:
-                    raise ValueError("no tokenizer/text_encoder attached: pass `negative_prompt_embeds`")
-                neg = [""] * bs if negative_prompt is None else (
-                    [negative_prompt] if isinstance(negative_prompt, str) else negative_prompt)
-                ids = self.tokenizer(neg, padding="max_length", max_length=L, truncation=True,
-                                     return_tensors="pt").input_ids
-                negative_prompt_embeds = self.text_encoder(ids.to(self._execution_device))[0]
-            negative_prompt_embeds = negative_prompt_embeds.repeat(1, num_images_per_prompt, 1).view(
-                bs * num_images_per_prompt, L, D)
-            prompt_embeds = torch.cat([negative_prompt_embeds.to(prompt_embeds.device), prompt_embeds])
-        return prompt_embeds
-
-    def prepare_latents(self, batch_size, num_channels_latents, height, width, dtype, generator, latents=None):
-        shape = (batch_size, num_channels_latents, height // self.vae_scale_factor, width // self.vae_scale_factor)
-        if isinstance(generator, list) and len(generator) != batch_size:
-            raise ValueError(f"You have passed a list of generators of length {len(generator)}, but requested an"
-                             f" effective batch size of {batch_size}.")
-        if latents is None:
-            latents = randn_tensor(shape, generator=generator, dtype=dtype)
-        return latents * self.scheduler.init_noise_sigma
-
     def prepare_masked_image_latents(self, masked_image, batch_size, dtype, generator):
         """utils/...inpaint.py:1056-1105 (without the CFG duplication the caller immediately undoes)."""
         if self.vae is None:
@@ -412,45 +543,6 @@ class StableDiffusionControlNetInpaintPipeline:
                 raise ValueError("The passed images and the required batch size don't match.")
             lat = lat.repeat(batch_size // lat.shape[0], 1, 1, 1)
         return lat
-
-    def _vae_device(self):
-        v = self.vae
-        for attr in ("device", "dev"):
-            d = getattr(v, attr, None)
-            if isinstance(d, (torch.device, str)):
-                return torch.device(d)
-        if hasattr(v, "parameters"):
-            try:
-                return next(iter(v.parameters())).device
-            except StopIteration:
-                return None
-        return None
-
-    def run_safety_checker(self, image, device, dtype):
-        """utils/...inpaint.py:705-716."""
-        if self.safety_checker is not None:
-            safety_checker_input = self.feature_extractor(self.numpy_to_pil(image), return_tensors="pt").to(device)
-            image, has_nsfw_concept = self.safety_checker(images=image,
-                                                          clip_input=safety_checker_input.pixel_values.to(dtype))
-        else:
-            has_nsfw_concept = None
-        return image, has_nsfw_concept
-
-    def decode_latents(self, latents):
-        """utils/...inpaint.py:718-724.  A `VaeDecoderEngine` (editanything_b200.vae) does the 1/scaling_factor,
-        the decode and the (x / 2 + 0.5).clamp(0, 1) in its own kernels; any other object with the diffusers
-        AutoencoderKL surface goes through the reference's three lines."""
-        if hasattr(self.vae, "decode_latents"):
-            image = self.vae.decode_latents(latents)
-        else:
-            image = self.vae.decode(latents / self.vae.config.scaling_factor).sample
-            image = (image / 2 + 0.5).clamp(0, 1)
-        return image.cpu().permute(0, 2, 3, 1).float().numpy()
-
-    @staticmethod
-    def numpy_to_pil(images):
-        images = (images * 255).round().astype("uint8")
-        return [PIL.Image.fromarray(i) for i in images]
 
     # ---------------------------------------------------------------------------------------
     @torch.no_grad()
@@ -523,10 +615,6 @@ class StableDiffusionControlNetInpaintPipeline:
 
         eng.prepare(prompt_embeds, conds, controlnet_conditioning_scale, guess_mode=guess_mode, cfg_duplicated=do_cfg,
                     guided=do_cfg)
-        # fused step: the built-in DDIM, and UniPC (what every reference entry point installs, editany_lora.py:383,418)
-        # through its per-step coefficient rows; any other scheduler object runs eng.eps + scheduler.step
-        unipc = isinstance(self.scheduler, UniPCMultistepScheduler) and self.scheduler.config.solver_order <= 2
-        fused = isinstance(self.scheduler, DDIMScheduler) or unipc
         n_t = len(timesteps)
         blend_steps = 0 if alignment_ratio is None else sum(1 for i in range(n_t) if i < n_t * alignment_ratio)
         if blend_steps and blend_steps >= n_t:
@@ -534,65 +622,216 @@ class StableDiffusionControlNetInpaintPipeline:
             raise IndexError("alignment_ratio covers the last step: timesteps[i + 1] is out of range")
         # everything below lives on the execution device (the noise was DRAWN on the generator's device above,
         # like diffusers' randn_tensor, then moved - utils/...inpaint.py:998-1012)
-        lat = lat.to(dev, torch.float32)
         if inpaint_unet:
-            noise_d = init_d = m_d = None
+            lat = self._denoise(lat, timesteps, guidance_scale, do_cfg, callback, callback_steps,
+                                unet_condition=(mask_lat, masked_lat))
         else:
             noise_d, init_d, m_d = noise.to(dev, torch.float32), init_lat.to(dev, torch.float32), m.to(dev, torch.float32)
-        if fused:
-            acp = self.scheduler.alphas_cumprod
-            coefs = [(float(acp[int(t)]), float(acp[int(t)])) for t in timesteps] if unipc else \
-                [self.scheduler.coefficients(t) for t in timesteps]
-            # the kept region of step i is add_noise(init, noise, timesteps[i + 1]) while i < len * alignment_ratio
-            # (:1647-1656).  With a callback the blend runs on the host side AFTER the callback, like the reference
-            # (:1640-1656 calls back with the un-blended latents); otherwise it is fused into the step's last kernel.
-            host_blend = callback is not None and blend_steps > 0
-            k_next = [(math.sqrt(float(acp[int(timesteps[i + 1])])), math.sqrt(1.0 - float(acp[int(timesteps[i + 1])])))
-                      if i < blend_steps else (1.0, 0.0) for i in range(n_t)]
-            on = [1.0 if (i < blend_steps and not host_blend) else 0.0 for i in range(n_t)]
-            eng.set_schedule([int(t) for t in timesteps], [c[0] for c in coefs], [c[1] for c in coefs],
-                             blend=([k[0] for k in k_next], [k[1] for k in k_next], on),
-                             multistep=self.scheduler.coefficient_rows() if unipc else None,
-                             prediction_type=self.scheduler.config.prediction_type)
-            if inpaint_unet:
-                eng.set_unet_condition(mask_lat, masked_lat)
-            eng.begin(lat, guidance_scale, known_nchw=init_d if blend_steps else None,
-                      mask_n1hw=m_d if blend_steps else None, noise_nchw=noise_d if blend_steps else None)
-            for i, t in enumerate(timesteps):
-                eng.step()
-                if callback is not None and i % callback_steps == 0:
-                    callback(i, t, eng.latents())
-                if host_blend and i < blend_steps:
-                    eng.blend_now(k_next[i][0], k_next[i][1])
-            lat = eng.latents()
-        else:
-            copies = 2 if do_cfg else 1
-            if inpaint_unet:
-                cond = torch.cat([torch.cat([mask_lat] * copies), torch.cat([masked_lat] * copies)], 1)
-            for i, t in enumerate(timesteps):
-                x_in = self.scheduler.scale_model_input(torch.cat([lat] * copies), t)
-                if inpaint_unet:
-                    x_in = torch.cat([x_in, cond], 1)                                  # :1550-1558
-                eps = eng.eps(x_in, float(t))
-                e = eps[:N] + guidance_scale * (eps[N:] - eps[:N]) if do_cfg else eps   # :1627-1631
-                lat = self.scheduler.step(e, t, lat).prev_sample
-                if callback is not None and i % callback_steps == 0:
-                    callback(i, t, lat)
-                if i < blend_steps:
-                    lat = self.scheduler.add_noise(init_d, noise_d, timesteps[i + 1]) * m_d + lat * (1 - m_d)
-        if not inpaint_unet and (alignment_ratio is None or alignment_ratio == 1.0):
-            lat = init_d * m_d + lat * (1 - m_d)                                   # :1658-1664
+            lat = self._denoise(lat, timesteps, guidance_scale, do_cfg, callback, callback_steps,
+                                blend=(blend_steps, init_d, m_d, noise_d))
+            if alignment_ratio is None or alignment_ratio == 1.0:
+                lat = init_d * m_d + lat * (1 - m_d)                                   # :1658-1664
+        return self._output(lat, output_type, return_dict, edt)
 
-        if output_type == "latent":
-            images, nsfw = lat, None
+
+class StableDiffusionControlNetPipeline(_ControlNetPipelineBase):
+    """Text-to-image generation with ControlNets on the fused denoising step: the call of diffusers 0.17.1's
+    `StableDiffusionControlNetPipeline`, which the reference imports for all-region generation (editany_lora.py:22,
+    :365-370, :796-812) and sam2image.py:28-50.  Its contract is the in-tree `StableDiffusionControlNetPipeline2.
+    __call__` (utils/stable_diffusion_controlnet.py:346-662) without the scale map.  The helpers it inherits from
+    diffusers 0.17.1 (`_default_height_width`, `check_inputs`, `prepare_image`, `_encode_prompt`, `prepare_latents`,
+    `decode_latents`) are not in the reference tree; they are restated here from that release.
+
+    The latents are drawn from the generator and scaled by the scheduler's init_noise_sigma; nothing else is drawn,
+    and there is no image to encode, blend or paste back.  Guess mode with classifier-free guidance adds the
+    ControlNet residuals to the conditional rows only (:579-602; DenoiseEngine.prepare(controlnet_rows=
+    "conditional")); without guidance the ControlNets drive every row (:579-583).
+
+    Not supported (raise before any launch): a UNet that does not take 4 latent channels, eta != 0, ControlNets
+    whose config sets `global_pool_conditions` (the shuffle ControlNet), and guess mode with guidance on a scheduler
+    whose `scale_model_input` is not the identity (the sigma-based ones: Euler, LMS, Heun, ...).  There the reference
+    feeds the ControlNet the unscaled latents and the UNet the scaled ones (:579-582), while the engine's networks
+    read one input.  DDIM and UniPC scale by 1 and run; so does guess mode without guidance and every request
+    without guess mode, where both read the scaled latents (:583-584)."""
+
+    def _default_height_width(self, height, width, image):
+        """diffusers 0.17.1: from the first control image (tensors: shape[2] is the height)."""
+        while isinstance(image, list):
+            image = image[0]
+        if height is None:
+            height = image.shape[2] if isinstance(image, torch.Tensor) else image.height
+            height = (height // 8) * 8
+        if width is None:
+            width = image.shape[3] if isinstance(image, torch.Tensor) else image.width
+            width = (width // 8) * 8
+        return height, width
+
+    def _multi(self, controlnet_conditioning_scale):
+        """Whether the nets take lists of images and scales, like diffusers' MultiControlNetModel: always for several
+        nets, and for one net as `from_pretrained` was given it (a list: `controlnet.multi`).  A pipeline built
+        directly on an engine has no record of that, since the engine always holds a list; it then takes the form of
+        the call: a list scale means the list form, where diffusers would raise TypeError for a single
+        ControlNetModel with a non-float scale.  Either form gives the same images for one net."""
+        multi = getattr(self.controlnet, "multi", None)
+        if multi is None:
+            multi = isinstance(controlnet_conditioning_scale, list)
+        return multi or len(self.controlnet.nets) > 1
+
+    @staticmethod
+    def check_image(image, prompt, prompt_embeds):
+        """diffusers 0.17.1."""
+        is_pil = PIL is not None and isinstance(image, PIL.Image.Image)
+        is_tensor = isinstance(image, torch.Tensor)
+        is_pil_list = isinstance(image, list) and PIL is not None and isinstance(image[0], PIL.Image.Image)
+        is_tensor_list = isinstance(image, list) and isinstance(image[0], torch.Tensor)
+        if not (is_pil or is_tensor or is_pil_list or is_tensor_list):
+            raise TypeError("image must be passed and be one of PIL image, torch tensor, list of PIL images, or list of"
+                            " torch tensors")
+        image_batch_size = 1 if is_pil else image.shape[0] if is_tensor else len(image)
+        if prompt is not None and isinstance(prompt, str):
+            prompt_batch_size = 1
+        elif prompt is not None and isinstance(prompt, list):
+            prompt_batch_size = len(prompt)
         else:
-            if self.vae is None:
-                raise ValueError("a VAE is required unless output_type='latent'")
-            images = self.decode_latents(lat.to(next(iter(self.vae.parameters())).dtype)
-                                         if hasattr(self.vae, "parameters") else lat)
-            images, nsfw = self.run_safety_checker(images, dev, edt)
-            if output_type == "pil":
-                images = self.numpy_to_pil(images)
-        if not return_dict:
-            return images, nsfw
-        return StableDiffusionPipelineOutput(images=images, nsfw_content_detected=nsfw)
+            prompt_batch_size = prompt_embeds.shape[0]
+        if image_batch_size != 1 and image_batch_size != prompt_batch_size:
+            raise ValueError(f"If image batch size is not 1, image batch size must be same as prompt batch size. image"
+                             f" batch size: {image_batch_size}, prompt batch size: {prompt_batch_size}")
+
+    def check_inputs(self, prompt, image, height, width, callback_steps, negative_prompt=None, prompt_embeds=None,
+                     negative_prompt_embeds=None, controlnet_conditioning_scale=1.0):
+        """diffusers 0.17.1: the prompt checks the inpaint pipeline makes, then the control images and scales."""
+        if height % 8 != 0 or width % 8 != 0:
+            raise ValueError(f"`height` and `width` have to be divisible by 8 but are {height} and {width}.")
+        if callback_steps is None or not isinstance(callback_steps, int) or callback_steps <= 0:
+            raise ValueError(f"`callback_steps` has to be a positive integer but is {callback_steps} of type"
+                             f" {type(callback_steps)}.")
+        if prompt is not None and prompt_embeds is not None:
+            raise ValueError("Cannot forward both `prompt` and `prompt_embeds`. Please make sure to only forward one"
+                             " of the two.")
+        if prompt is None and prompt_embeds is None:
+            raise ValueError("Provide either `prompt` or `prompt_embeds`. Cannot leave both `prompt` and"
+                             " `prompt_embeds` undefined.")
+        if prompt is not None and not isinstance(prompt, (str, list)):
+            raise ValueError(f"`prompt` has to be of type `str` or `list` but is {type(prompt)}")
+        if negative_prompt is not None and negative_prompt_embeds is not None:
+            raise ValueError("Cannot forward both `negative_prompt` and `negative_prompt_embeds`.")
+        if prompt_embeds is not None and negative_prompt_embeds is not None \
+                and prompt_embeds.shape != negative_prompt_embeds.shape:
+            raise ValueError("`prompt_embeds` and `negative_prompt_embeds` must have the same shape when passed"
+                             f" directly, but got {prompt_embeds.shape} != {negative_prompt_embeds.shape}.")
+        n_nets = len(self.controlnet.nets)
+        if self._multi(controlnet_conditioning_scale):
+            if not isinstance(image, list):
+                raise TypeError("For multiple controlnets: `image` must be type `list`")
+            if any(isinstance(i, list) for i in image):
+                raise ValueError("A single batch of multiple conditionings are supported at the moment.")
+            if len(image) != n_nets:
+                raise ValueError("For multiple controlnets: `image` must have the same length as the number of"
+                                 " controlnets.")
+            for image_ in image:
+                self.check_image(image_, prompt, prompt_embeds)
+            if isinstance(controlnet_conditioning_scale, list):
+                if any(isinstance(i, list) for i in controlnet_conditioning_scale):
+                    raise ValueError("A single batch of multiple conditionings are supported at the moment.")
+                if len(controlnet_conditioning_scale) != n_nets:
+                    raise ValueError("For multiple controlnets: When `controlnet_conditioning_scale` is specified as"
+                                     " `list`, it must have the same length as the number of controlnets")
+        else:
+            self.check_image(image, prompt, prompt_embeds)
+            if not isinstance(controlnet_conditioning_scale, float):
+                raise TypeError("For single controlnet: `controlnet_conditioning_scale` must be type `float`.")
+
+    @staticmethod
+    def prepare_image(image, width, height, batch_size, num_images_per_prompt, dtype, do_classifier_free_guidance,
+                      guess_mode):
+        """prepare_controlnet_conditioning_image (utils/stable_diffusion_controlnet.py:308-344), except that guess mode
+        does not double the images for guidance: the ControlNets then add to the conditional rows only."""
+        return prepare_controlnet_conditioning_image(image, width, height, batch_size, num_images_per_prompt, dtype,
+                                                     do_classifier_free_guidance and not guess_mode)
+
+    def _check_supported(self, eta, guess_mode, scale_map):
+        if self.unet.config.in_channels != 4:
+            raise NotImplementedError(f"text-to-image generation runs a UNet of 4 latent channels, this one takes "
+                                      f"{self.unet.config.in_channels}")
+        if eta != 0.0:
+            raise NotImplementedError("only deterministic sampling (eta = 0) is fused")
+        if any(getattr(n.config, "global_pool_conditions", False) for n in self.controlnet.nets):
+            raise NotImplementedError("ControlNets with global_pool_conditions (pooled residuals) are not fused")
+        if guess_mode and scale_map is not None:
+            raise NotImplementedError("guess_mode with a spatial conditioning_scale map")
+
+    @torch.no_grad()
+    def __call__(self, prompt=None, image=None, height=None, width=None, num_inference_steps=50, guidance_scale=7.5,
+                 negative_prompt=None, num_images_per_prompt=1, eta=0.0, generator=None, latents=None,
+                 prompt_embeds=None, negative_prompt_embeds=None, output_type="pil", return_dict=True, callback=None,
+                 callback_steps=1, cross_attention_kwargs=None, controlnet_conditioning_scale=1.0, guess_mode=False):
+        return self._generate(prompt, image, height, width, num_inference_steps, guidance_scale, negative_prompt,
+                              num_images_per_prompt, eta, generator, latents, prompt_embeds, negative_prompt_embeds,
+                              output_type, return_dict, callback, callback_steps, controlnet_conditioning_scale, None,
+                              guess_mode)
+
+    def _generate(self, prompt, image, height, width, num_inference_steps, guidance_scale, negative_prompt,
+                  num_images_per_prompt, eta, generator, latents, prompt_embeds, negative_prompt_embeds, output_type,
+                  return_dict, callback, callback_steps, controlnet_conditioning_scale, scale_map, guess_mode):
+        """utils/stable_diffusion_controlnet.py:465-662."""
+        self._check_supported(eta, guess_mode, scale_map)
+        height, width = self._default_height_width(height, width, image)
+        self.check_inputs(prompt, image, height, width, callback_steps, negative_prompt, prompt_embeds,
+                          negative_prompt_embeds, controlnet_conditioning_scale)
+        if prompt is not None and isinstance(prompt, str):
+            batch_size = 1
+        elif prompt is not None:
+            batch_size = len(prompt)
+        else:
+            batch_size = prompt_embeds.shape[0]
+        N = batch_size * num_images_per_prompt
+        do_cfg = guidance_scale > 1.0
+        multi = self._multi(controlnet_conditioning_scale)
+        if multi and isinstance(controlnet_conditioning_scale, float):
+            controlnet_conditioning_scale = [controlnet_conditioning_scale] * len(self.controlnet.nets)
+        if scale_map is not None:                                                # :490-495
+            if isinstance(controlnet_conditioning_scale, list):
+                controlnet_conditioning_scale = [s * scale_map for s in controlnet_conditioning_scale]
+            else:
+                controlnet_conditioning_scale = controlnet_conditioning_scale * scale_map
+        scales = controlnet_conditioning_scale if multi else [controlnet_conditioning_scale]
+        images = image if multi else [image]
+
+        prompt_embeds = self._encode_prompt(prompt, num_images_per_prompt, do_cfg, negative_prompt, prompt_embeds,
+                                            negative_prompt_embeds)
+        conds = [self.prepare_image(im, width, height, N, num_images_per_prompt, torch.float32, do_cfg, guess_mode)
+                 for im in images]
+        self.scheduler.set_timesteps(num_inference_steps, device=self._execution_device)
+        timesteps = self.scheduler.timesteps
+        lat = self.prepare_latents(N, 4, height, width, prompt_embeds.dtype, generator, latents)
+        conditional = guess_mode and do_cfg
+        if conditional and not self._fused_scheduler()[0] and \
+                any(not torch.equal(self.scheduler.scale_model_input(lat, t), lat) for t in timesteps):
+            # :579-582 feeds the ControlNet the unscaled latents and the UNet scale_model_input(latents); the engine
+            # feeds every network the same input, which is right only where scale_model_input is the identity (DDIM,
+            # UniPC, not the sigma-based schedulers).  Probed on the initial latents, before anything is launched.
+            raise NotImplementedError(f"guess_mode with guidance on {type(self.scheduler).__name__}, whose "
+                                      "scale_model_input is not the identity: the ControlNet would read the scaled "
+                                      "latents")
+        self.engine.prepare(prompt_embeds, conds, scales, guess_mode=guess_mode, cfg_duplicated=do_cfg and not guess_mode,
+                            guided=do_cfg, controlnet_rows="conditional" if conditional else "all")
+        lat = self._denoise(lat, timesteps, guidance_scale, do_cfg, callback, callback_steps)
+        return self._output(lat, output_type, return_dict, prompt_embeds.dtype)
+
+
+class StableDiffusionControlNetPipeline2(StableDiffusionControlNetPipeline):
+    """utils/stable_diffusion_controlnet.py:346-662: the text-to-image pipeline with `controlnet_conditioning_scale_map`,
+    a spatial [H, W] (or [1, H, W], [1, 1, H, W]) map that multiplies every net's scale (:490-495) and is resized
+    bilinearly to every residual (ControlNetModel2.forward, :787-802), as sketch2image.py:140-175 uses it."""
+
+    @torch.no_grad()
+    def __call__(self, prompt=None, image=None, height=None, width=None, num_inference_steps=50, guidance_scale=7.5,
+                 negative_prompt=None, num_images_per_prompt=1, eta=0.0, generator=None, latents=None,
+                 prompt_embeds=None, negative_prompt_embeds=None, output_type="pil", return_dict=True, callback=None,
+                 callback_steps=1, cross_attention_kwargs=None, controlnet_conditioning_scale=1.0,
+                 controlnet_conditioning_scale_map=None, guess_mode=False):
+        return self._generate(prompt, image, height, width, num_inference_steps, guidance_scale, negative_prompt,
+                              num_images_per_prompt, eta, generator, latents, prompt_embeds, negative_prompt_embeds,
+                              output_type, return_dict, callback, callback_steps, controlnet_conditioning_scale,
+                              controlnet_conditioning_scale_map, guess_mode)
