@@ -207,8 +207,8 @@ class VaeDecoderEngine(_VaeBase):
     @engine_call
     def decode_latents(self, latents, use_graph=True):
         """latents as the denoising loop leaves them -> fp32 [B, 3, 8h, 8w] in [0, 1]
-        (decode_latents up to the .cpu().permute().numpy() plumbing).  On the CUDA backend the ~170
-        launches are captured once per latent shape into a CUDA graph and replayed."""
+        (decode_latents up to the .cpu().permute().numpy() plumbing).  On the CUDA backend the launches (71
+        for the SD VAE) are captured once per latent shape into a CUDA graph and replayed."""
         if not use_graph or self.dev.type != "cuda":
             return self._decode(latents.float() / self.cfg.scaling_factor, post=True)
         return self._graphed(("dec",) + tuple(latents.shape), latents,

@@ -81,6 +81,103 @@ def groupnorm(x, gammas, betas, groups, eps, silu_on):
     return (silu(out) if silu_on else out), out, terms
 
 
+def gn_geometry(B, HW, C, groups, n_sm):
+    """ea_groupnorm's launch geometry (ea_pointwise.cu, ea_groupnorm) as (chunks, ppc, lanes, parts): `chunks` CTAs
+    per image of `ppc` pixels each, `lanes` pixel lanes per CTA (thread = lane x 8-channel vector), and the `parts`
+    threads per statistic that sum the image's per-CTA partials."""
+    chunks = max(1, min(n_sm // B, HW))
+    ppc = -(-HW // chunks)
+    chunks = -(-HW // ppc)
+    nvec = C // 8
+    threads = min(512, -(-((512 // nvec) * nvec) // 32) * 32)
+    lanes = threads // nvec
+    parts = max(1, min(threads // (2 * groups), lanes * (C // groups)))
+    return chunks, ppc, lanes, parts
+
+
+def _chain(v, dim):
+    """A serial fp32 sum along `dim`, in float64: (sum of |partial sums|, the total).  The rounding error of the
+    recursive sum is at most u times the sum of its partial sums' magnitudes (Higham, Accuracy and Stability of
+    Numerical Algorithms, 2nd ed., (4.3)); zero padding at the end of a chain only adds to that sum."""
+    cs = v.cumsum(dim)
+    return cs.abs().sum(dim), cs.select(dim, -1)
+
+
+def gn_cta_sums(d, lanes, groups):
+    """One CTA's part of ea_groupnorm's statistics.  d: [n, C] float64, the CTA's pixels minus each channel's shift
+    k_g.  The kernel sums d and d^2 in this order: thread (lane l, channel c) adds pixels l, l + lanes, ...; then one
+    thread per (group, statistic) adds the lanes x cpg thread partials, lane-major.  Returns
+    [2, groups] (the CTA totals, the sum of |partial sums| over both stages) for (sum d, sum d^2)."""
+    n, C = d.shape
+    cpg = C // groups
+    T = -(-n // lanes)
+    tot, run = [], []
+    for v in (d, d * d):
+        r1, t1 = _chain(torch.nn.functional.pad(v, (0, 0, 0, T * lanes - n)).reshape(T, lanes, C), 0)
+        r2, t2 = _chain(t1.reshape(lanes, groups, cpg).permute(1, 0, 2).reshape(groups, lanes * cpg), 1)
+        tot.append(t2)
+        run.append(r1.reshape(lanes, groups, cpg).sum(dim=(0, 2)) + r2)
+    return torch.stack(tot), torch.stack(run)
+
+
+def gn_cross_cta(totals, parts):
+    """The kernel's sum of one image's per-CTA totals [chunks, 2, groups]: thread pidx of each statistic adds CTAs
+    pidx, pidx + parts, ... in order, then one thread adds the parts in order.  Returns the sum of |partial sums|
+    [2, groups]."""
+    chunks = totals.shape[0]
+    rows = -(-chunks // parts)
+    t = torch.nn.functional.pad(totals, (0, 0, 0, 0, 0, rows * parts - chunks)).reshape(rows, parts, *totals.shape[1:])
+    r1, t1 = _chain(t, 0)
+    r2, _ = _chain(t1, 0)
+    return r1.sum(0) + r2
+
+
+def gn_stats_err(run, abs_sum, sq_sum, n, mean_dev, var, eps):
+    """Bounds on ea_groupnorm's fp32 statistics per (image, group) from their summation order: `run` [2, ...] the sum
+    of |partial sums| of sum d and sum d^2 over every stage (gn_cta_sums, gn_cross_cta), abs_sum / sq_sum the sums of
+    |d| and d^2 (the rounding of d = x - k and of d^2), n the pixels x channels of the group, mean_dev the mean of d,
+    var the group's variance.  The sums are off by dS1 = u (run_1 + sum |d|) and dS2 = u (run_2 + 3 sum d^2) (x1.01 for
+    the second-order terms); the kernel's dm = S1 inv_n (3 u) gives the mean's bound, and q inv_n - dm^2 the
+    variance's: dS2 / n + 2 |dm| dS1 / n + 4 u E[d^2] + 8 u dm^2.  Returns (bound on the mean, relative bound on
+    rstd = (var + eps)^-1/2: half the variance's relative error plus 2 u)."""
+    dS1 = 1.01 * U32 * (run[0] + abs_sum)
+    dS2 = 1.01 * U32 * (run[1] + 3 * sq_sum)
+    m = mean_dev.abs()
+    d_mean = dS1 / n + 3 * U32 * m
+    d_var = dS2 / n + 2 * m * dS1 / n + 4 * U32 * sq_sum / n + 8 * U32 * m * m
+    return d_mean, 0.5 * d_var / (var + eps) + 2 * U32
+
+
+def gn_stats_bound(x, groups, eps, n_sm):
+    """gn_stats_err for a whole [B, HW, C] float64 input (the kernel's fp16 values): per (image, group) the bound on
+    the mean, the relative bound on rstd, and rstd itself, each [B, groups]."""
+    B, HW, C = x.shape
+    cpg = C // groups
+    chunks, ppc, lanes, parts = gn_geometry(B, HW, C, groups, n_sm)
+    xg = x.reshape(B, HW, groups, cpg)
+    k = xg[:, 0, :, 0]
+    d_mean, d_rstd, r = [], [], []
+    for b in range(B):
+        kc = k[b].repeat_interleave(cpg)
+        cta = [gn_cta_sums(x[b, c * ppc:(c + 1) * ppc] - kc, lanes, groups) for c in range(chunks)]
+        run = sum(r_ for _, r_ in cta) + gn_cross_cta(torch.stack([t for t, _ in cta]), parts)
+        dk = xg[b] - k[b][None, :, None]
+        var = xg[b].var(dim=(0, 2), correction=0)
+        dm, dr = gn_stats_err(run, dk.abs().sum(dim=(0, 2)), (dk * dk).sum(dim=(0, 2)), HW * cpg,
+                              dk.mean(dim=(0, 2)), var, eps)
+        d_mean.append(dm)
+        d_rstd.append(dr)
+        r.append((var + eps).rsqrt())
+    return torch.stack(d_mean), torch.stack(d_rstd), torch.stack(r)
+
+
+def gn_stats_excess(y, gamma, r, d_mean, d_rstd, allowance):
+    """What the statistics' rounding (gn_stats_err) can add to g (x - mean) rstd + b beyond `allowance` |g|, the unit
+    the normalisation bound has always given them: |g| max(0, rstd d_mean + |y| d_rstd - allowance).  y: the
+    normalised value; r / d_mean / d_rstd broadcast against it."""
+    return gamma.abs() * (r * d_mean + y.abs() * d_rstd - allowance).clamp_min(0.0)
+
+
 def layernorm(x, gamma, beta, eps):
     """x: [M, C].  Returns (y, terms) like groupnorm (no SiLU)."""
     y = F.layer_norm(x, (x.shape[-1],), gamma, beta, eps)

@@ -13,7 +13,11 @@ tests/cpu_ops.py on the CPU).  For every call it
     lane the engine selected), synchronises again;
  3. recomputes the written operands in float64 from the snapshot and applies the per-element bound of that kernel's
     suite (tests/test_gpu_kernels_fp64.py, tests/test_gpu_conv_fp64.py, tests/test_gpu_attention.py); layout and copy
-    kernels must be bit-exact, a grouped GEMM is checked group by group;
+    kernels must be bit-exact, a grouped GEMM is checked group by group.  The float64 side is built in bands of at
+    most CHUNK_ELEMS outputs (rows of a GEMM; output rows of one image for a convolution, with the input rows they
+    reach; pixel rows of one image for GroupNorm, whose statistics are merged over the bands first; query rows of one
+    batch element for attention), and only the slice of each operand a band reads is upcast, so that the full
+    2048 x 2752 tile-refinement layers (2.9 GB fp16 activations) are checked in bounded memory;
  4. requires every element of a written storage outside the declared written extent to be bit-identical to the
     snapshot, the GEMM split-K and GroupNorm workspace counters to be zero again and the step counter to be +1;
  5. re-runs the call on relocated copies of every storage: each a fresh allocation with a NaN margin of at least
@@ -31,6 +35,7 @@ import traceback
 
 import numpy as np
 import torch
+import torch.nn.functional as F
 
 from tests import attn_ref, cpu_ops
 from tests import fp64_refs as R
@@ -42,7 +47,7 @@ MARGIN_ROWS = 128
 LINEAR, CONV_S1, CONV_S2, CONV_S2A = 0, 1, 2, 3
 ACT = {0: "none", 1: "silu", 2: "gelu", 3: "geglu"}
 GEMM_WS_COUNTER_BYTES = 65536
-CHUNK_ELEMS = 1 << 24       # float64 GEMM references are built this many outputs at a time
+CHUNK_ELEMS = 1 << 24       # float64 references are built at most this many outputs at a time (at least one row)
 # operator-table entries that launch nothing
 PASSTHROUGH = {"half_dtype", "set_lane", "launch_count", "reset_launch_count", "gn_workspace", "gemm_workspace",
                "weight_lookahead", "WeightLookahead", "check_out_buffers", "check_prediction"}
@@ -104,10 +109,86 @@ def _sync(dev):
 
 class Spec:
     """The operands of one call and its float64 check: check(snap, got) yields (operand, got, ref, bound) with
-    bound None for bit-exact, snap(name) / got(name) the float64 pre-call / the post-call declared view."""
+    bound None for bit-exact, snap(name) / got(name) the pre-call / the post-call declared view, both in the stored
+    dtype (a check upcasts the slices it reads with _d)."""
 
     def __init__(self, op, operands, check, after=None):
         self.op, self.operands, self.check, self.after = op, operands, check, after
+
+
+def _d(t):
+    """float64 (integer storages: int64) copy of a slice of an operand."""
+    return t.double() if t.is_floating_point() else t.long()
+
+
+def bands(n, per):
+    """[lo, hi) ranges covering range(n), at most max(1, per) long."""
+    per = max(1, int(per))
+    return [(lo, min(n, lo + per)) for lo in range(0, n, per)]
+
+
+def _whole(snap):
+    """snap for a check of small operands: each one upcast whole."""
+    return lambda name: _d(snap(name))
+
+
+def _tag(parts, label):
+    """The band an operand's check covers, in its name when there is more than one band."""
+    return f" [{label}]" if len(parts) > 1 else ""
+
+
+def conv_rows(x, w, k, stride, top, wpad, y0, y1):
+    """Output rows [y0, y1) of a k x k convolution without bias: x NHWC [B, Hin, Win, Cin] in any dtype, of which only
+    the input rows the band reaches are upcast; w [k, k, Cin, Cout] float64.  The input is zero-padded by `top` rows
+    above row 0 (and below the last row as far as the kernel reaches) and by wpad = (left, right) columns; output row
+    y reads padded rows stride * y .. stride * y + k - 1.  Returns (out [B, y1 - y0, Wo, Cout], sum of |x w|)."""
+    Hin = x.shape[1]
+    p0, p1 = stride * y0 - top, stride * (y1 - 1) - top + k       # input rows read, in image coordinates
+    lo, hi = max(0, p0), min(Hin, p1)
+    xb = F.pad(x[:, lo:hi].double().permute(0, 3, 1, 2), (wpad[0], wpad[1], lo - p0, p1 - hi))
+    wt = w.permute(3, 2, 0, 1)
+    out = F.conv2d(xb, wt, stride=stride).permute(0, 2, 3, 1)
+    mag = F.conv2d(xb.abs(), wt.abs(), stride=stride).permute(0, 2, 3, 1)
+    return out, mag
+
+
+# ea_gemm's convolution modes as (stride, zero rows above row 0, zero columns (left, right)) - R.conv_gemm's padding
+CONV_GEOM = {CONV_S1: (1, 1, (1, 1)), CONV_S2: (2, 1, (1, 1)), CONV_S2A: (2, 0, (0, 1))}
+
+
+def conv_gemm_rows(x, w, mode, y0, y1, extra=None):
+    """R.conv_gemm(x, w, mode, extra)[:, y0:y1] built from the input rows those outputs reach: +-1 row for CONV_S1,
+    rows 2y - 1 .. 2y + 1 for CONV_S2, 2y .. 2y + 2 (the last one the bottom zero pad) for CONV_S2A, and extra's rows
+    y0 .. y1 - 1.  x / extra in any dtype (sliced, then upcast), w [Cout, 9 Cin (+ Cin_extra)] float64."""
+    cout, cin = w.shape[0], x.shape[-1]
+    s, top, wpad = CONV_GEOM[mode]
+    out, mag = conv_rows(x, w[:, :9 * cin].reshape(cout, 3, 3, cin).permute(1, 2, 3, 0), 3, s, top, wpad, y0, y1)
+    if extra is not None:
+        we = w[:, 9 * cin:]
+        e = extra[:, y0:y1].double()
+        out, mag = out + e @ we.T, mag + e.abs() @ we.abs().T
+    return out, mag
+
+
+def groupnorm_stats(band_iter, B, groups):
+    """Per (image, group) float64 (count, mean, M2) over bands of one image's pixel rows, merged pairwise (Chan, Golub
+    & LeVeque): n = na + nb, mean = mean_a + d nb / n, M2 = M2_a + M2_b + d^2 na nb / n with d = mean_b - mean_a.
+    band_iter yields (image, band [rows, groups, C / groups] float64)."""
+    n = [0.0] * B
+    mean = m2 = None
+    for b, xg in band_iter:
+        if mean is None:
+            mean = torch.zeros(B, groups, dtype=torch.float64, device=xg.device)
+            m2 = torch.zeros_like(mean)
+        nb = float(xg.shape[0] * xg.shape[2])
+        mb = xg.mean(dim=(0, 2))
+        m2b = ((xg - mb[:, None]) ** 2).sum(dim=(0, 2))
+        na, tot = n[b], n[b] + nb
+        d = mb - mean[b]
+        mean[b] += d * (nb / tot)
+        m2[b] += m2b + d * d * (na * nb / tot)
+        n[b] = tot
+    return n, mean, m2
 
 
 # ================================================ handlers ======================================================
@@ -174,37 +255,39 @@ def _gemm_spec(a, w, out, kw, hdt, prefix=""):
     dname = P + ("out_f32" if o32 is not None else "out")
 
     def chunks():
-        """Row ranges the float64 reference is built in (whole images for the convolutions): at most CHUNK_ELEMS
-        outputs at a time."""
-        step = max(1, CHUNK_ELEMS // max(N, 1))
-        if mode != LINEAR:
-            step = max(1, step // batch_rows) * batch_rows
-        return [(r0, min(M, r0 + step)) for r0 in range(0, M, step)]
+        """(first row, end row, label, image, first output row, end output row) of the bands the float64 reference
+        is built in, at most CHUNK_ELEMS outputs (and for a LINEAR problem CHUNK_ELEMS A elements) each: rows of M,
+        or for a convolution whole output rows of one image."""
+        if mode == LINEAR:
+            return [(r0, r1, f"rows {r0}-{r1 - 1}", None, None, None)
+                    for r0, r1 in bands(M, CHUNK_ELEMS // max(N, Ktot, 1))]
+        B, H, W_ = kw["conv"][:3]
+        return [(b * H * W_ + y0 * W_, b * H * W_ + y1 * W_, f"image {b} rows {y0}-{y1 - 1}", b, y0, y1)
+                for b in range(B) for y0, y1 in bands(H, CHUNK_ELEMS // max(N * W_, 1))]
 
     def check(snap, got):
-        A, Wd = snap(P + "a"), snap(P + "w")
-        bd = snap(P + "bias") if bias is not None else None
-        rvd = snap(P + "rowvec") if rv is not None else None
-        rsd = snap(P + "row_scale") if rs is not None else None
+        A, Wd = snap(P + "a"), _d(snap(P + "w"))
+        bd = _d(snap(P + "bias")) if bias is not None else None
+        rvd = _d(snap(P + "rowvec")) if rv is not None else None
+        rsd = _d(snap(P + "row_scale")) if rs is not None else None
         g_all = got(dname)
         parts = chunks()
-        for r0, r1 in parts:
-            tag = f"[rows {r0}:{r1}]" if len(parts) > 1 else ""
+        for r0, r1, label, b, y0, y1 in parts:
+            tag = _tag(parts, label)
             if mode == LINEAR:
-                Ac = A[r0:r1]
+                Ac = _d(A[r0:r1])
                 if ln is not None:
                     mu = Ac.mean(-1, keepdim=True)
                     r = (Ac.var(-1, correction=0, keepdim=True) + ln[2]).rsqrt()
                     pre = ((Ac - mu) * r) @ Wd.T
-                    e = (Ktot + 2) * U * r * (Ac.abs() @ Wd.abs().T + mu.abs() * snap(P + "ln_g").abs())
+                    e = (Ktot + 2) * U * r * (Ac.abs() @ Wd.abs().T + mu.abs() * _d(snap(P + "ln_g")).abs())
                 else:
                     pre = Ac @ Wd.T
                     mag = Ac.abs() @ Wd.abs().T
+                del Ac
             else:
-                b0, b1 = r0 // batch_rows, r1 // batch_rows
-                xe_ = snap(P + "a_extra")[b0:b1] if xe is not None else None
-                md = {CONV_S1: "s1", CONV_S2: "s2", CONV_S2A: "s2a"}[mode]
-                pre, mag = R.conv_gemm(A[b0:b1], Wd, md, xe_)
+                xe_ = snap(P + "a_extra")[b:b + 1] if xe is not None else None
+                pre, mag = conv_gemm_rows(A[b:b + 1], Wd, mode, y0, y1, xe_)
                 pre, mag = pre.reshape(r1 - r0, N), mag.reshape(r1 - r0, N)
             if ln is not None:
                 if bd is not None:
@@ -228,9 +311,9 @@ def _gemm_spec(a, w, out, kw, hdt, prefix=""):
                 n_scale += 1
             extras = []
             if res is not None:
-                extras.append(snap(P + "residual")[r0:r1])
+                extras.append(_d(snap(P + "residual")[r0:r1]))
             if acc:
-                extras.append(snap(dname)[r0:r1])
+                extras.append(_d(snap(dname)[r0:r1]))
             ref, bound = R.gemm_out(y, err, scale, extras, None if o32 is not None else hdt, n_scale)
             del y, err
             g = g_all[r0:r1]
@@ -285,11 +368,19 @@ def h_attention(be, a, hdt):
         o += [dense("rel_h", a["rel_h"], (B * heads, Nq, S)), dense("rel_w", a["rel_w"], (B * heads, Nq, S))]
 
     def check(snap, got):
-        sh = lambda t, n: t.reshape(B, n, heads, d)
-        ref, bound = attn_ref.attention_bound(sh(snap("q"), Nq), sh(snap("k"), Nkv), sh(snap("v"), Nkv), a["scale"],
-                                              snap("rel_h") if rel else None, snap("rel_w") if rel else None, S,
-                                              dtype=hdt)
-        yield "out", got("out"), ref.reshape(B, Nq, hd), bound.reshape(B, Nq, hd)
+        """One batch element and at most CHUNK_ELEMS outputs at a time: attention_bound upcasts K and V of one
+        (element, head) and builds its logits in chunks of query rows, so no float64 tensor is larger than those
+        plus one band's output and bound."""
+        sh = lambda t, n: t.reshape(1, n, heads, d)
+        parts = [(b, r0, r1) for b in range(B) for r0, r1 in bands(Nq, CHUNK_ELEMS // hd)]
+        for b, r0, r1 in parts:
+            hs = slice(b * heads, (b + 1) * heads)
+            ref, bound = attn_ref.attention_bound(sh(snap("q")[b:b + 1, r0:r1], r1 - r0), sh(snap("k")[b:b + 1], Nkv),
+                                                  sh(snap("v")[b:b + 1], Nkv), a["scale"],
+                                                  snap("rel_h")[hs, r0:r1] if rel else None,
+                                                  snap("rel_w")[hs, r0:r1] if rel else None, S, dtype=hdt)
+            yield ("out" + _tag(parts, f"batch {b} rows {r0}-{r1 - 1}"), got("out")[b:b + 1, r0:r1],
+                   ref.reshape(1, r1 - r0, hd), bound.reshape(1, r1 - r0, hd))
     return Spec("attention", o, check)
 
 
@@ -313,20 +404,76 @@ def h_groupnorm(be, a, hdt):
     o.append(dense("workspace", ws, (2 * B + 2 * groups * 256,), "scratch"))
 
     def check(snap, got):
-        xs = snap("x")
-        if x2 is not None:
-            xs = torch.cat([xs, snap("x2")], -1)
-        y, pre, terms = R.groupnorm(xs.reshape(B, HW, C), [snap(f"gamma{i}") for i in range(len(gl))],
-                                    [snap(f"beta{i}") for i in range(len(gl))], groups, a["eps"], a["silu"])
-        e = NORM_K * U * terms
-        bound = R.ulp(y, hdt) + (1.1 * e + R.silu_eval_err(pre) if a["silu"] else e)
-        yield "out", got("out"), y.reshape(B * HW, C), bound.reshape(B * HW, C)
+        """R.groupnorm in two passes.  Pass 1 walks each image one CTA's pixels at a time in the kernel's launch
+        geometry (R.gn_geometry): the per-(image, group) mean and M2 merged over the CTAs, and the running error
+        bound of the kernel's fp32 sums in their order (R.gn_cta_sums, R.gn_cross_cta).  Pass 2 builds y, the
+        pre-SiLU value, the rounding terms and the bound in bands of pixel rows.  The bound is the NORM_K-ulp one of
+        the kernel suite plus what R.gn_stats_err derives for the statistics beyond the NORM_K unit those terms
+        already give them; the worst ratio against the former alone is kept in `unit_worst`."""
+        cpg = C // groups
+        parts = [(b, p0, p1) for b in range(B) for p0, p1 in bands(HW, CHUNK_ELEMS // C)]
+
+        def band(b, p0, p1):
+            rws = slice(b * HW + p0, b * HW + p1)
+            xb = _d(snap("x")[rws])
+            if x2 is not None:
+                xb = torch.cat([xb, _d(snap("x2")[rws])], -1)
+            return xb.reshape(p1 - p0, groups, cpg)
+        ks = torch.stack([band(b, 0, 1)[0, :, 0] for b in range(B)])        # the kernel's shifts [B, groups]
+        n_sm = torch.cuda.get_device_properties(ks.device).multi_processor_count if ks.is_cuda else 132
+        chunks, ppc, lanes, nparts = R.gn_geometry(B, HW, C, groups, n_sm)
+        ctas = [(b, c * ppc, min(HW, (c + 1) * ppc)) for b in range(B) for c in range(chunks)]
+        sa, sq = torch.zeros_like(ks), torch.zeros_like(ks)
+        run = torch.zeros(B, 2, groups, dtype=torch.float64, device=ks.device)
+        totals = [[] for _ in range(B)]
+
+        def pass1():
+            for b, p0, p1 in ctas:
+                xg = band(b, p0, p1)
+                dk = xg - ks[b][:, None]
+                sa[b] += dk.abs().sum(dim=(0, 2))
+                sq[b] += (dk * dk).sum(dim=(0, 2))
+                t, r_ = R.gn_cta_sums(dk.reshape(p1 - p0, C), lanes, groups)
+                run[b] += r_
+                totals[b].append(t)
+                del dk
+                yield b, xg
+        n, mean, m2 = groupnorm_stats(pass1(), B, groups)
+        for b in range(B):
+            run[b] += R.gn_cross_cta(torch.stack(totals[b]), nparts)
+        nt = torch.tensor(n, dtype=torch.float64, device=m2.device)[:, None]
+        var = m2 / nt
+        r = (var + a["eps"]).rsqrt()
+        d_mean, d_rstd = R.gn_stats_err(run.permute(1, 0, 2), sa, sq, nt, mean - ks, var, a["eps"])
+        gs = [_d(snap(f"gamma{i}")) for i in range(len(gl))]
+        bs = [_d(snap(f"beta{i}")) for i in range(len(gl))]
+        per_net = B // len(gl)
+        for b, p0, p1 in parts:
+            g, bt = gs[b // per_net], bs[b // per_net]
+            y = ((band(b, p0, p1) - mean[b, :, None]) * r[b, :, None]).reshape(p1 - p0, C)
+            amu = (mean[b].abs() * r[b]).repeat_interleave(cpg)
+            pre = y * g + bt
+            terms = (y.abs() + amu + 1.0) * g.abs() + bt.abs()
+            ch = lambda t: t[b].repeat_interleave(cpg)
+            e = NORM_K * U * terms
+            excess = R.gn_stats_excess(y, g, ch(r), ch(d_mean), ch(d_rstd), NORM_K * U)
+            del y, terms
+            ref = R.silu(pre) if a["silu"] else pre
+            gb = got("out")[b * HW + p0:b * HW + p1]
+            unit = R.ulp(ref, hdt) + (1.1 * e + R.silu_eval_err(pre) if a["silu"] else e)
+            unit_worst[0] = max(unit_worst[0], R.worst_element(gb, ref, unit)[0])
+            bound = unit + (1.1 * excess if a["silu"] else excess)
+            del pre, e, excess, unit
+            yield "out" + _tag(parts, f"image {b} rows {p0}-{p1 - 1}"), gb, ref, bound
 
     def after(post):
         cnt = post("workspace")[:2 * B]
         if bool(_bits(cnt).ne(0).any()):
             yield "workspace", "arrival counters not zero after the call"
-    return Spec("groupnorm", o, check, after)
+    unit_worst = [0.0]
+    spec = Spec("groupnorm", o, check, after)
+    spec.unit_worst = unit_worst
+    return spec
 
 
 def h_layernorm(be, a, hdt):
@@ -335,9 +482,25 @@ def h_layernorm(be, a, hdt):
          rows("out", a["out"], M, C, a.get("ldo") or C, "w")]
 
     def check(snap, got):
-        y, terms = R.layernorm(snap("x"), snap("gamma"), snap("beta"), a["eps"])
-        yield "out", got("out"), y, R.ulp(y, hdt) + NORM_K * U * terms
+        g, b = _d(snap("gamma")), _d(snap("beta"))
+        parts = bands(M, CHUNK_ELEMS // C)
+        for r0, r1 in parts:
+            y, terms = R.layernorm(_d(snap("x")[r0:r1]), g, b, a["eps"])
+            yield "out" + _tag(parts, f"rows {r0}-{r1 - 1}"), got("out")[r0:r1], y, R.ulp(y, hdt) + NORM_K * U * terms
     return Spec("layernorm", o, check)
+
+
+def _conv_nhwc_bands(snap, k, s, B, Ho, Wo, Cout, has_bias):
+    """R.conv_nhwc(x, w, bias, stride=s) (pad k // 2) in bands of whole output rows of one image, at most CHUNK_ELEMS
+    outputs each: yields (label, image, y0, y1, out, sum of |x w| + |bias|)."""
+    w = _d(snap("w"))
+    bd = _d(snap("bias")) if has_bias else None
+    parts = [(b, y0, y1) for b in range(B) for y0, y1 in bands(Ho, CHUNK_ELEMS // max(Wo * Cout, 1))]
+    for b, y0, y1 in parts:
+        pre, mag = conv_rows(snap("x")[b:b + 1], w, k, s, k // 2, (k // 2, k // 2), y0, y1)
+        if bd is not None:
+            pre, mag = pre + bd, mag + bd.abs()
+        yield _tag(parts, f"image {b} rows {y0}-{y1 - 1}"), b, y0, y1, pre, mag
 
 
 def h_conv_direct(be, a, hdt):
@@ -353,14 +516,14 @@ def h_conv_direct(be, a, hdt):
     o.append(Operand("out", out, (B, Ho, Wo, Cout), (Ho * Wo * ldo, Wo * ldo, ldo, 1), out.storage_offset(), "w"))
 
     def check(snap, got):
-        pre, mag = R.conv_nhwc(snap("x"), snap("w"), snap("bias") if a.get("bias") is not None else None, stride=s)
-        e = (k * k * Cin + 1) * U * mag
-        y = pre
-        if a["silu"]:
-            y, e = R.silu(pre), 1.1 * e + R.silu_eval_err(pre)
-        ad = snap("add") if add is not None else torch.zeros_like(y)
-        ref = y + ad
-        yield "out", got("out"), ref, R.ulp(ref, hdt) + e + 2 * U * (y.abs() + ad.abs())
+        for tag, b, y0, y1, pre, mag in _conv_nhwc_bands(snap, k, s, B, Ho, Wo, Cout, a.get("bias") is not None):
+            e = (k * k * Cin + 1) * U * mag
+            y = pre
+            if a["silu"]:
+                y, e = R.silu(pre), 1.1 * e + R.silu_eval_err(pre)
+            ad = _d(snap("add")[b:b + 1, y0:y1]) if add is not None else torch.zeros_like(y)
+            ref = y + ad
+            yield "out" + tag, got("out")[b:b + 1, y0:y1], ref, R.ulp(ref, hdt) + e + 2 * U * (y.abs() + ad.abs())
     return Spec("conv_direct", o, check)
 
 
@@ -381,20 +544,26 @@ def h_conv_in(be, a, hdt):
         o.append(nhwc("out2", out2, a.get("ldo2") or Cout, "w"))
 
     def check(snap, got):
-        ref, mag = R.conv_nhwc(snap("x"), snap("w"), snap("bias") if a.get("bias") is not None else None)
-        ad = snap("add") if add is not None else torch.zeros_like(ref)
-        ref = ref + ad
-        g = got("out")
-        yield "out", g, ref, R.ulp(ref, hdt) + (9 * Cin + 2) * U * (mag + ad.abs())
-        if out2 is not None:
-            yield "out2", got("out2"), g, None
+        for tag, b, y0, y1, ref, mag in _conv_nhwc_bands(snap, 3, 1, B, H, W_, Cout, a.get("bias") is not None):
+            ad = _d(snap("add")[b:b + 1, y0:y1]) if add is not None else torch.zeros_like(ref)
+            ref = ref + ad
+            g = got("out")[b:b + 1, y0:y1]
+            yield "out" + tag, g, ref, R.ulp(ref, hdt) + (9 * Cin + 2) * U * (mag + ad.abs())
+            if out2 is not None:
+                yield "out2" + tag, got("out2")[b:b + 1, y0:y1], g, None
     return Spec("conv_in", o, check)
 
 
 def h_upsample2x(be, a, hdt):
     B, H, W_, C = a["B"], a["H"], a["W"], a["C_"]
     o = [dense("x", a["x"], (B, H, W_, C)), dense("out", a["out"], (B, 2 * H, 2 * W_, C), "w")]
-    return Spec("upsample2x", o, lambda snap, got: iter([("out", got("out"), R.upsample2x(snap("x")), None)]))
+
+    def check(snap, got):
+        parts = [(b, y0, y1) for b in range(B) for y0, y1 in bands(H, CHUNK_ELEMS // (4 * W_ * C))]
+        for b, y0, y1 in parts:
+            yield ("out" + _tag(parts, f"image {b} rows {2 * y0}-{2 * y1 - 1}"), got("out")[b:b + 1, 2 * y0:2 * y1],
+                   R.upsample2x(_d(snap("x")[b:b + 1, y0:y1])), None)
+    return Spec("upsample2x", o, check)
 
 
 def h_small_linear(be, a, hdt):
@@ -405,6 +574,7 @@ def h_small_linear(be, a, hdt):
     o.append(dense("y", a["y"], (M, N), "w"))
 
     def check(snap, got):
+        snap = _whole(snap)
         x, w = snap("x"), snap("w")
         ref, pre, mag = R.small_linear(x, w, snap("bias") if a.get("bias") is not None else None, a["silu_in"],
                                        a["silu_out"])
@@ -422,6 +592,7 @@ def h_timestep_embedding(be, a, hdt):
     o = [dense("t", a["t"], (B,)), dense("out", a["out"], (B, dim), "w")]
 
     def check(snap, got):
+        snap = _whole(snap)
         ref, arg, xf = R.timestep_embedding(snap("t"), dim)
         arg_err = (3 * xf[None].abs() + 4) * U * arg.abs()
         yield "out", got("out"), ref, torch.cat([arg_err, arg_err], dim=-1) + 4 * U
@@ -445,6 +616,7 @@ def _h_out(copies):
             o.append(dense("coef", a["coef"], (16 if hist is not None else 7 if noise is not None else 4,)))
 
         def check(snap, got):
+            snap = _whole(snap)
             eps, mag = R.out_conv(snap("xn"), snap("w"), snap("bias"))
             eb = (9 * C + 1) * U * mag
             if a.get("eps_out") is not None:
@@ -502,6 +674,7 @@ def h_step_gather(be, a, hdt):
         o += [dense(f"table{i}", t, (n_rows, d.numel())), dense(f"dst{i}", d, (d.numel(),), "w")]
 
     def check(snap, got):
+        snap = _whole(snap)
         r = max(0, min(int(snap("step_counter")[0]), n_rows - 1))
         for i in range(len(a["tables"])):
             yield f"dst{i}", got(f"dst{i}"), snap(f"table{i}")[r], None
@@ -516,6 +689,7 @@ def h_sam_relpos(be, a, hdt):
          dense("rel_h", a["rel_h"], (B * heads, S * S, S), "w"), dense("rel_w", a["rel_w"], (B * heads, S * S, S), "w")]
 
     def check(snap, got):
+        snap = _whole(snap)
         rh, rw, mh, mw = R.sam_relpos(snap("q").reshape(B, S * S, heads, d), snap("Rh"), snap("Rw"))
         yield "rel_h", got("rel_h"), rh, (d + 1) * U * mh
         yield "rel_w", got("rel_w"), rw, (d + 1) * U * mw
@@ -530,7 +704,7 @@ def h_window_partition(be, a, hdt):
     B, H, W_, C, ws = a["B"], a["H"], a["W"], a["C_"], a["ws"]
     o = [dense("x", a["x"], (B, H, W_, C)), dense("out", a["out"], (B * _n_win(H, W_, ws), ws, ws, C), "w")]
     return Spec("window_partition", o,
-                lambda snap, got: iter([("out", got("out"), R.window_partition(snap("x"), ws), None)]))
+                lambda snap, got: iter([("out", got("out"), R.window_partition(_d(snap("x")), ws), None)]))
 
 
 def h_window_unpartition(be, a, hdt):
@@ -542,6 +716,7 @@ def h_window_unpartition(be, a, hdt):
     o.append(dense("out", a["out"], (B, H, W_, C), "w"))
 
     def check(snap, got):
+        snap = _whole(snap)
         ref = R.window_unpartition(snap("xw"), B, H, W_, ws)
         if res is None:
             yield "out", got("out"), ref, None
@@ -555,13 +730,20 @@ def h_sam_patchify(be, a, hdt):
     B, Cin, H, W_, ps = a["B"], a["Cin"], a["H"], a["W"], a["ps"]
     o = [dense("img", a["img"], (B, Cin, H, W_)),
          dense("out", a["out"], (B * (H // ps) * (W_ // ps), Cin * ps * ps), "w")]
-    return Spec("sam_patchify", o, lambda snap, got: iter([("out", got("out"), R.sam_patchify(snap("img"), ps), None)]))
+    return Spec("sam_patchify", o,
+                lambda snap, got: iter([("out", got("out"), R.sam_patchify(_d(snap("img")), ps), None)]))
 
 
 def h_nhwc_to_nchw_f32(be, a, hdt):
     B, HW, C = a["B"], a["HW"], a["C_"]
     o = [dense("x", a["x"], (B, HW, C)), dense("out", a["out"], (B, C, HW), "w")]
-    return Spec("nhwc_to_nchw_f32", o, lambda snap, got: iter([("out", got("out"), R.nhwc_to_nchw(snap("x")), None)]))
+
+    def check(snap, got):
+        parts = [(b, p0, p1) for b in range(B) for p0, p1 in bands(HW, CHUNK_ELEMS // C)]
+        for b, p0, p1 in parts:
+            yield ("out" + _tag(parts, f"image {b} pixels {p0}-{p1 - 1}"), got("out")[b:b + 1, :, p0:p1],
+                   R.nhwc_to_nchw(_d(snap("x")[b:b + 1, p0:p1])), None)
+    return Spec("nhwc_to_nchw_f32", o, check)
 
 
 def h_softmax_rows(be, a, hdt):
@@ -569,8 +751,10 @@ def h_softmax_rows(be, a, hdt):
     o = [rows("s", a["s"], r, c, a.get("lds") or c), rows("p", a["p"], r, c, a.get("ldp") or c, "w")]
 
     def check(snap, got):
-        ref = R.softmax_rows(snap("s"))
-        yield "p", got("p"), ref, R.ulp(ref, hdt) + 1e-5 * ref.abs()
+        parts = bands(r, CHUNK_ELEMS // c)
+        for r0, r1 in parts:
+            ref = R.softmax_rows(_d(snap("s")[r0:r1]))
+            yield "p" + _tag(parts, f"rows {r0}-{r1 - 1}"), got("p")[r0:r1], ref, R.ulp(ref, hdt) + 1e-5 * ref.abs()
     return Spec("softmax_rows", o, check)
 
 
@@ -579,8 +763,13 @@ def h_image_out(be, a, hdt):
     o = [Operand("x", a["x"], (B, HW, C), (HW * ldx, ldx, 1), a["x"].storage_offset(), "r"),
          dense("out", a["out"], (B, C, HW), "w")]
     sc = (a["scale"], a["shift"], a["lo"], a["hi"])
-    return Spec("image_out", o,
-                lambda snap, got: iter([("out", got("out"), R.image_out(snap("x"), C, *sc), None)]))
+
+    def check(snap, got):
+        parts = [(b, p0, p1) for b in range(B) for p0, p1 in bands(HW, CHUNK_ELEMS // C)]
+        for b, p0, p1 in parts:
+            yield ("out" + _tag(parts, f"image {b} pixels {p0}-{p1 - 1}"), got("out")[b:b + 1, :, p0:p1],
+                   R.image_out(_d(snap("x")[b:b + 1, p0:p1]), C, *sc), None)
+    return Spec("image_out", o, check)
 
 
 HANDLERS = {"gemm": h_gemm, "gemm_grouped": h_gemm_grouped, "attention": h_attention, "groupnorm": h_groupnorm,
@@ -655,7 +844,13 @@ class Auditor:
         self.enabled = True     # False: forward launches unchecked (auditing chosen layers of a large network)
         self.unaudited = 0
         self.worst = {}
+        self.worst_unit = {}    # GroupNorm: worst error / the bound without the derived statistics term
         self.counts = {}
+        # CUDA only: the device's peak allocation over the audited calls (the auditor resets the peak statistics at
+        # every call, so a caller reads max(this, torch.cuda.max_memory_allocated())), and the largest growth during
+        # one call over what was allocated when it started: the auditor's own snapshots, copies and references
+        self.peak_bytes = 0
+        self.own_peak_bytes = 0
 
     def __getattr__(self, name):
         fn = getattr(self.be, name)
@@ -692,6 +887,19 @@ class Auditor:
         raise AuditError(f"{self.case}: call {where[2]} ops.{where[0]} at {where[1]}, operand {operand}: {msg}")
 
     def _audit(self, name, fn, handler, a):
+        dev = next(iter(_tensors(a))).device
+        if dev.type != "cuda":
+            return self._audit_call(name, fn, handler, a)
+        self.peak_bytes = max(self.peak_bytes, torch.cuda.max_memory_allocated(dev))
+        torch.cuda.reset_peak_memory_stats(dev)
+        base = torch.cuda.memory_allocated(dev)
+        r = self._audit_call(name, fn, handler, a)
+        peak = torch.cuda.max_memory_allocated(dev)
+        self.peak_bytes = max(self.peak_bytes, peak)
+        self.own_peak_bytes = max(self.own_peak_bytes, peak - base)
+        return r
+
+    def _audit_call(self, name, fn, handler, a):
         hdt = self.be.half_dtype()
         spec = handler(self.be, a, hdt)            # may fill in an output the operator would allocate itself
         self.calls += 1
@@ -747,8 +955,12 @@ class Auditor:
                                                                f"in {int(d.sum())} elements: a read outside the "
                                                                f"declared operands reaches the result"
                                                                + self._culprit(fn, a, spec, storages, snap, written))
+            del fenced
+        del written
         self._check(spec, snap, storages, where)
         key = where[:2]
+        if hasattr(spec, "unit_worst"):
+            self.worst_unit[key] = max(self.worst_unit.get(key, 0.0), spec.unit_worst[0])
         self.counts[key] = self.counts.get(key, 0) + 1
         if name == "gemm":
             return a["out"] if a.get("out") is not None else a["out_f32"]
@@ -766,14 +978,10 @@ class Auditor:
 
     def _check(self, spec, snap, storages, where):
         ops_ = {o.name: o for o in spec.operands}
-        cache = {}
         key = where[:2]
 
         def s(n):
-            if n not in cache:
-                v = snap.pre(ops_[n])
-                cache[n] = v.double() if v.is_floating_point() else v.long()
-            return cache[n]
+            return snap.pre(ops_[n])
 
         def g(n):
             o = ops_[n]

@@ -1,21 +1,19 @@
 """-m gpu: the tile-refinement sizes on one H100.  The SD VAE encodes a 2048 x 2752 image and decodes 256 x 344
 latents (N = 88064 attention tokens, past vae.FUSED_ATTN_MIN_TOKENS: the AttnBlock runs ea_attention) with graphs
-on, within a fraction of the N x N logits the GEMM path would store; its mid blocks (ResnetBlock, AttnBlock,
-ResnetBlock) pass the launch auditor at that size; the decoder matches the fp32 oracle at 128 x 128 latents on both
+on, within a fraction of the N x N logits the GEMM path would store (tests/test_gpu_highres_audit.py audits every
+launch at that size); the decoder matches the fp32 oracle at 128 x 128 latents on both
 AttnBlock paths; and the SD1.5 tile pass runs end to end at 2048 x 2752."""
 import numpy as np
 import PIL.Image
 import pytest
 import torch
 
-from editanything_b200 import ops
 from editanything_b200.denoise import DenoiseEngine
 from editanything_b200.pipeline import StableDiffusionControlNetInpaintPipeline
 from editanything_b200 import vae as vae_mod
 from editanything_b200.unet_spec import SD15, make_state_dict
-from editanything_b200.vae import SD_VAE, VaeDecoderEngine, VaeEncoderEngine, VaeEngine, make_vae_state_dict
+from editanything_b200.vae import SD_VAE, VaeDecoderEngine, VaeEngine, make_vae_state_dict
 from oracle import vae_oracle as V
-from tests.launch_audit import Auditor
 
 pytestmark = pytest.mark.gpu
 DEV = torch.device("cuda", 0)
@@ -57,37 +55,6 @@ def test_vae_2048x2752_graphed():
     print(f"peak allocation growth: encode {grow_e / 2**30:.2f} GiB, decode {grow_d / 2**30:.2f} GiB "
           f"(N^2 half = {N2_HALF / 2**30:.2f} GiB)")
     assert grow_e < N2_HALF and grow_d < N2_HALF
-
-
-def _audit_mid(eng, aud):
-    """Enable the auditor on the engine's mid ResnetBlocks and AttnBlock only."""
-    res, attn = eng._res, eng._attn
-
-    def wrap(fn):
-        def run(p, *args):
-            aud.enabled = ".mid." in "." + p
-            try:
-                return fn(p, *args)
-            finally:
-                aud.enabled = False
-        return run
-    eng._res, eng._attn = wrap(res), wrap(attn)
-    aud.enabled = False
-
-
-def test_vae_2048x2752_mid_blocks_audited():
-    for part, Eng in (("decoder", VaeDecoderEngine), ("encoder", VaeEncoderEngine)):
-        aud = Auditor(ops, f"sd_vae_{part}_{H}x{W}_mid")
-        eng = Eng(SD_VAE, make_vae_state_dict(SD_VAE, 7, part=part), DEV, backend=aud)
-        _audit_mid(eng, aud)
-        g = torch.Generator().manual_seed(1)
-        if part == "decoder":
-            eng.decode_latents(torch.randn(1, 4, H // 8, W // 8, generator=g), use_graph=False)
-        else:
-            eng.encode(torch.rand(1, 3, H, W, generator=g) * 2 - 1, use_graph=False)
-        torch.cuda.synchronize()
-        assert aud.calls >= 5, (part, aud.calls)      # GroupNorm + conv x 2 per ResnetBlock, ... the attention
-        print(f"{part}: {aud.calls} audited launches")
 
 
 @pytest.mark.parametrize("fused", [False, True])

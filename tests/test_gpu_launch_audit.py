@@ -30,20 +30,24 @@ pytestmark = pytest.mark.gpu
 
 DEV = torch.device("cuda", 0)
 WORST = {}          # (op, call site) -> worst error / bound over every case
-RUNS = {}           # case -> (audited launches, seconds, peak GiB)
+WORST_UNIT = {}     # GroupNorm (op, call site) -> the same without the derived statistics term
+RUNS = {}           # case -> (audited launches, seconds, peak GiB, the auditor's own peak GiB)
 
 
 @pytest.fixture(scope="module", autouse=True)
 def _report():
     yield
     if RUNS:
-        print("\naudited launches, wall time and peak device memory per case:")
-        for k, (n, s, m) in RUNS.items():
-            print(f"  {k:32s} {n:5d} launches  {s:7.1f} s  {m:6.2f} GiB")
+        print("\naudited launches, wall time, peak device memory and the auditor's own largest growth in one call, "
+              "per case:")
+        for k, (n, s, m, own) in RUNS.items():
+            print(f"  {k:32s} {n:5d} launches  {s:7.1f} s  {m:6.2f} GiB  auditor {own:6.2f} GiB")
     if WORST:
         print("worst error / bound per (op, call site):")
         for (op, site), v in sorted(WORST.items()):
-            print(f"  {op:20s} {site:18s} {v:.3f}")
+            unit = f"  (without the derived statistics term: {WORST_UNIT[(op, site)]:.3f})" if (op, site) in WORST_UNIT \
+                else ""
+            print(f"  {op:20s} {site:18s} {v:.3f}{unit}")
 
 
 def _audited(case, body):
@@ -53,9 +57,12 @@ def _audited(case, body):
     t0 = time.perf_counter()
     body(aud)
     torch.cuda.synchronize()
-    RUNS[case] = (aud.calls, time.perf_counter() - t0, torch.cuda.max_memory_allocated(DEV) / 2 ** 30)
+    peak = max(aud.peak_bytes, torch.cuda.max_memory_allocated(DEV))      # the auditor resets the peak per call
+    RUNS[case] = (aud.calls, time.perf_counter() - t0, peak / 2 ** 30, aud.own_peak_bytes / 2 ** 30)
     for k, v in aud.worst.items():
         WORST[k] = max(WORST.get(k, 0.0), v)
+    for k, v in aud.worst_unit.items():
+        WORST_UNIT[k] = max(WORST_UNIT.get(k, 0.0), v)
     assert aud.calls > 0
     return aud
 
