@@ -88,6 +88,7 @@ SYMBOLS = {
     "ea_out_ddim": (_I, [_P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _P]),
     "ea_out_cfg_vpred": (_I, [_P, _P, _P, _P, _P, _P, _F, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _P]),
     "ea_out_vpred": (_I, [_P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _P]),
+    "ea_latent_mix": (_I, [_P, _P, _P, _P, _P, _F, _P, _I, _P, _I, _I, _I, _I, _P]),
     "ea_step_gather": (_I, [_P, _I, _I, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.POINTER(C.c_longlong), _P]),
     "ea_sam_relpos": (_I, [_P, _L, _L, _P, _P, _P, _P, _I, _I, _I, _I, _P]),
     "ea_window_partition": (_I, [_P, _P, _I, _I, _I, _I, _I, _P]),

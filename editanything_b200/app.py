@@ -56,8 +56,14 @@ and text encoder of the current one when the LoRA lists match), the mask is all 
 text-to-image `StableDiffusionControlNetPipeline` runs with the SAM ControlNet alone; without it the inpaint pipeline
 repaints the whole image.  The tile pass then runs as usual.
 
-Not supported here (raise NotImplementedError instead of diverging silently): reference-only mode (`ref_image`),
-the alpha-mixing pipeline.
+Alpha mixing: with a `StableDiffusionControlNetInpaintMixingPipeline` injected as `pipe` (and as `tile_model`), the
+main pass gets `alpha_weight` and, with `use_scale_map`, the ControlNet scale map 1 - mask of the source mask, and
+the tile pass gets `alpha_weight`, `refine_alignment_ratio` and the same map (editany_lora.py:829-856, :902-918).
+Like the reference, the constructor never builds that pipeline itself, and a plain tile pipeline next to a mixing
+`pipe` raises TypeError on `alpha_weight`.
+
+Not supported here (raise NotImplementedError instead of diverging silently): reference-only mode (`ref_image`) and
+the constructor's `alpha_mixing` argument.
 """
 import copy
 import os
@@ -272,6 +278,7 @@ class EditAnythingLoraModel:
                 ref_prompt=None, ref_sam_scale=None, ref_inpaint_scale=None, ref_auto_prompt=False, ref_textinv=True,
                 ref_textinv_path=None, ref_scale=None):
         """editany_lora.py:609-938 -> (results_tile: list[PIL], results: list[PIL], [full_segmask, mask], prompt)."""
+        from .pipeline import StableDiffusionControlNetInpaintMixingPipeline, prepare_mask_image
         if ref_image is not None:
             raise NotImplementedError("reference-only mode (utils/stable_diffusion_reference.py) is not implemented")
         this_controlnet_path = self.default_controlnet_path if condition_model in (None, "EditAnything") else condition_model
@@ -330,13 +337,24 @@ class EditAnythingLoraModel:
             if self.extra_inpaint:
                 multi_condition_image.append(make_inpaint_condition(img, mask_image_tmp).type(torch.float16))
                 multi_condition_scale.append(1.0)
-            # use_scale_map: the reference builds the map (:838-848) but hands it only to the alpha-mixing pipeline
-            x_samples = self.pipe(image=img, mask_image=mask_image, prompt_embeds=prompt_embeds,
-                                  negative_prompt_embeds=negative_prompt_embeds, num_images_per_prompt=num_samples,
-                                  num_inference_steps=ddim_steps, generator=generator,
-                                  controlnet_conditioning_image=multi_condition_image, height=H, width=W,
-                                  controlnet_conditioning_scale=multi_condition_scale, guidance_scale=scale,
-                                  guess_mode=guess_mode).images
+            scale_map = None
+            if use_scale_map:                                              # :829-839: 1 outside the edit mask
+                tmp = cv2.resize(HWC3(source_image["mask"].astype(np.uint8)), (W, H), interpolation=cv2.INTER_LINEAR)
+                scale_map = 1.0 - prepare_mask_image(PIL.Image.fromarray(tmp)).float()
+            if isinstance(self.pipe, StableDiffusionControlNetInpaintMixingPipeline):     # :841-856
+                x_samples = self.pipe(image=img, mask_image=mask_image, prompt_embeds=prompt_embeds,
+                                      negative_prompt_embeds=negative_prompt_embeds, num_images_per_prompt=num_samples,
+                                      num_inference_steps=ddim_steps, generator=generator,
+                                      controlnet_conditioning_image=multi_condition_image, height=H, width=W,
+                                      controlnet_conditioning_scale=multi_condition_scale, guidance_scale=scale,
+                                      alpha_weight=alpha_weight, controlnet_conditioning_scale_map=scale_map).images
+            else:
+                x_samples = self.pipe(image=img, mask_image=mask_image, prompt_embeds=prompt_embeds,
+                                      negative_prompt_embeds=negative_prompt_embeds, num_images_per_prompt=num_samples,
+                                      num_inference_steps=ddim_steps, generator=generator,
+                                      controlnet_conditioning_image=multi_condition_image, height=H, width=W,
+                                      controlnet_conditioning_scale=multi_condition_scale, guidance_scale=scale,
+                                      guess_mode=guess_mode).images
         results = [x_samples[i] for i in range(num_samples)]
 
         results_tile = []
@@ -349,10 +367,16 @@ class EditAnythingLoraModel:
                 if i == 0:
                     mask_image_tile = PIL.Image.fromarray(cv2.resize(mask_imag_ori, (img_tile.size[0], img_tile.size[1]),
                                                                      interpolation=cv2.INTER_LINEAR))
-                results_tile += self.tile_pipe(
-                    image=img_tile, mask_image=mask_image_tile, prompt_embeds=prompt_embeds,
-                    negative_prompt_embeds=negative_prompt_embeds, num_images_per_prompt=1,
-                    num_inference_steps=ddim_steps, generator=generator, controlnet_conditioning_image=img_tile,
-                    height=img_tile.size[1], width=img_tile.size[0], controlnet_conditioning_scale=1.0,
-                    alignment_ratio=refine_alignment_ratio, guidance_scale=scale, guess_mode=guess_mode).images
+                kw = dict(image=img_tile, mask_image=mask_image_tile, prompt_embeds=prompt_embeds,
+                          negative_prompt_embeds=negative_prompt_embeds, num_images_per_prompt=1,
+                          num_inference_steps=ddim_steps, generator=generator, controlnet_conditioning_image=img_tile,
+                          height=img_tile.size[1], width=img_tile.size[0], controlnet_conditioning_scale=1.0,
+                          alignment_ratio=refine_alignment_ratio, guidance_scale=scale)
+                if isinstance(self.pipe, StableDiffusionControlNetInpaintMixingPipeline):   # :902-918
+                    # the main pass's map, at the main pass's size; a plain tile pipeline refuses alpha_weight
+                    # (TypeError), as in the reference
+                    kw.update(alpha_weight=alpha_weight, controlnet_conditioning_scale_map=scale_map)
+                else:
+                    kw.update(guess_mode=guess_mode)
+                results_tile += self.tile_pipe(**kw).images
         return results_tile, results, [full_segmask, mask_image], postive_prompt

@@ -563,6 +563,46 @@ __global__ void out_ddim_kernel(const ea_half* __restrict__ xn, const float* __r
   }
 }
 
+// ---------------- alpha-mixing of the latents (last kernel of a mixing pipeline's step) -------------
+// utils/stable_diffusion_controlnet_inpaint.py:2039-2051, after the scheduler update of step r = *ctr - 1 (the
+// epilogue before this kernel has advanced the counter).  One thread per latent pixel (4 fp32 channels).
+//   p = k_init * known + k_noise * noise[r]                    (add_noise(init, randn, t_{r+1}))
+//   x = m * (in_window ? p : x) + (1 - m) * ((1 - alpha) x + alpha p)
+// Rows with active == 0 (the last step) and counters outside [1, n_rows] leave everything untouched.
+__global__ void latent_mix_kernel(float* __restrict__ latents, const float* __restrict__ known,
+                                  const float* __restrict__ mask, const float* __restrict__ noise,
+                                  const float* __restrict__ mix, float alpha, const int* __restrict__ ctr,
+                                  int n_rows, ea_half* __restrict__ lat_half, int copies, long long npix) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const int r = *ctr - 1;
+  if (r < 0 || r >= n_rows) return;
+  const float k_init = mix[r * 4 + 0], k_noise = mix[r * 4 + 1], in_window = mix[r * 4 + 2];
+  if (mix[r * 4 + 3] == 0.f) return;
+  const float* z = noise + (long long)r * npix * 4;
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  for (long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x; p < npix; p += stride) {
+    const float m = mask[p];
+    const float4 x = reinterpret_cast<const float4*>(latents)[p];
+    const float4 k = __ldg(reinterpret_cast<const float4*>(known) + p);
+    const float4 n = __ldg(reinterpret_cast<const float4*>(z) + p);
+    float xv[4] = {x.x, x.y, x.z, x.w};
+    const float kv[4] = {k.x, k.y, k.z, k.w}, nv[4] = {n.x, n.y, n.z, n.w};
+#pragma unroll
+    for (int c = 0; c < 4; ++c) {
+      const float pv = k_init * kv[c] + k_noise * nv[c];
+      const float keep = in_window != 0.f ? pv : xv[c];
+      xv[c] = keep * m + ((1.f - alpha) * xv[c] + alpha * pv) * (1.f - m);
+    }
+    reinterpret_cast<float4*>(latents)[p] = make_float4(xv[0], xv[1], xv[2], xv[3]);
+    if (lat_half) {
+      ea_half h4[4] = {ea_f2h(xv[0]), ea_f2h(xv[1]), ea_f2h(xv[2]), ea_f2h(xv[3])};
+      const uint2 hv = *reinterpret_cast<const uint2*>(h4);
+      for (int c = 0; c < copies; ++c) reinterpret_cast<uint2*>(lat_half)[c * npix + p] = hv;
+    }
+  }
+}
+
 // ---------------- per-step table gather (first kernel of a captured denoising step) -------------
 // Everything that changes from step to step (the scheduler coefficients and every net's time-embedding rows)
 // lives in device tables with one row per step; this kernel copies row min(*ctr, n_rows - 1) of each table into
@@ -1045,6 +1085,20 @@ extern "C" int ea_out_vpred(const void* xn, const float* w, const float* bias, f
                             void* stream) {
   return launch_out_ddim<false, true>(xn, w, bias, latents, eps_out, coef, 0.f, known, noise, mask, lat_half_out,
                                       step_counter, hist, Nimg, H, W, C, stream);
+}
+
+extern "C" int ea_latent_mix(float* latents, const float* known, const float* mask, const float* noise,
+                             const float* mix, float alpha, const int* step_counter, int n_rows, void* lat_half_out,
+                             int copies, int Nimg, int H, int W, void* stream) {
+  if (!latents || !known || !mask || !noise || !mix || !step_counter) return EA_ERR_ARG;
+  if (copies != 1 && copies != 2) return EA_ERR_ARG;
+  if (Nimg < 1 || H < 1 || W < 1 || n_rows < 1) return EA_ERR_SHAPE;
+  const uintptr_t a16 = (uintptr_t)latents | (uintptr_t)known | (uintptr_t)noise;
+  if ((a16 & 15) != 0 || ((uintptr_t)lat_half_out & 7) != 0) return EA_ERR_SHAPE;
+  const long long npix = (long long)Nimg * H * W;
+  ea_launch(latent_mix_kernel, dim3(grid_for(npix, 256)), dim3(256), (size_t)0, EA_STREAM(stream), latents, known,
+            mask, noise, mix, alpha, step_counter, n_rows, reinterpret_cast<ea_half*>(lat_half_out), copies, npix);
+  return EA_LAUNCH_OK();
 }
 
 extern "C" int ea_step_gather(const int* step_counter, int n_rows, int n_tables, const float* const* src,

@@ -224,7 +224,8 @@ class DenoiseEngine:
 
     # -- the sampling schedule as device tables -------------------------------------------------
     @engine_call
-    def set_schedule(self, timesteps, alphas, alphas_prev, blend=None, multistep=None, prediction_type="epsilon"):
+    def set_schedule(self, timesteps, alphas, alphas_prev, blend=None, multistep=None, prediction_type="epsilon",
+                     mix=None):
         """Everything that changes from step to step of the loop (utils/...inpaint.py:1540-1656), as device
         tables with one row per step: the DDIM coefficients (cldm/ddim_hacked.py:203-231), the per-ResBlock
         time-embedding rows of every net, and the inpaint-blend terms.  `blend` = (k_init[S], k_noise[S],
@@ -233,9 +234,21 @@ class DenoiseEngine:
         the kept region is `known` itself on every step.  The captured step indexes the tables with a device
         counter (ea_step_gather), so the host issues ONE graph launch per step.
         prediction_type: what the UNet predicts, "epsilon" or "v_prediction" (SD2.1-768; the update converts v to
-        x0 and eps, cldm/ddim_hacked.py:194-217) - the scheduler's `config.prediction_type`."""
+        x0 and eps, cldm/ddim_hacked.py:194-217) - the scheduler's `config.prediction_type`.
+        mix = (k_init[S], k_noise[S], in_window[S], active[S]): the alpha-mixing pipeline's per-step mix
+        (utils/...inpaint.py:2039-2051), run by ea_latent_mix after the step's update with the noise table and alpha
+        given to begin(); the update's own blend is then off.  Without `mix` the step has no such launch."""
         if prediction_type not in PREDICTION_TYPES:
             raise ValueError(f"prediction_type must be one of {PREDICTION_TYPES}, got {prediction_type!r}")
+        if mix is not None and blend is not None:
+            raise ValueError("a schedule takes the inpaint blend or the alpha mix, not both")
+        if mix is not None and (len(mix) != 4 or any(len(col) != len(timesteps) for col in mix)):
+            raise ValueError(f"mix = (k_init, k_noise, in_window, active), one value per step each "
+                             f"({len(timesteps)} steps)")
+        new_mix = None if mix is None else torch.tensor(list(zip(*mix)), dtype=torch.float32).to(self.dev)
+        if (new_mix is None) != (getattr(self, "mix_tab", None) is None):
+            self._graph = None        # the step gains or loses its ea_latent_mix launch
+        self._keep("mix_tab", new_mix)
         if prediction_type != self.prediction_type:
             self._graph = None        # the step's last launch differs (ea_out_*ddim / ea_out_*vpred)
         self.prediction_type = prediction_type
@@ -301,7 +314,10 @@ class DenoiseEngine:
                              [self.coef_dev] + self.emb_bufs)
         xn = self.runner.eps_features(self.x_half, self.t_dev, self.ctx_cache, self.hints, self.scales, self.gn_ws,
                                       embs=self.emb_bufs, ctx_ls=self.ctx_ls, cond_in=self._step_cond())
-        kw = dict(latents=self.lat, coef=self.coef_dev, known=self.known, noise=self.noise, mask=self.mask,
+        mixing = self.mix_tab is not None
+        # the alpha mix replaces the update's blend: the epilogue then reads no known / noise / mask
+        kw = dict(latents=self.lat, coef=self.coef_dev, known=None if mixing else self.known,
+                  noise=None if mixing else self.noise, mask=None if mixing else self.mask,
                   lat_half_out=self.x_half, step_counter=self.step_ctr, hist=self.hist, H=H, W=W_,
                   C_=self.cfg.model_channels)
         if self.prediction_type != "epsilon":
@@ -311,6 +327,12 @@ class DenoiseEngine:
                                   Nimg=self.B // 2, **kw)
         else:
             self.ops.out_ddim(xn, self.unet.w["out.w"], self.unet.w["out.cb"], Nimg=self.B, **kw)
+        if mixing:
+            if self.mix_noise is None or self.mix_alpha is None:
+                raise RuntimeError("a schedule with `mix` needs begin(..., mix_alpha=, mix_noise=)")
+            self.ops.latent_mix(self.lat, self.known, self.mask, self.mix_noise, self.mix_tab, alpha=self.mix_alpha,
+                                step_counter=self.step_ctr, lat_half_out=self.x_half, copies=2 if self.guided else 1,
+                                Nimg=self.lat.shape[0], H=H, W=W_)
 
     def _step_cond(self):
         if self.unet.x_channels == self.cfg.in_channels:
@@ -320,12 +342,16 @@ class DenoiseEngine:
         return self.cond_in
 
     @engine_call
-    def begin(self, latents_nchw, guidance, known_nchw=None, mask_n1hw=None, noise_nchw=None, use_graph=True):
+    def begin(self, latents_nchw, guidance, known_nchw=None, mask_n1hw=None, noise_nchw=None, use_graph=True,
+              mix_alpha=None, mix_noise=None):
         """latents: fp32 [N, 4, h, w] initial noise (N = B/2 images, or B without guidance; `guidance` is then
         unused).  known/mask: optional inpaint blend tensors (mask == 1 keeps `known`,
         utils/...inpaint.py:1484-1489,1647-1664); noise: the initial latent noise the kept region is re-noised with
         (:1446,1650).  The blend buffers always exist (an all-zero mask is an exact no-op), so switching the blend on,
-        off or ending its window never re-captures the graph."""
+        off or ending its window never re-captures the graph.
+        mix_alpha / mix_noise: for a schedule with `mix`, the alpha-mixing weight and the noise drawn for each
+        step's mix, [R, N, 4, h, w] with R <= the number of steps (row i mixes after step i; steps without a row are
+        inactive in the schedule); known / mask are then the source latents and the keep mask it mixes with."""
         def nhwc(t):
             return t.to(self.dev, torch.float32).permute(0, 2, 3, 1).contiguous()
         lat = nhwc(latents_nchw)
@@ -350,6 +376,20 @@ class DenoiseEngine:
         self._keep("mask", m)
         # history of the multistep schedulers (x0 predictions of the two previous steps, previous corrected sample)
         self._keep("hist", torch.zeros((3,) + tuple(lat.shape), device=self.dev, dtype=torch.float32))
+        if mix_noise is not None:
+            S = self.mix_tab.shape[0] if getattr(self, "mix_tab", None) is not None else 0
+            if mix_noise.dim() != 5 or mix_noise.shape[0] > S or tuple(mix_noise.shape[1:]) != tuple(latents_nchw.shape):
+                raise ValueError(f"mix_noise {tuple(mix_noise.shape)}: expected [R <= {S} steps of a schedule with "
+                                 f"mix, {', '.join(map(str, latents_nchw.shape))}]")
+            z = torch.zeros((S,) + tuple(lat.shape), device=self.dev, dtype=torch.float32)
+            z[:mix_noise.shape[0]] = mix_noise.to(self.dev, torch.float32).permute(0, 1, 3, 4, 2)
+            self._keep("mix_noise", z)
+        else:
+            self._keep("mix_noise", None)
+        a = None if mix_alpha is None else float(mix_alpha)
+        if getattr(self, "mix_alpha", None) != a:
+            self._graph = None        # alpha is an argument of the captured ea_latent_mix launch
+        self.mix_alpha = a
         use = use_graph and self.dev.type == "cuda"
         if use != getattr(self, "_use_graph", None):
             self._graph = None
@@ -367,6 +407,17 @@ class DenoiseEngine:
         (utils/...inpaint.py:1647-1656) - for callers that must observe the un-blended latents first."""
         m = self.mask[..., None]
         self.lat.copy_((k_init * self.known + k_noise * self.noise) * m + self.lat * (1 - m))
+        self.x_half.copy_(torch.cat([self.lat] * (2 if self.guided else 1)).to(self.hdt))
+
+    @engine_call
+    def mix_now(self, k_init, k_noise, in_window, alpha, noise_nchw):
+        """The alpha mix of ea_latent_mix outside the fused step (utils/...inpaint.py:2039-2051), with `known` /
+        `mask` of begin() and this step's noise [N, 4, h, w] - for callers that must observe the un-mixed latents
+        first."""
+        m = self.mask[..., None]
+        p = k_init * self.known + k_noise * noise_nchw.to(self.dev, torch.float32).permute(0, 2, 3, 1)
+        keep = p if in_window else self.lat
+        self.lat.copy_(keep * m + ((1 - alpha) * self.lat + alpha * p) * (1 - m))
         self.x_half.copy_(torch.cat([self.lat] * (2 if self.guided else 1)).to(self.hdt))
 
     @engine_call

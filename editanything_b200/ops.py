@@ -350,6 +350,34 @@ def out_ddim(xn, w, bias, *, latents=None, eps_out=None, coef=None, known=None, 
             name)
 
 
+def check_mix_buffers(latents, known, mask, noise, mix, step_counter, lat_half_out, copies, Nimg, H, W):
+    """The element counts of ea_latent_mix's buffers, checked before the launch (the kernel indexes them from
+    (Nimg, H, W) and the step counter alone).  `mix` is [n_rows, 4] and the noise table holds n_rows rows of
+    [Nimg, H, W, 4]."""
+    if min(Nimg, H, W) < 1 or copies not in (1, 2):
+        raise ValueError(f"latent_mix: Nimg, H, W must be positive and copies 1 or 2, got {(Nimg, H, W, copies)}")
+    px = Nimg * H * W
+    want = {"latents": (latents, px * 4), "known": (known, px * 4), "mask": (mask, px), "step_counter": (step_counter, 1),
+            "lat_half_out": (lat_half_out, copies * px * 4)}
+    for name, (t, n) in want.items():
+        if t is not None and t.numel() != n:
+            raise ValueError(f"latent_mix: {name} has {t.numel()} elements, Nimg={Nimg}, H={H}, W={W} needs {n}")
+    if mix.dim() != 2 or mix.shape[1] != 4 or mix.shape[0] < 1:
+        raise ValueError(f"latent_mix: mix must be [n_rows, 4], got {tuple(mix.shape)}")
+    if noise.numel() != mix.shape[0] * px * 4:
+        raise ValueError(f"latent_mix: noise has {noise.numel()} elements, {mix.shape[0]} rows of {px * 4} needed")
+
+
+def latent_mix(latents, known, mask, noise, mix, *, alpha, step_counter, lat_half_out=None, copies=1, Nimg, H, W):
+    """ea_latent_mix: the alpha-mixing pipeline's per-step mix of the latents with the re-noised source, row
+    *step_counter - 1 of `mix` = [n_rows, 4] {k_init, k_noise, in_window, active} and of the noise table."""
+    check_mix_buffers(latents, known, mask, noise, mix, step_counter, lat_half_out, copies, Nimg, H, W)
+    lib = L.lib()
+    L.check(lib.ea_latent_mix(_p(latents), _p(known), _p(mask), _p(noise), _p(mix), float(alpha), _p(step_counter),
+                              int(mix.shape[0]), _p(lat_half_out), int(copies), Nimg, H, W, _stream()),
+            "ea_latent_mix")
+
+
 def step_gather(step_counter, n_rows, tables, dsts):
     """dsts[k][:] = tables[k][min(*step_counter, n_rows - 1)] for fp32 tables [rows, ...] (one launch)."""
     lib = L.lib()

@@ -34,6 +34,10 @@ text-to-image pipelines of all-region generation, sam2image.py and sketch2image.
 sampling loop (`_denoise`): no image, mask or blend, an optional spatial scale map, and in guess mode with guidance the
 residuals on the conditional rows only (utils/stable_diffusion_controlnet.py:579-602).
 
+`StableDiffusionControlNetInpaintMixingPipeline` is the alpha-mixing inpaint pipeline (:1706-2092) on the same loop:
+a spatial scale map, a re-noised start in the kept region and a per-step mix with freshly drawn noise, fused as one
+extra launch after the step's update.
+
 Not supported (raises NotImplementedError rather than silently diverging): the reference-only mode
 (`ref_image`, `utils/stable_diffusion_reference.py`).
 """
@@ -367,22 +371,30 @@ class _ControlNetPipelineBase:
         return isinstance(self.scheduler, DDIMScheduler) or unipc, unipc
 
     def _denoise(self, lat, timesteps, guidance_scale, do_cfg, callback=None, callback_steps=1, blend=None,
-                 unet_condition=None):
+                 unet_condition=None, mix=None):
         """The sampling loop of both pipelines (utils/...inpaint.py:1540-1656, utils/stable_diffusion_controlnet.py:
         566-627) on the engine `prepare`d for this request: returns the final latents [N, 4, h, w] on the engine's
         device.  lat: the initial latents [N, 4, h, w].  blend = (blend_steps, init, keep, noise): the inpaint
         pipeline's kept region, re-noised from `init` while i < blend_steps (keep = 1 keeps it).  unet_condition =
-        (mask, masked-image latents) of a 9-channel UNet."""
+        (mask, masked-image latents) of a 9-channel UNet.  mix = (alpha, alignment_ratio, init, keep, draw): the
+        alpha-mixing pipeline's mix after every step but the last (:2039-2051), with the noise `draw()` returns for
+        each such step, drawn in step order."""
         eng = self.engine
         N = lat.shape[0]
         lat = lat.to(eng.dev, torch.float32)
         blend_steps, init_d, m_d, noise_d = blend if blend is not None else (0, None, None, None)
         n_t = len(timesteps)
+        if mix is not None:
+            alpha, ratio, init_d, m_d, draw = mix
+            in_window = [i < n_t * ratio for i in range(n_t)]
         fused, unipc = self._fused_scheduler()
         if fused:
             acp = self.scheduler.alphas_cumprod
             coefs = [(float(acp[int(t)]), float(acp[int(t)])) for t in timesteps] if unipc else \
                 [self.scheduler.coefficients(t) for t in timesteps]
+            if mix is not None:
+                return self._denoise_mixing(lat, timesteps, guidance_scale, coefs, unipc, callback, callback_steps,
+                                            alpha, in_window, init_d, m_d, draw)
             # the kept region of step i is add_noise(init, noise, timesteps[i + 1]) while i < len * alignment_ratio
             # (:1647-1656).  With a callback the blend runs on the host side AFTER the callback, like the reference
             # (:1640-1656 calls back with the un-blended latents); otherwise it is fused into the step's last kernel.
@@ -420,7 +432,44 @@ class _ControlNetPipelineBase:
                 callback(i, t, lat)
             if i < blend_steps:
                 lat = self.scheduler.add_noise(init_d, noise_d, timesteps[i + 1]) * m_d + lat * (1 - m_d)
+            if mix is not None and i < n_t - 1:
+                p = self.scheduler.add_noise(init_d, draw(), timesteps[i + 1])
+                keep = p if in_window[i] else lat
+                lat = keep * m_d + ((1 - alpha) * lat + alpha * p) * (1 - m_d)
         return lat
+
+    def _denoise_mixing(self, lat, timesteps, guidance_scale, coefs, unipc, callback, callback_steps, alpha, in_window,
+                        init_d, m_d, draw):
+        """The fused loop of the alpha-mixing pipeline: every step's update, then ea_latent_mix with the noise of all
+        S - 1 mixes drawn up front (nothing else draws between them).  With a callback the step runs without the mix
+        and the mix runs on the host after the callback, drawing its noise there, as the reference calls back with
+        the un-mixed latents (:2035-2051)."""
+        eng = self.engine
+        n_t = len(timesteps)
+        acp = self.scheduler.alphas_cumprod
+        k_next = [(math.sqrt(float(acp[int(timesteps[i + 1])])), math.sqrt(1.0 - float(acp[int(timesteps[i + 1])])))
+                  if i < n_t - 1 else (1.0, 0.0) for i in range(n_t)]
+        host_mix = callback is not None
+        sched = dict(multistep=self.scheduler.coefficient_rows() if unipc else None,
+                     prediction_type=self.scheduler.config.prediction_type)
+        if host_mix:
+            sched["blend"] = ([1.0] * n_t, [0.0] * n_t, [0.0] * n_t)        # the update's own blend off
+        else:
+            sched["mix"] = ([k[0] for k in k_next], [k[1] for k in k_next], [float(w) for w in in_window],
+                            [1.0] * (n_t - 1) + [0.0])
+        eng.set_schedule([int(t) for t in timesteps], [c[0] for c in coefs], [c[1] for c in coefs], **sched)
+        table = None
+        if not host_mix:
+            table = torch.stack([draw() for _ in range(n_t - 1)]) if n_t > 1 else lat.new_zeros((0,) + lat.shape)
+        eng.begin(lat, guidance_scale, known_nchw=init_d, mask_n1hw=m_d,
+                  mix_alpha=None if host_mix else alpha, mix_noise=table)
+        for i, t in enumerate(timesteps):
+            eng.step()
+            if callback is not None and i % callback_steps == 0:
+                callback(i, t, eng.latents())
+            if host_mix and i < n_t - 1:
+                eng.mix_now(k_next[i][0], k_next[i][1], in_window[i], alpha, draw())
+        return eng.latents()
 
     def _output(self, lat, output_type, return_dict, dtype):
         """Latents -> the requested output: "latent", "pil" or numpy images (utils/...inpaint.py:1666-1703)."""
@@ -558,6 +607,18 @@ class StableDiffusionControlNetInpaintPipeline(_ControlNetPipelineBase):
             raise NotImplementedError("reference-only mode needs per-module hooks the fused UNet does not expose")
         if eta != 0.0:
             raise NotImplementedError("only deterministic sampling (eta = 0) is fused")
+        return self._inpaint(prompt, image, mask_image, controlnet_conditioning_image, height, width,
+                             num_inference_steps, guidance_scale, negative_prompt, num_images_per_prompt, generator,
+                             latents, prompt_embeds, negative_prompt_embeds, output_type, return_dict, callback,
+                             callback_steps, controlnet_conditioning_scale, alignment_ratio, guess_mode)
+
+    def _inpaint(self, prompt, image, mask_image, controlnet_conditioning_image, height, width, num_inference_steps,
+                 guidance_scale, negative_prompt, num_images_per_prompt, generator, latents, prompt_embeds,
+                 negative_prompt_embeds, output_type, return_dict, callback, callback_steps,
+                 controlnet_conditioning_scale, alignment_ratio, guess_mode, scale_map=None, alpha=None):
+        """The inpaint pipeline's call (:1131-1703) after its rejections; with `alpha` (a float) the alpha-mixing
+        pipeline's instead (:1706-2092): `scale_map` multiplies every net's scale, and a 4-channel UNet starts from
+        the re-noised source in the kept region and mixes after every step but the last, with no paste-back."""
         height, width = self._default_height_width(height, width, controlnet_conditioning_image)
         self.check_inputs(prompt, image, mask_image, controlnet_conditioning_image, height, width, callback_steps,
                           negative_prompt, prompt_embeds, negative_prompt_embeds, controlnet_conditioning_scale)
@@ -575,6 +636,8 @@ class StableDiffusionControlNetInpaintPipeline(_ControlNetPipelineBase):
             controlnet_conditioning_scale = [controlnet_conditioning_scale] * n_nets
         if not isinstance(controlnet_conditioning_image, list):
             controlnet_conditioning_image = [controlnet_conditioning_image]
+        if scale_map is not None:                                              # :1874-1880
+            controlnet_conditioning_scale = [s * scale_map for s in controlnet_conditioning_scale]
 
         prompt_embeds = self._encode_prompt(prompt, num_images_per_prompt, do_cfg, negative_prompt, prompt_embeds,
                                             negative_prompt_embeds)
@@ -616,6 +679,19 @@ class StableDiffusionControlNetInpaintPipeline(_ControlNetPipelineBase):
         eng.prepare(prompt_embeds, conds, controlnet_conditioning_scale, guess_mode=guess_mode, cfg_duplicated=do_cfg,
                     guided=do_cfg)
         n_t = len(timesteps)
+        if alpha is not None and not inpaint_unet:
+            # :1965-1977 and :2039-2051: every draw is randn_like(init) on the execution device's default generator,
+            # one for the starting latents, then one per mix in step order
+            init_dev = init_lat.to(dev)
+
+            def draw():
+                return torch.randn_like(init_dev).to(torch.float32)
+            init_d, m_d = init_dev.to(torch.float32), m.to(dev, torch.float32)
+            lat = lat.to(dev, torch.float32)
+            lat = m_d * self.scheduler.add_noise(init_d, draw(), timesteps[0]) + (1 - m_d) * lat
+            lat = self._denoise(lat, timesteps, guidance_scale, do_cfg, callback, callback_steps,
+                                mix=(alpha, alignment_ratio, init_d, m_d, draw))
+            return self._output(lat, output_type, return_dict, edt)
         blend_steps = 0 if alignment_ratio is None else sum(1 for i in range(n_t) if i < n_t * alignment_ratio)
         if blend_steps and blend_steps >= n_t:
             # the reference indexes timesteps[i + 1] (:1652): alignment_ratio = 1.0 raises there too
@@ -632,6 +708,40 @@ class StableDiffusionControlNetInpaintPipeline(_ControlNetPipelineBase):
             if alignment_ratio is None or alignment_ratio == 1.0:
                 lat = init_d * m_d + lat * (1 - m_d)                                   # :1658-1664
         return self._output(lat, output_type, return_dict, edt)
+
+
+class StableDiffusionControlNetInpaintMixingPipeline(StableDiffusionControlNetInpaintPipeline):
+    """utils/stable_diffusion_controlnet_inpaint.py:1706-2092, the inpaint pipeline behind the demos' "alpha_weight"
+    slider and `use_scale_map` (editany_lora.py:841-856, :902-918).  Against the inpaint pipeline:
+
+    - `controlnet_conditioning_scale_map` ([H, W], [1, H, W] or [1, 1, H, W]) multiplies every net's scale and is
+      resized bilinearly to every residual (:1874-1880); there is no guess mode and no reference-only mode.
+    - A 4-channel UNet starts from m * add_noise(init, randn, t_0) + (1 - m) * latents, m = 1 where the source is
+      kept (:1965-1977), and after every step but the last mixes with p = add_noise(init, randn, t_{i+1}):
+      x = p m + ((1 - a) x + a p)(1 - m) while i < S * alignment_ratio, x m + ((1 - a) x + a p)(1 - m) after
+      (:2039-2051), a = alpha_weight.  The mix is one extra launch of the fused step (ea_latent_mix).  Nothing is
+      pasted back after the loop.
+    - Every randn is randn_like(init) on the execution device's default generator, not `generator`: one for the
+      start, then one per mix in step order, all drawn before the loop (DDIM with eta = 0 and UniPC draw nothing).
+      A callback sees the un-mixed latents; the mix and its draw then follow it on the host.  Any other scheduler
+      runs network, `step` and mix on the host, drawing at each step.
+    - A 9-channel UNet runs as in the inpaint pipeline: no start blend and no mix, so alpha_weight has no effect
+      (:1933-1953, :1996-1999)."""
+
+    @torch.no_grad()
+    def __call__(self, prompt=None, image=None, mask_image=None, controlnet_conditioning_image=None, height=None,
+                 width=None, num_inference_steps=50, guidance_scale=7.5, negative_prompt=None,
+                 num_images_per_prompt=1, eta=0.0, generator=None, latents=None, prompt_embeds=None,
+                 negative_prompt_embeds=None, output_type="pil", return_dict=True, callback=None, callback_steps=1,
+                 cross_attention_kwargs=None, controlnet_conditioning_scale=1.0, controlnet_conditioning_scale_map=None,
+                 alignment_ratio=0.95, alpha_weight=0.5):
+        if eta != 0.0:
+            raise NotImplementedError("only deterministic sampling (eta = 0) is fused")
+        return self._inpaint(prompt, image, mask_image, controlnet_conditioning_image, height, width,
+                             num_inference_steps, guidance_scale, negative_prompt, num_images_per_prompt, generator,
+                             latents, prompt_embeds, negative_prompt_embeds, output_type, return_dict, callback,
+                             callback_steps, controlnet_conditioning_scale, alignment_ratio, False,
+                             scale_map=controlnet_conditioning_scale_map, alpha=float(alpha_weight))
 
 
 class StableDiffusionControlNetPipeline(_ControlNetPipelineBase):

@@ -287,6 +287,22 @@ int ea_out_vpred(const void* xn, const float* w, const float* bias, float* laten
                  const float* coef, const float* known, const float* noise, const float* mask,
                  void* lat_half_out, int* step_counter, float* hist, int Nimg, int H, int W, int C, void* stream);
 
+/* ---- ea_latent_mix: alpha-mixing of the latents with the re-noised source -------------------------
+ * The per-step mix of the alpha-mixing inpaint pipeline (utils/stable_diffusion_controlnet_inpaint.py:2039-2051),
+ * launched after ea_out_* (run with its own blend off) in the same step.  Row r = *step_counter - 1 of the tables is
+ * the step that epilogue just finished (it advanced the counter); with r outside [0, n_rows) nothing is touched.
+ * latents fp32 NHWC [Nimg, H, W, 4], updated in place; known fp32 [Nimg, H, W, 4] (the source image latents);
+ * mask fp32 [Nimg, H, W] (1 = keep the source); noise fp32 [n_rows][Nimg, H, W, 4] (row r read only when row r
+ * of mix is active); mix fp32 [n_rows][4] = {k_init, k_noise, in_window, active}.  For an active row:
+ *   p = k_init * known + k_noise * noise[r]          (add_noise(init, noise, t_{r+1}))
+ *   x = m * (in_window != 0 ? p : x) + (1 - m) * ((1 - alpha) x + alpha p)
+ * lat_half_out (optional): half [copies * Nimg, H, W, 4], the updated latents written `copies` (1 or 2) times, the
+ * next step's network input.  latents / known / noise 16-byte aligned and lat_half_out 8-byte aligned, else
+ * EA_ERR_SHAPE; a NULL operand or copies not 1 or 2 is EA_ERR_ARG; both before any launch. */
+int ea_latent_mix(float* latents, const float* known, const float* mask, const float* noise, const float* mix,
+                  float alpha, const int* step_counter, int n_rows, void* lat_half_out, int copies, int Nimg,
+                  int H, int W, void* stream);
+
 /* ---- ea_step_gather: first kernel of a captured denoising step ---------------------------------
  * The loop of utils/stable_diffusion_controlnet_inpaint.py:1540-1656 changes only scalars from step to step
  * (scheduler coefficients, the timestep behind every ResBlock's emb_layers projection, openaimodel.py:204-210).
