@@ -29,7 +29,7 @@ class GemmArgs(C.Structure):
         ("out2", C.c_void_p), ("ldo2", C.c_longlong),
         ("out_f32", C.c_void_p),
         ("act", C.c_int), ("out_scale", C.c_float), ("accumulate", C.c_int),
-        ("force_bn", C.c_int), ("force_splits", C.c_int), ("force_2cta", C.c_int), ("no_spin", C.c_int),
+        ("force_bn", C.c_int), ("force_splits", C.c_int), ("force_2cta", C.c_int),
         ("force_persistent", C.c_int),
         ("rowstats_out", C.c_void_p), ("ln_stats", C.c_void_p), ("ln_g", C.c_void_p), ("ln_parts", C.c_int),
         ("ln_eps", C.c_float), ("row_scale", C.c_void_p),
@@ -56,7 +56,7 @@ class GnArgs(C.Structure):
         ("gamma", C.c_void_p), ("beta", C.c_void_p),
         ("out", C.c_void_p), ("ldo", C.c_longlong),
         ("B", C.c_int), ("HW", C.c_int), ("C", C.c_int), ("groups", C.c_int),
-        ("eps", C.c_float), ("silu", C.c_int), ("two_pass", C.c_int),
+        ("eps", C.c_float), ("silu", C.c_int),
         ("workspace", C.c_void_p),
         ("n_nets", C.c_int), ("gamma_more", C.c_void_p * 2), ("beta_more", C.c_void_p * 2),
     ]

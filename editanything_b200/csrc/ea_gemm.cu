@@ -92,7 +92,6 @@ struct GemmKParams {
   // split-K: blockIdx.z = split index; partial tiles go through `ws`, arrival counters in `cnt`
   int splits;
   int kb_per_split;
-  int no_spin;       // split-K without the sibling wait (concurrent streams)
   float* ws;   // [items][splits][RP * 128][BN] fp32
   int* cnt;    // [items][2]: arrived, done (zero between launches)
   // LayerNorm fold (see ea_gemm_args): producer side / consumer side
@@ -943,30 +942,21 @@ ea_gemm_kernel(const __grid_constant__ GemmLaunch<NG> L, const int tiles_per_gro
       __threadfence();
       epi_bar_sync();
       int* cnt = p.cnt + 2 * tile_id;
-      bool take_all = false;   // no_spin: the LAST split CTA to arrive finishes the whole tile
-      volatile int* flag = reinterpret_cast<volatile int*>(cb + (it & 1) * RP * 512);   // one slot for the CTA
-      if (p.no_spin) {
-        if (et == 0) *flag = atomicAdd(cnt, 1);
-        epi_bar_sync();
-        take_all = *flag == p.splits - 1;
-        epi_bar_sync();
-      } else {
-        if (et == 0) {
-          atomicAdd(cnt, 1);
-          uint32_t spins = 0;
-          while (ld_acquire_gpu(cnt) < p.splits) {
-            __nanosleep(40);
-            if (++spins > (1u << 24)) { asm volatile("trap;"); }
-          }
+      if (et == 0) {
+        atomicAdd(cnt, 1);
+        uint32_t spins = 0;
+        while (ld_acquire_gpu(cnt) < p.splits) {
+          __nanosleep(40);
+          if (++spins > (1u << 24)) { asm volatile("trap;"); }
         }
-        epi_bar_sync();
       }
+      epi_bar_sync();
       __threadfence();
-      if (!p.no_spin || take_all) {
+      {
         const int chunks = geglu ? (half_bn >> 5) : (BN >> 5);
         const int units = RB * chunks;
-        const int u0 = take_all ? 0 : (int)(((long long)units * zsplit) / p.splits);
-        const int u1 = take_all ? units : (int)(((long long)units * (zsplit + 1)) / p.splits);
+        const int u0 = (int)(((long long)units * zsplit) / p.splits);
+        const int u1 = (int)(((long long)units * (zsplit + 1)) / p.splits);
         // Stage 1 (all consumer threads, float4 granularity, loads of the sibling partials unrolled for
         // memory-level parallelism) sums this CTA's share into the (published, now dead) accumulator staging;
         // stage 2 runs the fused epilogue on whole 32-column units, one per thread.
@@ -1032,17 +1022,13 @@ ea_gemm_kernel(const __grid_constant__ GemmLaunch<NG> L, const int tiles_per_gro
         }
         epi_bar_sync();
         if (et == 0) {
-          if (take_all) {
+          int old = atomicAdd(cnt + 1, 1);
+          if (old == p.splits - 1) {  // last finisher: re-arm the counters for the next launch
             cnt[0] = 0;
-          } else {
-            int old = atomicAdd(cnt + 1, 1);
-            if (old == p.splits - 1) {  // last finisher: re-arm the counters for the next launch
-              cnt[0] = 0;
-              cnt[1] = 0;
-            }
+            cnt[1] = 0;
           }
         }
-      }  // !no_spin || take_all
+      }
     }
     // the staged accumulator has been read: hand the ring back to the producer (its next loads are async-proxy
     // writes over what this thread wrote and read through the generic proxy)
@@ -1291,7 +1277,7 @@ static bool gemm_same_problem(const ea_gemm_args* a, const ea_gemm_args* b) {
          (!a->rowvec) == (!b->rowvec) && a->rows_per_batch == b->rows_per_batch &&
          (!a->rowstats_out) == (!b->rowstats_out) && (!a->ln_stats) == (!b->ln_stats) && a->ln_parts == b->ln_parts &&
          a->force_bn == b->force_bn && a->force_splits == b->force_splits && a->force_2cta == b->force_2cta &&
-         a->no_spin == b->no_spin && a->force_persistent == b->force_persistent;
+         a->force_persistent == b->force_persistent;
 }
 
 template <typename K>
@@ -1383,7 +1369,7 @@ extern "C" int ea_gemm_grouped(const ea_gemm_args* args, int n_groups, void* str
     return EA_ERR_SHAPE;
   // the spinning split-K fix-up makes split CTAs wait for their siblings: every CTA of the grid must be resident at
   // once (one per SM; the planner guarantees it, forced test configurations are checked here instead of deadlocking)
-  if (plan.splits > 1 && !a->no_spin && tiles * G * plan.splits > (long long)sm_count()) return EA_ERR_SHAPE;
+  if (plan.splits > 1 && tiles * G * plan.splits > (long long)sm_count()) return EA_ERR_SHAPE;
 
   int stages = plan.stages;
   if (stages > 8) stages = 8;
@@ -1397,7 +1383,6 @@ extern "C" int ea_gemm_grouped(const ea_gemm_args* args, int n_groups, void* str
     p.stages = stages;
     p.splits = plan.splits;
     p.kb_per_split = plan.kbps;
-    p.no_spin = a->no_spin;
     if (p.splits > 1) {   // every group has its own counters and partial tiles in the (shared) workspace
       p.cnt = reinterpret_cast<int*>(a->workspace) + 2 * g * tiles;
       p.ws = reinterpret_cast<float*>(reinterpret_cast<char*>(a->workspace) + 65536) +

@@ -34,7 +34,7 @@ gn_fused_kernel(const ea_half* __restrict__ x, long long ldx, int C1,
                 const ea_half* __restrict__ x2, long long ldx2,
                 const GnAffine aff,
                 ea_half* __restrict__ out, long long ldo, int HW, int C, int groups, float eps,
-                int silu, int chunks, int ppc, int cached, int part_bytes, int phase,
+                int silu, int chunks, int ppc, int cached, int part_bytes,
                 float* __restrict__ ws) {
   pdl_launch_dependents();
   const int net = aff.ipg > 0 ? (int)blockIdx.y / aff.ipg : 0;
@@ -71,9 +71,6 @@ gn_fused_kernel(const ea_half* __restrict__ x, long long ldx, int C1,
   // floating-point atomics, so the statistics (and everything downstream) are bit-reproducible run to run
   int* cnt = reinterpret_cast<int*>(ws) + 2 * b;
   float* pws_b = ws + 2 * gridDim.y + (size_t)b * chunks * (2 * groups);
-  // phase 0: fused (pass 1, image-wide spin barrier, pass 2).  phases 1 / 2: the two passes as
-  // SEPARATE launches without any inter-CTA wait - used when several streams run concurrently and
-  // a spinning, partially resident grid could starve another one (no co-residency guarantee then).
   for (int i = threadIdx.x; i < groups * 2; i += blockDim.x) sh[i] = 0.f;
   __syncthreads();
   const ea_half* src;
@@ -98,7 +95,6 @@ gn_fused_kernel(const ea_half* __restrict__ x, long long ldx, int C1,
       shift[j] = kv;
     }
   }
-  if (phase != 2) {
   // ---- pass 1: load (cache) + per-thread, per-channel partial sums (the thread's 8 channels
   //      are fixed, so their groups are too: shared-memory atomics only once, after the loop)
   float cs[8], cq[8];
@@ -167,7 +163,6 @@ gn_fused_kernel(const ea_half* __restrict__ x, long long ldx, int C1,
   for (int i = threadIdx.x; i < groups * 2; i += blockDim.x) __stcg(&pws_b[(size_t)blockIdx.x * (2 * groups) + i], sh[i]);
   __threadfence();
   __syncthreads();
-  if (phase == 1) return;
   // ---- image-wide barrier
   if (threadIdx.x == 0) {
     atomicAdd(cnt, 1);
@@ -179,7 +174,6 @@ gn_fused_kernel(const ea_half* __restrict__ x, long long ldx, int C1,
   }
   __syncthreads();
   __threadfence();
-  }  // phase != 2
   // ---- pass 2: y = x * a + b with a = rstd*gamma, b = beta - mean*a (per channel of this thread)
   // the image's 2*groups statistics come back in ONE L2 round trip (per-thread dependent loads of
   // "its" groups cost several serialized round trips)
@@ -245,7 +239,7 @@ gn_fused_kernel(const ea_half* __restrict__ x, long long ldx, int C1,
   }
   // ---- leave the counters zero for the next launch (the partial slots are simply overwritten)
   __syncthreads();
-  if (phase == 0 && threadIdx.x == 0) {
+  if (threadIdx.x == 0) {
     int old = atomicAdd(cnt + 1, 1);
     if (old == chunks - 1) {
       cnt[0] = 0;
@@ -976,19 +970,9 @@ extern "C" int ea_groupnorm(const ea_gn_args* a, void* stream) {
     aff.ipg = a->B / a->n_nets;
   }
   dim3 grid(chunks, a->B);
-  if (a->two_pass) {
-    const int smem1 = 512 + part_bytes;
-    for (int phase = 1; phase <= 2; ++phase)
-      ea_launch(gn_fused_kernel, grid, dim3(threads), (size_t)smem1, st,
-                reinterpret_cast<const ea_half*>(a->x), a->ldx, C1, reinterpret_cast<const ea_half*>(a->x2),
-                a->ldx2, aff, reinterpret_cast<ea_half*>(a->out), a->ldo, a->HW, a->C,
-                a->groups, a->eps, a->silu, chunks, ppc, 0, part_bytes, phase, a->workspace);
-    ea_count_launch();
-    return EA_LAUNCH_OK();
-  }
   ea_launch(gn_fused_kernel, dim3(grid), dim3(threads), (size_t)(smem), st, reinterpret_cast<const ea_half*>(a->x), a->ldx, C1, reinterpret_cast<const ea_half*>(a->x2),
       a->ldx2, aff, reinterpret_cast<ea_half*>(a->out), a->ldo, a->HW, a->C,
-      a->groups, a->eps, a->silu, chunks, ppc, cached, part_bytes, 0, a->workspace);
+      a->groups, a->eps, a->silu, chunks, ppc, cached, part_bytes, a->workspace);
   return EA_LAUNCH_OK();
 }
 

@@ -145,12 +145,10 @@ class DenoiseEngine:
             self._graph = None        # the step's last launch differs (ea_out_cfg_ddim / ea_out_ddim)
         self.guided = bool(guided)
         self.B = ctx.shape[0]
-        nets = [self.unet] + self.cns
-        # lockstep (nets.UNetRunner): the encoder-side K/V of all networks live stacked in ctx_ls; only the UNet
-        # (whose decoder runs alone) keeps its own per-layer cache
-        ls = self.runner.lockstep
-        self._keep("ctx_cache", [n.precompute_context(ctx) for n in (nets[:1] if ls else nets)])
-        self._keep("ctx_ls", self.runner.precompute_context_lockstep(ctx) if ls else None)
+        # the encoder-side K/V of every group of networks (nets.UNetRunner.groups) live stacked in ctx_groups; the UNet
+        # (whose decoder runs alone) also keeps its own per-layer cache
+        self._keep("ctx_cache", [self.unet.precompute_context(ctx)])
+        self._keep("ctx_groups", self.runner.precompute_context_groups(ctx))
         # cfg_duplicated: the conditioning images are [x; x] (prepare_controlnet_conditioning_image doubles them for
         # classifier-free guidance, utils/...inpaint.py:380-381) - run the hint stack on one half only; conditional
         # rows: the N images arrive once and are stacked the same way
@@ -297,8 +295,8 @@ class DenoiseEngine:
             x_nchw = x_nchw[:, :4]
         xh = x_nchw.to(self.dev).permute(0, 2, 3, 1).contiguous().to(self.hdt)
         self._fill_emb(t)
-        xn = self.runner.eps_features(xh, self.t_dev, self.ctx_cache, self.hints, self.scales, self.gn_ws,
-                                      embs=self.emb_bufs, ctx_ls=self.ctx_ls, cond_in=cond)
+        xn = self.runner.eps_features(xh, self.t_dev, self.ctx_cache, self.ctx_groups, self.hints, self.scales,
+                                      self.gn_ws, embs=self.emb_bufs, cond_in=cond)
         eps = torch.empty(B, H, W_, 4, device=self.dev, dtype=torch.float32)
         w, cb, mc = self.unet.w["out.w"], self.unet.w["out.cb"], self.cfg.model_channels
         if self.guided and B % 2 == 0:    # the two guidance halves, as the guided step reduces them
@@ -312,8 +310,8 @@ class DenoiseEngine:
         H, W_ = self.lat.shape[1], self.lat.shape[2]
         self.ops.step_gather(self.step_ctr, self._sched_cap, [self.coef_tab] + self.emb_tabs,
                              [self.coef_dev] + self.emb_bufs)
-        xn = self.runner.eps_features(self.x_half, self.t_dev, self.ctx_cache, self.hints, self.scales, self.gn_ws,
-                                      embs=self.emb_bufs, ctx_ls=self.ctx_ls, cond_in=self._step_cond())
+        xn = self.runner.eps_features(self.x_half, self.t_dev, self.ctx_cache, self.ctx_groups, self.hints,
+                                      self.scales, self.gn_ws, embs=self.emb_bufs, cond_in=self._step_cond())
         mixing = self.mix_tab is not None
         # the alpha mix replaces the update's blend: the epilogue then reads no known / noise / mask
         kw = dict(latents=self.lat, coef=self.coef_dev, known=None if mixing else self.known,
@@ -447,8 +445,7 @@ class DenoiseEngine:
             # prefetch hint (ops.WeightLookahead).  Not measured on H100.
             dist = int(os.environ.get("EA_WEIGHT_PREFETCH", "0"))
             mk = getattr(self.ops, "WeightLookahead", None)
-            single = self.runner.lockstep or not self.runner.cns     # launch order = execution order
-            la = mk(dist, int(os.environ.get("EA_WEIGHT_PREFETCH_MAXM", "512"))) if (mk is not None and dist > 0 and single) else None
+            la = mk(dist, int(os.environ.get("EA_WEIGHT_PREFETCH_MAXM", "512"))) if (mk is not None and dist > 0) else None
             with torch.cuda.stream(s):
                 if la is not None:
                     with self.ops.weight_lookahead(la):

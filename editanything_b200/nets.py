@@ -46,9 +46,6 @@ class PackedNet:
     def __init__(self, cfg: UNetConfig, kind: str, state_dict, device, backend=None):
         self.cfg, self.kind = cfg, kind
         self.ops = backend or default_ops()
-        # LayerNorm folded into the GEMMs around it (ea_gemm_args.rowstats_out / ln_*): no LayerNorm launch, no
-        # normalised tensor.  EA_LN_FOLD=0 keeps the separate ea_layernorm launches (A/B, debugging).
-        self.ln_fold = os.environ.get("EA_LN_FOLD", "1") != "0"
         self.dev = device
         self.hdt = self.ops.half_dtype()
         self.topo = build_topology(cfg, with_decoder=(kind == "unet"))
@@ -156,24 +153,20 @@ class PackedNet:
         q2 = sd[f"{tb}.attn2.to_q.weight"]
         idx = _geglu_interleave(inner * 4)
         ff1, ff1b = sd[f"{tb}.ff.net.0.proj.weight"][idx], sd[f"{tb}.ff.net.0.proj.bias"][idx]
-        if self.ln_fold:
-            # LN(x) W^T + b = rstd * (x (W*gamma)^T - mean * g) + (W beta + b)   (attention.py:263-275)
-            for name, wt, bt, nrm in (("qkv1", qkv1, None, "norm1"), ("q2", q2, None, "norm2"), ("ff1", ff1, ff1b, "norm3")):
-                gam, bet = sd[f"{tb}.{nrm}.weight"].double(), sd[f"{tb}.{nrm}.bias"].double()
-                wg = H((wt.double() * gam[None, :]).float())
-                self.w[f"{p}.{name}.w"] = wg
-                self.w[f"{p}.{name}.g"] = F(wg.double().sum(1).float())     # of the ROUNDED weights: exact cancellation
-                c = wt.double() @ bet
-                self.w[f"{p}.{name}.b"] = F((c + bt.double() if bt is not None else c).float())
-        else:
-            self.w[p + ".qkv1.w"], self.w[p + ".q2.w"] = H(qkv1), H(q2)
-            self.w[p + ".ff1.w"], self.w[p + ".ff1.b"] = H(ff1), F(ff1b)
+        # LayerNorm folded into the GEMMs that consume its output (ea_gemm_args.rowstats_out / ln_*): no LayerNorm
+        # launch, no normalised tensor.  LN(x) W^T + b = rstd * (x (W*gamma)^T - mean * g) + (W beta + b)
+        # (attention.py:263-275)
+        for name, wt, bt, nrm in (("qkv1", qkv1, None, "norm1"), ("q2", q2, None, "norm2"), ("ff1", ff1, ff1b, "norm3")):
+            gam, bet = sd[f"{tb}.{nrm}.weight"].double(), sd[f"{tb}.{nrm}.bias"].double()
+            wg = H((wt.double() * gam[None, :]).float())
+            self.w[f"{p}.{name}.w"] = wg
+            self.w[f"{p}.{name}.g"] = F(wg.double().sum(1).float())     # of the ROUNDED weights: exact cancellation
+            c = wt.double() @ bet
+            self.w[f"{p}.{name}.b"] = F((c + bt.double() if bt is not None else c).float())
         self.w[p + ".o1.w"], self.w[p + ".o1.b"] = H(sd[f"{tb}.attn1.to_out.0.weight"]), F(sd[f"{tb}.attn1.to_out.0.bias"])
         self.w[p + ".kv2.w"] = H(torch.cat([sd[f"{tb}.attn2.to_k.weight"], sd[f"{tb}.attn2.to_v.weight"]], 0))
         self.w[p + ".o2.w"], self.w[p + ".o2.b"] = H(sd[f"{tb}.attn2.to_out.0.weight"]), F(sd[f"{tb}.attn2.to_out.0.bias"])
         self.w[p + ".ff2.w"], self.w[p + ".ff2.b"] = H(sd[f"{tb}.ff.net.2.weight"]), F(sd[f"{tb}.ff.net.2.bias"])
-        for n in ("norm1", "norm2", "norm3"):
-            self.w[f"{p}.{n}.g"], self.w[f"{p}.{n}.b"] = F(sd[f"{tb}.{n}.weight"]), F(sd[f"{tb}.{n}.bias"])
 
     def weight_bytes(self):
         return sum(t.numel() * t.element_size() for t in self.w.values())
@@ -265,18 +258,22 @@ class PackedNet:
         return torch.empty(*shape, device=self.dev, dtype=self.hdt)
 
 
+# networks one grouped launch can run: the group limit of ea_gemm_grouped and ea_gn_args.n_nets
+MAX_GROUP = 3
+
+
 class BlockRunner:
-    """Executes ResBlocks / SpatialTransformers / resampling convolutions for ONE network or for n networks of
-    the same topology in lockstep (the UNet encoder and the ControlNets: cldm/cldm.py:22-45 vs 284-305 - the same
-    layers, different weights, the same latent).  In lockstep the activations are stacked along the batch dimension
-    ([n*B, H, W, C], network g = images [g*B, (g+1)*B)), every GEMM is ONE grouped launch (ea_gemm_grouped: group
-    g = network g's weights on its slice), GroupNorm takes one (gamma, beta) per network, attention simply sees
+    """Executes ResBlocks / SpatialTransformers / resampling convolutions for ONE network or for n <= MAX_GROUP
+    networks of the same topology in lockstep (the UNet encoder and the ControlNets: cldm/cldm.py:22-45 vs 284-305 -
+    the same layers, different weights, the same latent).  In lockstep the activations are stacked along the batch
+    dimension ([n*B, H, W, C], network g = images [g*B, (g+1)*B)), every GEMM is ONE grouped launch (ea_gemm_grouped:
+    group g = network g's weights on its slice), GroupNorm takes one (gamma, beta) per network, attention simply sees
     n*B batch entries.  `out2` (the UNet's skip-concat dual store) applies to network 0 only."""
 
     def __init__(self, nets):
         self.nets, self.n = list(nets), len(nets)
         n0 = self.nets[0]
-        self.cfg, self.dev, self.hdt, self.ln_fold = n0.cfg, n0.dev, n0.hdt, n0.ln_fold
+        self.cfg, self.dev, self.hdt = n0.cfg, n0.dev, n0.hdt
         self.emb_off = n0.emb_off
 
     @property
@@ -371,28 +368,22 @@ class BlockRunner:
         N, M = H * W_, B * H * W_
         xn = self._new(B, H, W_, c)
         self.groupnorm(x, p + ".norm", xn, B=B, HW=N, C_=c, eps=1e-6, silu=False, workspace=gn_ws, ldx=x.stride(2))
-        fold = self.ln_fold
 
         def stats():   # per-row partial (sum, M2 about the chunk mean) per 32-column chunk, written by the producing GEMM
-            return torch.empty(n, inner // 32, M // n, 2, device=self.dev, dtype=torch.float32) if fold else None
+            return torch.empty(n, inner // 32, M // n, 2, device=self.dev, dtype=torch.float32)
 
-        def normed(t, st, name, nrm, **kw):   # GEMM on LayerNorm(t): folded, or LayerNorm launch + plain GEMM
-            if fold:
-                return self.gemm(t, f"{p}.{name}.w", bias=f"{p}.{name}.b", ln=(st, f"{p}.{name}.g", 1e-5), **kw)
-            w = self.nets[0].w                 # (lockstep needs the fold: UNetRunner checks)
-            nn_ = self._new(M, inner)
-            o.layernorm(t, w[f"{p}.{nrm}.g"], w[f"{p}.{nrm}.b"], nn_, M=M, C_=inner)
-            return self.gemm(nn_, f"{p}.{name}.w", bias=f"{p}.{name}.b" if f"{p}.{name}.b" in w else None, **kw)
+        def normed(t, st, name, **kw):        # GEMM on LayerNorm(t), the LayerNorm folded into it
+            return self.gemm(t, f"{p}.{name}.w", bias=f"{p}.{name}.b", ln=(st, f"{p}.{name}.g", 1e-5), **kw)
 
         st0, st1, st2 = stats(), stats(), stats()
         t0 = self.gemm(xn.view(M, c), p + ".proj_in.w", bias=p + ".proj_in.b", rowstats_out=st0)
-        qkv = normed(t0, st0, "qkv1", "norm1")                  # [M, 3*inner]
+        qkv = normed(t0, st0, "qkv1")                          # [M, 3*inner]
         ao = self._new(M, inner)
         o.attention(qkv, qkv[:, inner:], qkv[:, 2 * inner:], ao, B=B, heads=heads, Nq=N, Nkv=N, d=dh,
                     q_strides=(N * 3 * inner, 3 * inner), k_strides=(N * 3 * inner, 3 * inner),
                     v_strides=(N * 3 * inner, 3 * inner), o_strides=(N * inner, inner), scale=dh ** -0.5)
         t1 = self.gemm(ao, p + ".o1.w", bias=p + ".o1.b", residual=t0, rowstats_out=st1)
-        q2 = normed(t1, st1, "q2", "norm2")
+        q2 = normed(t1, st1, "q2")
         kv = ctxc["kv"][p]                                       # [B*L, 2*inner] (stacked like x in lockstep)
         Lc = ctxc["L"]
         ao2 = self._new(M, inner)
@@ -400,7 +391,7 @@ class BlockRunner:
                     q_strides=(N * inner, inner), k_strides=(Lc * 2 * inner, 2 * inner),
                     v_strides=(Lc * 2 * inner, 2 * inner), o_strides=(N * inner, inner), scale=dh ** -0.5)
         t2 = self.gemm(ao2, p + ".o2.w", bias=p + ".o2.b", residual=t1, rowstats_out=st2)
-        g = normed(t2, st2, "ff1", "norm3", act=L.EA_ACT_GEGLU)   # [M, 4*inner]
+        g = normed(t2, st2, "ff1", act=L.EA_ACT_GEGLU)         # [M, 4*inner]
         t3 = self.gemm(g, p + ".ff2.w", bias=p + ".ff2.b", residual=t2)
         if out is None:
             out = self._new(B, H, W_, c)
@@ -445,34 +436,31 @@ class UNetRunner:
         self.unet, self.cns, self.dev = unet, list(controlnets), device
         self.ops = unet.ops
         self.hdt = unet.hdt
-        self.concurrent = os.environ.get("EA_CONCURRENT", "1") != "0"
-        self._streams = []
         self._gn_ws = {}
-        # Lockstep: the UNet encoder and the ControlNets as ONE sequence of grouped launches (BlockRunner) instead of
-        # one stream per network.  Needs identical topologies (conv_in, run per network, may differ in its input
-        # channels), the LayerNorm fold and at most 3 networks (ea_gemm_grouped); EA_LOCKSTEP=0 falls back to the
-        # concurrent streams (A/B).
+        # The UNet encoder and the ControlNets run as grouped launches: [unet] + cns split into consecutive groups of
+        # at most MAX_GROUP networks, each group ONE sequence of launches on stacked activations (BlockRunner), one
+        # group after another on the current stream.  Grouping needs identical topologies (conv_in, run per network,
+        # may differ in its input channels).
         nets = [unet] + self.cns
         same = replace(unet.cfg, in_channels=0)
-        self.lockstep = (os.environ.get("EA_LOCKSTEP", "1") != "0" and 2 <= len(nets) <= 3 and unet.ln_fold
-                         and all(replace(n.cfg, in_channels=0) == same and n.ln_fold for n in nets))
-        self.solo = [BlockRunner([n]) for n in nets]      # the UNet, then each ControlNet, on its own
-        self.group = BlockRunner(nets) if self.lockstep else None
+        for i, n in enumerate(self.cns):
+            if replace(n.cfg, in_channels=0) != same:
+                raise ValueError(f"ControlNet {i} does not have the UNet's topology: {n.cfg} vs {unet.cfg}")
+        self.groups = [BlockRunner(nets[i:i + MAX_GROUP]) for i in range(0, len(nets), MAX_GROUP)]
+        self.decoder = BlockRunner([unet])
 
-    def _workspaces(self, B, n):
-        """n zeroed GroupNorm workspaces for batch B (one per concurrent stream), allocated once."""
-        key = (B, n)
-        if key not in self._gn_ws:
-            self._gn_ws[key] = [self.ops.gn_workspace(B, self.dev) for _ in range(n)]
-        return self._gn_ws[key]
+    def _gn_workspace(self, B):
+        """A zeroed GroupNorm workspace for a stacked batch of B images, allocated once."""
+        if B not in self._gn_ws:
+            self._gn_ws[B] = self.ops.gn_workspace(B, self.dev)
+        return self._gn_ws[B]
 
-    def _encoder(self, R: BlockRunner, x_half, embs, ctxc, gn_ws, sinks, hints, scales, cond_in=None, deferred=None):
+    def _encoder(self, R: BlockRunner, x_half, embs, ctxc, gn_ws, sinks, hints, scales, cond_in=None):
         """input_blocks + middle of the networks of R (the UNet, if there, first), stacked along the batch.  embs,
         hints, scales: one per network of R (hint and scale None for the UNet).  The UNet's skips are dual-stored into
         the decoder's concat slots; each ControlNet's zero-conv then accumulates `scale * zero_conv(h)` into the same
-        slot instead of materialising the residual (cldm/cldm.py:34-41,293-303), at once or, given `deferred`, later
-        by the caller.  cond_in: a 9-channel UNet's conv_in contribution of the condition channels, bias included
-        (PackedNet.precompute_condition)."""
+        slot instead of materialising the residual (cldm/cldm.py:34-41,293-303).  cond_in: a 9-channel UNet's conv_in
+        contribution of the condition channels, bias included (PackedNet.precompute_condition)."""
         n, nets = R.n, R.nets
         has_unet = nets[0].kind == "unet"
         topo = nets[0].topo
@@ -491,21 +479,20 @@ class UNetRunner:
                                   add=cond_in if un else hints[g])
             else:
                 h = R._run_layers(layers, h, embs, ctxc, gn_ws, final_out2=slot if has_unet else None)
-            self._zero_convs(R, h, i, slot, scales, deferred)
+            self._zero_convs(R, h, i, slot, scales)
         # the UNet on its own writes the middle output straight into the decoder's first concat; stacked with
         # ControlNets, its slice of the stacked output is dual-stored there
         mid = sinks["mid"]
         h = R._run_layers(topo.middle, h, embs, ctxc, gn_ws, final_out=mid if has_unet and n == 1 else None,
                           final_out2=mid if has_unet and n > 1 else None)
-        self._zero_convs(R, h, None, mid, scales, deferred)
+        self._zero_convs(R, h, None, mid, scales)
         return h
 
-    def _zero_convs(self, R, h, i, slot, scales, deferred):
-        """slot += scale * zero_conv_i(h) for every ControlNet of R (i = None: middle_block_out), or the same GEMMs
-        appended to `deferred` as (a, w, out, kwargs).  A net whose scale asks for the conditional rows only
-        (DenoiseEngine.prepare(controlnet_rows="conditional")) adds its residual to rows [B/2, B) of the slot and
-        leaves the unconditional rows untouched: cat([zeros_like(d), d]) (utils/stable_diffusion_controlnet.py:
-        579-602)."""
+    def _zero_convs(self, R, h, i, slot, scales):
+        """slot += scale * zero_conv_i(h) for every ControlNet of R (i = None: middle_block_out).  A net whose scale
+        asks for the conditional rows only (DenoiseEngine.prepare(controlnet_rows="conditional")) adds its residual to
+        rows [B/2, B) of the slot and leaves the unconditional rows untouched: cat([zeros_like(d), d])
+        (utils/stable_diffusion_controlnet.py:579-602)."""
         c = h.shape[-1]
         p = "mid_out" if i is None else f"zero_convs.{i}.0"
         for g, nt in enumerate(R.nets):
@@ -516,12 +503,8 @@ class UNetRunner:
             if self.conditional_rows(scales[g]):
                 a, out = self.conditional_half(a), self.conditional_half(slot)
             M = a.shape[0] * a.shape[1] * a.shape[2]
-            call = (a.reshape(M, c), nt.w[p + ".w"], out,
-                    dict(M=M, bias=nt.w[p + ".b"], out_scale=f, row_scale=rs, accumulate=True, ldo=slot.stride(2)))
-            if deferred is not None:
-                deferred.append(call)
-            else:
-                R.ops.gemm(*call[:3], **call[3])
+            R.ops.gemm(a.reshape(M, c), nt.w[p + ".w"], out, M=M, bias=nt.w[p + ".b"], out_scale=f, row_scale=rs,
+                       accumulate=True, ldo=slot.stride(2))
 
     @staticmethod
     def zc_scale(scale, i, shape):
@@ -554,23 +537,29 @@ class UNetRunner:
                              f"{v.data_ptr() - t.data_ptr()}, which is not a multiple of 16")
         return v
 
-    def precompute_context_lockstep(self, ctx):
-        """Cross-attention K/V of the encoder + middle attention layers of every network, stacked along the batch
-        like the lockstep activations: kv[p] = [n * B * L, 2 * inner] (network g = rows [g*B*L, (g+1)*B*L))."""
-        nets = [self.unet] + self.cns
-        n = len(nets)
+    def precompute_context_groups(self, ctx):
+        """Cross-attention K/V of the encoder + middle attention layers, one entry per group of self.groups, stacked
+        along the batch like the group's activations: kv[p] = [n * B * L, 2 * inner] (network g of the group = rows
+        [g*B*L, (g+1)*B*L)).  The UNet alone (no ControlNets) reads its own per-layer cache instead: entry None."""
+        if not self.cns:
+            return [None]
         B, Lc, D = ctx.shape
         ctx2 = ctx.to(self.hdt).reshape(B * Lc, D).contiguous()
         topo = self.unet.topo
-        kv = {}
-        for layers in list(topo.input_blocks) + [topo.middle]:
-            for b in layers:
-                if b.kind == "attn":
-                    p = b.prefix
-                    out = torch.empty(n * B * Lc, self.unet.w[p + ".kv2.w"].shape[0], device=self.dev, dtype=self.hdt)
-                    self.ops.gemm_grouped([(ctx2, nt.w[p + ".kv2.w"], out.chunk(n, 0)[g], {}) for g, nt in enumerate(nets)])
-                    kv[p] = out
-        return {"kv": kv, "B": n * B, "L": Lc}
+        out = []
+        for R in self.groups:
+            n = R.n
+            kv = {}
+            for layers in list(topo.input_blocks) + [topo.middle]:
+                for b in layers:
+                    if b.kind == "attn":
+                        p = b.prefix
+                        t = torch.empty(n * B * Lc, self.unet.w[p + ".kv2.w"].shape[0], device=self.dev, dtype=self.hdt)
+                        self.ops.gemm_grouped([(ctx2, nt.w[p + ".kv2.w"], t.chunk(n, 0)[g], {})
+                                               for g, nt in enumerate(R.nets)])
+                        kv[p] = t
+            out.append({"kv": kv, "B": n * B, "L": Lc})
+        return out
 
     def alloc_sinks(self, B, H, W_):
         """Skip-concat buffers of the decoder: cat_i = [h (C1) | skip_i + control_i (C2)]."""
@@ -601,10 +590,11 @@ class UNetRunner:
         per timestep instead of re-streaming ~93 MB of embedding weights every step."""
         return [n._emb(t_dev, B) for n in [self.unet] + self.cns]
 
-    def eps_features(self, x_half, t_dev, ctx_cache, hints, scales, gn_ws=None, embs=None, ctx_ls=None, cond_in=None):
+    def eps_features(self, x_half, t_dev, ctx_cache, ctx_groups, hints, scales, gn_ws=None, embs=None, cond_in=None):
         """Runs UNet encoder, ControlNets, UNet decoder; returns the GroupNorm+SiLU'd input of the
-        final convolution [B,H,W,mc] (the out conv itself is fused with CFG/DDIM).  x_half holds the 4 latent
-        channels; a 9-channel UNet also needs cond_in [B,H,W,mc] (PackedNet.precompute_condition)."""
+        final convolution [B,H,W,mc] (the out conv itself is fused with CFG/DDIM).  ctx_cache[0]: the UNet's
+        PackedNet.precompute_context; ctx_groups: precompute_context_groups.  x_half holds the 4 latent channels; a
+        9-channel UNet also needs cond_in [B,H,W,mc] (PackedNet.precompute_condition)."""
         un = self.unet
         o = self.ops
         B, H, W_, _ = x_half.shape
@@ -626,42 +616,16 @@ class UNetRunner:
                                      "activation do not start at a 16-byte boundary")
         if embs is None:
             embs = self.compute_embs(t_dev, B)
-        n = 1 + len(self.cns)
         hints, scales = [None] + list(hints), [None] + list(scales)     # one per network, UNet first
-        if self.lockstep and ctx_ls is not None:
-            o.set_lane(0, False)
-            self._encoder(self.group, x_half, embs, ctx_ls, self._workspaces(n * B, 1)[0], sinks, hints, scales,
-                          cond_in)
-        elif self.concurrent and n > 1 and x_half.is_cuda:
-            # The UNet encoder and every ControlNet only READ x and write their own activations: run
-            # them on parallel streams (many of their launches cannot fill 132 SMs on their own), join,
-            # then apply the zero-conv accumulations into the shared skip slots on the main stream.
-            # Inside the concurrent region GroupNorm / split-K use their variants without inter-CTA
-            # waits, and each stream has its own scratch lane.
-            main = torch.cuda.current_stream()
-            if len(self._streams) < len(self.cns):
-                self._streams = [torch.cuda.Stream() for _ in self.cns]
-            lanes_ws = self._workspaces(B, n)
-            deferred = []
-            for s in self._streams:
-                s.wait_stream(main)
-            o.set_lane(0, True)
-            self._encoder(self.solo[0], x_half, embs[:1], ctx_cache[0], lanes_ws[0], sinks, hints[:1], scales[:1],
-                          cond_in)
-            for g in range(1, n):
-                with torch.cuda.stream(self._streams[g - 1]):
-                    o.set_lane(g, True)
-                    self._encoder(self.solo[g], x_half, embs[g:g + 1], ctx_cache[g], lanes_ws[g], sinks,
-                                  hints[g:g + 1], scales[g:g + 1], deferred=deferred)
-            for s in self._streams:
-                main.wait_stream(s)
-            o.set_lane(0, False)
-            for a_, w_, out_, kw_ in deferred:
-                o.gemm(a_, w_, out_, **kw_)
-        else:
-            for g, R in enumerate(self.solo):
-                self._encoder(R, x_half, embs[g:g + 1], ctx_cache[g], gn_ws, sinks, hints[g:g + 1], scales[g:g + 1],
-                              cond_in)
+        g0 = 0
+        for R, ctxc in zip(self.groups, ctx_groups, strict=True):
+            if ctxc is None:        # the UNet alone: its own K/V cache and the caller's workspace
+                ctxc, ws = ctx_cache[0], gn_ws
+            else:
+                ws = self._gn_workspace(R.n * B)
+            g1 = g0 + R.n
+            self._encoder(R, x_half, embs[g0:g1], ctxc, ws, sinks, hints[g0:g1], scales[g0:g1], cond_in)
+            g0 = g1
         topo = un.topo
         cats = sinks["cats"]
         h = None
@@ -672,7 +636,7 @@ class UNetRunner:
                 dst = nxt[..., :n1]
             else:
                 dst = None
-            h = self.solo[0]._run_layers(layers, cat, embs[:1], ctx_cache[0], gn_ws, final_out=dst)
+            h = self.decoder._run_layers(layers, cat, embs[:1], ctx_cache[0], gn_ws, final_out=dst)
         mc = un.cfg.model_channels
         xn = un._new(B, H, W_, mc)
         o.groupnorm(h, un.w["out.g"], un.w["out.b"], xn, B=B, HW=H * W_, C_=mc, eps=1e-5, silu=True,

@@ -34,22 +34,12 @@ def reset_launch_count():
 
 _GEMM_WS = {}
 GEMM_WS_BYTES = 65536 + 48 * 1024 * 1024
-_LANE = [0]          # workspace lane: kernels on concurrently running streams must not share scratch
-_CONCURRENT = [False]
-
-
-def set_lane(lane, concurrent):
-    """Select the scratch lane of the calling stream and whether other streams run concurrently
-    (then GroupNorm and split-K GEMMs use their variants without inter-CTA waits)."""
-    _LANE[0] = lane
-    _CONCURRENT[0] = bool(concurrent)
 
 
 def gemm_workspace(device):
-    """Per-device (and per concurrent lane) split-K scratch of ea_gemm (64 KB zeroed counters + fp32
-    partial tiles); shared by every GEMM on a stream, allocated once so CUDA-graph captures see a
-    stable address."""
-    key = (device.type, device.index, _LANE[0])
+    """Per-device split-K scratch of ea_gemm (64 KB zeroed counters + fp32 partial tiles); shared by every GEMM,
+    allocated once so CUDA-graph captures see a stable address."""
+    key = (device.type, device.index)
     ws = _GEMM_WS.get(key)
     if ws is None:
         ws = torch.zeros(GEMM_WS_BYTES, device=device, dtype=torch.uint8)
@@ -109,7 +99,6 @@ def _fill_gemm(g, a, w, out=None, *, mode=L.EA_GEMM_LINEAR, M=None, N=None, K=No
     g.force_splits = force_splits
     g.force_2cta = force_2cta
     g.force_persistent = force_persistent
-    g.no_spin = 1 if _CONCURRENT[0] else 0
     if row_scale is not None:
         g.row_scale = row_scale.data_ptr()
     if rowstats_out is not None:
@@ -242,7 +231,6 @@ def groupnorm(x, gamma, beta, out, *, B, HW, C_, groups=32, eps=1e-5, silu=True,
     g.ldo = ldo if ldo is not None else C_
     g.B, g.HW, g.C, g.groups = B, HW, C_, groups
     g.eps, g.silu = eps, 1 if silu else 0
-    g.two_pass = 1 if _CONCURRENT[0] else 0
     if workspace is None:
         workspace = gn_workspace(B, x.device, groups)
     g.workspace = workspace.data_ptr()

@@ -77,7 +77,8 @@ void ea_reset_launch_count(void);
  * Split-K: when the output has fewer tiles than the GPU has SMs, K is split across CTAs; each
  *            split CTA publishes its fp32 partial tile to `workspace`, waits for its siblings
  *            (all resident by construction) and finishes a 1/splits share of the tile with the
- *            full fused epilogue — deterministic summation order, no extra launch.
+ *            full fused epilogue — deterministic summation order, no extra launch.  A split grid larger than
+ *            the GPU's SMs (forced test configurations) is EA_ERR_SHAPE, before any launch.
  * Constraints: N % 8 == 0, K % 8 == 0, Cin % 64 == 0, all leading dims % 8 == 0,
  *              pointers 16-byte aligned.  Leading dims cover a whole row: LINEAR lda >= K; CONV lda (if set)
  *              >= Cin and ld_extra (if set) >= Cin_extra; ldw (if set) >= total K; ldo, ldo2 and ldr >= the
@@ -113,8 +114,6 @@ typedef struct ea_gemm_args {
   int force_splits;          /* 0 = auto; 1 = never split K; n = split K n ways (testing) */
   int force_2cta;            /* row tiles per CTA: 1 = two vertically adjacent 128-row tiles sharing each W stage,
                                 -1 = one, 0 = the planner's choice (testing) */
-  int no_spin;               /* 1: split-K without the sibling wait - the last split CTA to arrive reduces
-                                the whole tile (required when other streams run kernels concurrently) */
   int force_persistent;      /* > 0: one CTA per SM walks the tile list (no split-K); 0 / -1 = one tile per CTA */
   /* LayerNorm folded into the GEMMs around it (BasicTransformerBlock norm1/2/3, ldm/modules/attention.py:
    * 263-275): LN(x) W^T = rstd[m] * (x (W*gamma)^T - mean[m] * g) + (W beta + b), g[n] = sum_k (W*gamma)[n,k].
@@ -185,6 +184,8 @@ int ea_attention(const ea_attn_args* args, void* stream);
  *   Normalize (eps 1e-6)  attention.py:88-89.
  *   x may be a channel-concatenation of two tensors x[.., 0:C1] ++ x2[.., 0:C-C1]
  *   (skip-concat, cldm/cldm.py:39-41); pass x2 = NULL for a single source.
+ *   One launch: the CTAs of an image publish partial sums and wait for each other (all resident: B <= SMs, at most
+ *   SMs / B CTAs per image) before normalising.
  * ea_layernorm: nn.LayerNorm over the last dim of [M, C]  (attention.py:263-265).
  */
 #define EA_GN_WS_FLOATS(B, groups) (2 * (B) + 2 * (groups) * 256)
@@ -195,8 +196,6 @@ typedef struct ea_gn_args {
   void* out; long long ldo;
   int B, HW, C, groups;
   float eps; int silu;
-  int two_pass;              /* 1: statistics and normalisation as two launches with no inter-CTA wait
-                                (required when other streams run kernels concurrently) */
   float* workspace;          /* >= 2*B + 2*groups*256 floats (EA_GN_WS_FLOATS), ZERO before the first call (the
                                 kernel leaves its counters zero); one workspace may serve every call on a stream.
                                 Layout: [B][2] int arrival counters, then one slot of 2*groups partial sums per

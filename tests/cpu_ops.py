@@ -17,10 +17,6 @@ def half_dtype():
     return torch.float32
 
 
-def set_lane(lane, concurrent):
-    pass
-
-
 def launch_count():
     return _count
 

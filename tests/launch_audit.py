@@ -49,7 +49,7 @@ ACT = {0: "none", 1: "silu", 2: "gelu", 3: "geglu"}
 GEMM_WS_COUNTER_BYTES = 65536
 CHUNK_ELEMS = 1 << 24       # float64 references are built at most this many outputs at a time (at least one row)
 # operator-table entries that launch nothing
-PASSTHROUGH = {"half_dtype", "set_lane", "launch_count", "reset_launch_count", "gn_workspace", "gemm_workspace",
+PASSTHROUGH = {"half_dtype", "launch_count", "reset_launch_count", "gn_workspace", "gemm_workspace",
                "weight_lookahead", "WeightLookahead", "check_out_buffers", "check_prediction"}
 
 
@@ -1096,7 +1096,7 @@ def denoise_engine(name, backend, device):
     usd = make_state_dict(cfg, "unet", 61)
     csds = [make_state_dict(TINY21 if cfg is TINY21_INPAINT else cfg, "controlnet", 62 + i) for i in range(n_cn)]
     x, ctx, hints = make_inputs(cfg, 2, 8, 7, 5, n_controlnets=2)
-    hints = (hints + [hints[0].flip(-1)])[:n_cn]
+    hints = (hints + [hints[0].flip(-1), hints[1].flip(-2)])[:n_cn]
     scales = [torch.rand(8, 8, generator=torch.Generator().manual_seed(9)) if s == "map" else s for s in scales]
     eng = DenoiseEngine(cfg, usd, csds, device, backend=backend)
     return eng, x, ctx, hints, scales, guess

@@ -49,7 +49,7 @@ def test_modes_operands_and_layouts():
     assert any(c.get("pad") and c.get("silu") for c in cs), "zero-padded channels through SiLU"
     assert any(c.get("f32") for c in cs) and any(c.get("slots") for c in cs)
     assert any(c.get("rowvec") for c in cs) and any(c.get("residual") for c in cs)
-    # the 2-row-tile layout with an odd number of row tiles (the last CTA's second tile is empty), split-K both ways
+    # the 2-row-tile layout with an odd number of row tiles (the last CTA's second tile is empty), split-K
     assert any(row_tiles(c) % 2 and "pair" in _layouts(c) for c in cs)
-    assert any(row_tiles(c) > 1 and "split_no_spin" in _layouts(c) for c in cs)
+    assert any(row_tiles(c) > 1 and "split" in _layouts(c) for c in cs)
     assert {conv_geometry(CASES[n]["H"], CASES[n]["W"])[2] for n in GROUPED} >= {2, 8}

@@ -101,11 +101,11 @@ def _bn_for(n):
 
 
 def _layouts(c):
-    """one: one row tile per CTA; pair: two per CTA, bit for bit equal to one; bnXX: forced tile width; split /
-    split_no_spin: K split 3 ways with and without the sibling wait (every CTA resident)."""
+    """one: one row tile per CTA; pair: two per CTA, bit for bit equal to one; bnXX: forced tile width; split: K split
+    3 ways (every CTA resident)."""
     out = ["auto", "pair", "bn32", "bn64", "bn128"]
     if row_tiles(c) * -(-c["cout"] // 128) * 3 <= 132:
-        out += ["split", "split_no_spin"]
+        out += ["split"]
     return out
 
 
@@ -249,17 +249,6 @@ def _case(name):
     return _BUILT[name]
 
 
-class _concurrent_lane:
-    """no_spin split-K, as used under concurrent streams; the default lane is always restored."""
-
-    def __enter__(self):
-        ops.set_lane(1, True)
-
-    def __exit__(self, *exc):
-        ops.set_lane(0, False)
-        return False
-
-
 def _layout_kw(c, layout):
     bn = _bn_for(c["cout"])
     return {"auto": {}, "one": dict(force_2cta=-1, force_splits=1, force_bn=bn),
@@ -267,8 +256,7 @@ def _layout_kw(c, layout):
             "bn32": dict(force_2cta=-1, force_splits=1, force_bn=32),
             "bn64": dict(force_2cta=-1, force_splits=1, force_bn=64),
             "bn128": dict(force_2cta=-1, force_splits=1, force_bn=128),
-            "split": dict(force_2cta=-1, force_splits=3, force_bn=128),
-            "split_no_spin": dict(force_2cta=-1, force_splits=3, force_bn=128)}[layout]
+            "split": dict(force_2cta=-1, force_splits=3, force_bn=128)}[layout]
 
 
 def _run(cs, layout):
@@ -276,12 +264,7 @@ def _run(cs, layout):
     out, out2, o32, bufs = cs.dests()
     saved = [b.clone() for b, _ in bufs]
     kw = dict(cs.kwargs(), **_layout_kw(cs.c, layout))
-    call = lambda: ops.gemm(cs.x, cs.w, out, out2=out2, out_f32=o32, accumulate=o32 is not None, **kw)
-    if layout == "split_no_spin":
-        with _concurrent_lane():
-            call()
-    else:
-        call()
+    ops.gemm(cs.x, cs.w, out, out2=out2, out_f32=o32, accumulate=o32 is not None, **kw)
     torch.cuda.synchronize()
     cout, M = cs.c["cout"], cs.M
     for (b, c0), s in zip(bufs, saved):   # all but the destination slot keeps its sentinel, guard rows included

@@ -130,7 +130,7 @@ def test_sd15_tile_step_256x344(monkeypatch):
     def body(aud):
         eng = DenoiseEngine(SD15, make_state_dict(SD15, "unet", 201), [make_state_dict(SD15, "controlnet", 202)], DEV,
                             backend=aud)
-        assert eng.runner.lockstep
+        assert [R.n for R in eng.runner.groups] == [2]
         eng.prepare(ctx, [torch.cat([hint, hint])], [1.0], cfg_duplicated=True)
         return eng, run(eng, False)
     aud, (eng, audited) = _audited("sd15_tile_step_256x344", body)

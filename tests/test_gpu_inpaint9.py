@@ -29,7 +29,7 @@ def _check_golden(name, cfg):
     m = g["meta"]
     eng = DenoiseEngine(cfg, make_state_dict(cfg, "unet", m["unet_seed"]),
                         [make_state_dict(controlnet_config(cfg), "controlnet", s) for s in m["cn_seeds"]], DEV)
-    assert eng.runner.lockstep
+    assert [R.n for R in eng.runner.groups] == [2]           # the UNet encoder and the ControlNet in lockstep
     torch.cuda.empty_cache()
     x, ctx, hints = make_inputs(cfg, m["B"], m["lat"], m["L"], m["in_seed"], n_controlnets=len(m["cn_seeds"]))
     eng.prepare(ctx, hints, m["scales"])

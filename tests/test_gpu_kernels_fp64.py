@@ -90,18 +90,6 @@ def _untouched(kernel, what, region, sentinel):
         raise AssertionError(f"{kernel} {what}: wrote outside its destination")
 
 
-class _concurrent_lane:
-    """The kernel variants without inter-CTA waits (two-pass GroupNorm, no_spin split-K), as used under concurrent
-    streams; the default lane is always restored."""
-
-    def __enter__(self):
-        ops.set_lane(1, True)
-
-    def __exit__(self, *exc):
-        ops.set_lane(0, False)
-        return False
-
-
 # ================================================ GroupNorm ====================================================
 GN_CASES = {
     # UNet levels (SD1.5 512^2, image + CFG)
@@ -150,7 +138,7 @@ def _gn_inputs(B, HW, C, C1=None, xpad=0, opad=0, n_nets=1, offset=0.0, std=1.0,
     return vals, srcs, gam, bet, out
 
 
-def _gn_run(case, two_pass, silu=None, eps=None):
+def _gn_run(case, silu=None, eps=None):
     c = dict(case)
     B, HW, C = c["B"], c["HW"], c["C"]
     silu = c.get("silu", True) if silu is None else silu
@@ -163,11 +151,7 @@ def _gn_run(case, two_pass, silu=None, eps=None):
     g_arg, b_arg = (gam, bet) if n_nets > 1 else (gam[0], bet[0])
     outs = []
     for _ in range(2):
-        if two_pass:
-            with _concurrent_lane():
-                ops.groupnorm(x, g_arg, b_arg, out, **kw)
-        else:
-            ops.groupnorm(x, g_arg, b_arg, out, **kw)
+        ops.groupnorm(x, g_arg, b_arg, out, **kw)
         torch.cuda.synchronize()
         assert not ws[:2 * B].view(torch.int32).any(), "workspace counters not left zero"
         outs.append(out.clone())
@@ -190,7 +174,7 @@ def _gn_run(case, two_pass, silu=None, eps=None):
     unit = (R.ulp(y, _half()) + 1.1 * e_aff + R.silu_eval_err(pre)) if silu else R.ulp(y, _half()) + e_aff
     # these shapes also hold the bound without the derived statistics term (the one they had before it): their
     # statistics' rounding stays far below its worst case
-    _close("ea_groupnorm (unit only)", f"{'two_pass' if two_pass else 'fused'}", out[..., :C], y, unit)
+    _close("ea_groupnorm (unit only)", "fused", out[..., :C], y, unit)
     del unit
     e_aff = e_aff + excess
     del excess
@@ -199,13 +183,12 @@ def _gn_run(case, two_pass, silu=None, eps=None):
     else:
         bound = R.ulp(y, _half()) + e_aff
     del pre
-    return _close("ea_groupnorm", f"{'two_pass' if two_pass else 'fused'}", out[..., :C], y, bound)
+    return _close("ea_groupnorm", "fused", out[..., :C], y, bound)
 
 
-@pytest.mark.parametrize("two_pass", [False, True], ids=["fused", "two_pass"])
 @pytest.mark.parametrize("name", list(GN_CASES))
-def test_groupnorm(name, two_pass):
-    _gn_run(GN_CASES[name], two_pass)
+def test_groupnorm(name):
+    _gn_run(GN_CASES[name])
 
 
 @pytest.mark.parametrize("C", [128, 256])
@@ -228,11 +211,10 @@ def test_groupnorm_tile_2048x2752(C):
     del x
 
 
-@pytest.mark.parametrize("two_pass", [False, True], ids=["fused", "two_pass"])
 @pytest.mark.parametrize("eps", [1e-5, 1e-6])
 @pytest.mark.parametrize("silu", [True, False])
-def test_groupnorm_flags(silu, eps, two_pass):
-    _gn_run(dict(B=2, HW=32 * 32, C=640, xpad=8, opad=8), two_pass, silu=silu, eps=eps)
+def test_groupnorm_flags(silu, eps):
+    _gn_run(dict(B=2, HW=32 * 32, C=640, xpad=8, opad=8), silu=silu, eps=eps)
 
 
 # ================================================ LayerNorm ====================================================
@@ -586,7 +568,7 @@ def test_step_gather_exact():
 
 
 # ================================================ GEMM epilogue inputs =========================================
-@pytest.mark.parametrize("variant", ["default", "splits1", "no_spin"])
+@pytest.mark.parametrize("variant", ["default", "splits1"])
 @pytest.mark.parametrize("MNK", [(128, 1280, 1280), (8192, 320, 320)], ids=["zero_conv_8x8", "zero_conv_64x64"])
 def test_gemm_row_scale(MNK, variant):
     """ControlNet zero-conv with a spatial conditioning-scale map: slot += 0.7 * rs[m] * (A W^T + b), in a slot of
@@ -604,11 +586,7 @@ def test_gemm_row_scale(MNK, variant):
     kw = dict(M=M, bias=bias, out_scale=0.7, row_scale=rs, accumulate=True, ldo=2 * N)
     if variant == "splits1":
         kw["force_splits"] = 1
-    if variant == "no_spin":
-        with _concurrent_lane():
-            ops.gemm(a, w, buf[:, N:], **kw)
-    else:
-        ops.gemm(a, w, buf[:, N:], **kw)
+    ops.gemm(a, w, buf[:, N:], **kw)
     _untouched("ea_gemm row_scale", "left half of the slot", buf[:, :N], left)
     ref, t, mag = R.gemm_epilogue(a.double(), w.double(), bias.double(), 0.7, rs.double(), old)
     bound = R.ulp(ref, h) + (K + 1) * U * mag + 3 * U * (t.abs() + old.abs())
@@ -649,13 +627,12 @@ def _act_check(kernel, what, got, act, pre, e, scale=1.0, res=None, old=None):
 
 
 # epilogue paths: the default (fast) one; the general one (a time-embedding row vector whose images change inside a
-# tile); forced split-K with the sibling wait and without it (no_spin); the persistent grid; two row tiles per CTA;
-# an fp32 destination accumulated into
-ACT_PATHS = ["default", "general", "split_k", "split_k_no_spin", "persistent", "row_pair", "f32_accumulate"]
+# tile); forced split-K; the persistent grid; two row tiles per CTA; an fp32 destination accumulated into
+ACT_PATHS = ["default", "general", "split_k", "persistent", "row_pair", "f32_accumulate"]
 # GEGLU has neither a row vector nor an fp32 destination; split-K only where every split CTA is resident (M = 300)
 ACT_CASES = [(act, M, K, path) for act in ACTS for path in ACT_PATHS for M in (300, 8192) for K in (320, 200)
              if not (act == "geglu" and path in ("general", "f32_accumulate"))
-             and not (path.startswith("split_k") and M > 300) and not (path == "f32_accumulate" and K != 320)]
+             and not (path == "split_k" and M > 300) and not (path == "f32_accumulate" and K != 320)]
 
 
 @pytest.mark.parametrize("act,M,K,path", ACT_CASES, ids=[f"{a}-M{m}-K{k}-{p}" for a, m, k, p in ACT_CASES])
@@ -673,7 +650,7 @@ def test_gemm_activation(act, M, K, path):
     if path == "general":
         rv = _randn(((M + 49) // 50, N), 114, scale=2.0)
         kw.update(rowvec=rv, rows_per_batch=50)            # a 128-row tile spans three images
-    elif path.startswith("split_k"):
+    elif path == "split_k":
         kw.update(force_splits=4, force_bn=128)            # 30 tiles x <= 4 splits: every CTA resident
     elif path == "persistent":
         kw["force_persistent"] = 2
@@ -689,15 +666,10 @@ def test_gemm_activation(act, M, K, path):
     if path == "f32_accumulate":
         old = _randn((M, n_out), 116)
         out = old.clone()
-        call = lambda: ops.gemm(a, w, out_f32=out, accumulate=True, **kw)
+        ops.gemm(a, w, out_f32=out, accumulate=True, **kw)
     else:
         out = torch.full((M, n_out), 7.0, device=DEV, dtype=h)
-        call = lambda: ops.gemm(a, w, out, **kw)
-    if path == "split_k_no_spin":
-        with _concurrent_lane():
-            call()
-    else:
-        call()
+        ops.gemm(a, w, out, **kw)
     torch.cuda.synchronize()
     pre, _, mag = R.gemm_epilogue(a.double(), w.double(), bias.double())
     if rv is not None:

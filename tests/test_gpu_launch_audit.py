@@ -71,8 +71,7 @@ def _audited(case, body):
 @pytest.mark.parametrize("name", list(CASES))
 def test_denoise_step_trace_cases(name, monkeypatch):
     """prepare (hint stack, context K/V, embeddings), three UniPC steps (the multistep history live) and one eps() of
-    every step-trace case; the cases without lockstep run their ControlNets on concurrent streams (no_spin split-K,
-    two-pass GroupNorm)."""
+    every step-trace case; with three or four ControlNets the encoder runs as two groups of grouped launches."""
     _set_env(monkeypatch, name)
 
     def body(aud):

@@ -99,27 +99,25 @@ def test_eps_vs_cpu_oracle_fresh_inputs():
         assert (eng.eps(x, t).cpu() - ref).abs().max().item() < EPS_TOL
 
 
-@pytest.mark.parametrize("concurrent", ["1", "0"])
-def test_three_controlnets_vs_cpu_oracle(concurrent, monkeypatch):
-    """Three ControlNets are more networks than one grouped launch takes, so the encoder runs network by network: on
-    one CUDA stream each with the zero-convs applied after the streams join (EA_CONCURRENT=1, the default), or one
-    after another on the current stream (EA_CONCURRENT=0)."""
-    monkeypatch.setenv("EA_CONCURRENT", concurrent)
+@pytest.mark.parametrize("n_cn,sizes", [(3, [3, 1]), (4, [3, 2])], ids=["cn3", "cn4"])
+def test_controlnet_groups_vs_cpu_oracle(n_cn, sizes):
+    """Three or four ControlNets are more networks than one grouped launch takes, so the encoder runs as two groups,
+    one after the other: the UNet with the first two ControlNets, then the rest."""
     cfg = TINY
     usd = make_state_dict(cfg, "unet", 71)
-    csds = [make_state_dict(cfg, "controlnet", 72 + i) for i in range(3)]
+    csds = [make_state_dict(cfg, "controlnet", 72 + i) for i in range(n_cn)]
     x, ctx, hints = make_inputs(cfg, 2, 16, 13, 8)
-    hints = hints + [hints[0].flip(-1)]
-    scales = [0.5, 1.0, 0.7]
+    hints = (hints + [hints[0].flip(-1), hints[1].flip(-2)])[:n_cn]
+    scales = [0.5, 1.0, 0.7, 0.9][:n_cn]
     eng = DenoiseEngine(cfg, usd, csds, torch.device("cuda:0"))
-    assert not eng.runner.lockstep and eng.runner.concurrent == (concurrent == "1")
+    assert [R.n for R in eng.runner.groups] == sizes
     eng.prepare(ctx, hints, scales)
     ut, ct = build_topology(cfg), build_topology(cfg, with_decoder=False)
     for t in (981, 501, 1):
         with torch.no_grad():
             ref = O.apply_model(usd, ut, [(sd, ct) for sd in csds], x, torch.full((2,), t), ctx, hints, scales)
         err = (eng.eps(x, t).cpu() - ref).abs().max().item()
-        assert err < EPS_TOL, (concurrent, t, err)
+        assert err < EPS_TOL, (n_cn, t, err)
 
 
 @pytest.mark.parametrize("use_graph", [False, True])

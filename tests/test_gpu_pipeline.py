@@ -107,7 +107,7 @@ def test_pipeline_call_on_cuda_matches_reference_loop(alignment_ratio):
     lat2 = pipe(generator=torch.manual_seed(7), output_type="latent", **kw).images
     assert pipe.engine._graph is g0
     # bit-reproducible: GroupNorm statistics are per-CTA partials summed in a fixed order (no floating-point
-    # atomics), split-K partial tiles are reduced in split order, the lockstep step runs on one stream
+    # atomics), split-K partial tiles are reduced in split order, the step runs on one stream
     assert torch.equal(lat2, lat), (lat2 - lat).abs().max().item()
 
 

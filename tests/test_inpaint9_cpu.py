@@ -36,7 +36,7 @@ def _golden_engine(n_cn=None):
 
 def test_eps_matches_reference_golden_and_keeps_lockstep():
     g, m, eng, x, ctx, hints, _, _ = _golden_engine()
-    assert x.shape[1] == 9 and eng.runner.lockstep
+    assert x.shape[1] == 9 and [R.n for R in eng.runner.groups] == [2]
     eng.prepare(ctx, hints, m["scales"])
     for t in m["timesteps"]:
         eps = eng.eps(x, t)
@@ -50,7 +50,7 @@ def test_eps_matches_reference_golden_and_keeps_lockstep():
 
 def test_two_controlnets_lockstep_matches_oracle():
     _, m, eng, x, ctx, hints, usd, csds = _golden_engine(n_cn=2)
-    assert eng.runner.lockstep and len(eng.cns) == 2
+    assert [R.n for R in eng.runner.groups] == [3]
     eng.prepare(ctx, hints, [0.5, 1.0])
     with torch.no_grad():
         ref = apply_model_9ch(usd, TINY21_INPAINT, csds, x, 601, ctx, hints, [0.5, 1.0])

@@ -366,8 +366,7 @@ def _trace(usd):
 
 
 def test_merged_engine_issues_the_base_engines_operator_calls(tmp_path, monkeypatch):
-    for k in ("EA_LOCKSTEP", "EA_LN_FOLD", "EA_CONCURRENT", "EA_HINT_TC"):
-        monkeypatch.delenv(k, raising=False)
+    monkeypatch.delenv("EA_HINT_TC", raising=False)
     te = _write_base(str(tmp_path / "base"))
     path = _lora_file(str(tmp_path / "l.safetensors"), TINY, te)
     base_lines, base_eng = _trace(W.diffusers_to_ldm(SL.unet_diffusers_state_dict(TINY), "unet", TINY))

@@ -23,16 +23,15 @@ from oracle.inputs import make_inputs
 from tests import cpu_ops
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "step_trace.json")
-ENV = ("EA_LOCKSTEP", "EA_LN_FOLD", "EA_CONCURRENT", "EA_HINT_TC")
+ENV = ("EA_HINT_TC",)
 
 # name: (config, ControlNets, environment, conditioning scales, guess mode)
 CASES = {
     "tiny_cn0": (TINY, 0, {}, [], False),
     "tiny_cn1": (TINY, 1, {}, [0.8], False),
     "tiny_cn2": (TINY, 2, {}, [0.5, 1.0], False),
-    "tiny_cn3_sequential": (TINY, 3, {}, [0.5, 1.0, 0.7], False),
-    "tiny_cn2_no_lockstep": (TINY, 2, {"EA_LOCKSTEP": "0"}, [0.5, 1.0], False),
-    "tiny_cn2_no_ln_fold": (TINY, 2, {"EA_LN_FOLD": "0"}, [0.5, 1.0], False),
+    "tiny_cn3": (TINY, 3, {}, [0.5, 1.0, 0.7], False),
+    "tiny_cn4": (TINY, 4, {}, [0.5, 1.0, 0.7, 0.9], False),
     "tiny21_inpaint_cn1": (TINY21_INPAINT, 1, {}, [0.9], False),
     "tiny_cn2_guess_mode": (TINY, 2, {}, [0.7, 1.0], True),
     "tiny_cn2_scale_map": (TINY, 2, {}, ["map", 0.5], False),
@@ -100,7 +99,7 @@ def record(name, swap=False):
     usd = make_state_dict(cfg, "unet", 61)
     csds = [make_state_dict(TINY21 if cfg is TINY21_INPAINT else cfg, "controlnet", 62 + i) for i in range(n_cn)]
     x, ctx, hints = make_inputs(cfg, 2, 8, 7, 5, n_controlnets=2)
-    hints = (hints + [hints[0].flip(-1)])[:n_cn]
+    hints = (hints + [hints[0].flip(-1), hints[1].flip(-2)])[:n_cn]
     scales = [torch.rand(8, 8, generator=torch.Generator().manual_seed(9)) if s == "map" else s for s in scales]
     rec = Recorder()
     eng = DenoiseEngine(cfg, usd, csds, torch.device("cpu"), backend=cpu_ops if swap else rec)
@@ -160,7 +159,7 @@ def test_step_trace_matches_golden(name, monkeypatch, tmp_path):
     _check(name, record(name), tmp_path)
 
 
-@pytest.mark.parametrize("name", ["tiny_cn2", "tiny_cn3_sequential"])
+@pytest.mark.parametrize("name", ["tiny_cn2", "tiny_cn3", "tiny_cn4"])
 def test_operator_table_swapped_after_construction_sees_every_call(name, monkeypatch, tmp_path):
     _set_env(monkeypatch, name)
     _check(name, record(name, swap=True), tmp_path)

@@ -95,22 +95,6 @@ def case_gemm_splitk():
     return res
 
 
-def case_concurrent_variants():
-    """The no-inter-CTA-wait variants used when several streams run concurrently: two-pass GroupNorm
-    and split-K whose last-arriving CTA reduces the tile (ops.set_lane(lane, True))."""
-    from editanything_b200 import ops
-    ops.set_lane(1, True)
-    try:
-        a = case_groupnorm()
-        b = case_gemm_splitk()
-        c = case_conv_8_skip_splitk()
-        d = case_gemm_splitk_geglu()
-    finally:
-        ops.set_lane(0, False)
-    w = max(a["max_abs"], b["max_abs"], c["max_abs"] / max(1.0, c["ref_max"]), d["max_abs"])
-    return {"max_abs": w, "ref_max": 1.0, "gn": a["max_abs"], "splitk": b["max_abs"], "conv": c["max_abs"], "geglu": d["max_abs"]}
-
-
 def case_gemm_splitk_geglu():
     import torch
     from editanything_b200 import ops, _lib as L
